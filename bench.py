@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — set-ops/sec of the Roaring hot path on B200 (BASELINE.json metric).
+"""bench.py — set-ops/sec of the Roaring hot path on H100 (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            # our CUDA path (C ABI, sm_100a kernels)
+    python bench.py --gpus N --steps K --warmup W            # our CUDA path (C ABI, sm_90a kernels)
     python bench.py --impl reference --gpus N --steps K ...   # unmodified CRoaring on host cores
 
 Headline workload (config.workload = realdata_allpairs, SURVEY.md §8(d) config 2b): the
@@ -23,6 +23,11 @@ The same JSON line carries the other BASELINE.json configs as sub-records, each 
     or_many_sharded configs[4]: 1000 bitmaps over a 10^8 universe, key ranges over the run's N
                     GPUs + one ncclAllReduce(uint32[K]) per call, timed
 See DESIGN.md §6 for the contract and the definitions of every number.
+
+--dump-outputs DIR writes, after the timed steps, what the headline path returned in its last
+step (rank 0's results): per (dataset, op) the cardinality of every result bitmap and the values of
+a fixed, seeded sample of the non-empty result bitmaps, as float64 .npy files (64 MB at most in all).  The inputs
+are the committed fixtures, so two builds run with the same arguments can be compared file by file.
 """
 import argparse
 import ctypes as C
@@ -111,12 +116,87 @@ def peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
     except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+        return 3350.0, "fallback 3350 GB/s (H100 SXM data sheet HBM3 bandwidth)"
+
+
+# ------------------------------------------------------------------------------- --dump-outputs
+DUMP_SAMPLE = 8                      # result bitmaps per (dataset, op) whose values are written
+DUMP_BUDGET = 64 << 20               # bytes of .npy payload in all
+
+
+def portable_values(blob):
+    """Values of one bitmap in the portable serialization (the format of the reference's
+    roaring_bitmap_portable_serialize), as a sorted uint32 array."""
+    cookie = int.from_bytes(blob[:4], "little")
+    if cookie & 0xFFFF == 12347:                       # with run containers: run flags, no offsets below 4
+        n = (cookie >> 16) + 1
+        runs = np.unpackbits(np.frombuffer(blob, np.uint8, (n + 7) // 8, 4), bitorder="little")[:n]
+        pos = 4 + (n + 7) // 8
+        offsets = n >= 4
+    elif cookie == 12346:
+        n = int.from_bytes(blob[4:8], "little")
+        runs, pos, offsets = np.zeros(n, np.uint8), 8, True
+    else:
+        raise ValueError("not a portable roaring bitmap")
+    desc = np.frombuffer(blob, "<u2", 2 * n, pos).astype(np.uint32)
+    pos += 4 * n + (4 * n if offsets else 0)
+    out = []
+    for k in range(n):
+        hi, card = desc[2 * k] << 16, int(desc[2 * k + 1]) + 1
+        if runs[k]:
+            nr = int.from_bytes(blob[pos:pos + 2], "little")
+            rl = np.frombuffer(blob, "<u2", 2 * nr, pos + 2).astype(np.uint32)
+            pos += 2 + 4 * nr
+            lo = np.concatenate([np.arange(a, a + l + 1, dtype=np.uint32) for a, l in zip(rl[0::2], rl[1::2])])
+        elif card <= 4096:
+            lo = np.frombuffer(blob, "<u2", card, pos).astype(np.uint32)
+            pos += 2 * card
+        else:
+            bits = np.unpackbits(np.frombuffer(blob, np.uint8, 8192, pos), bitorder="little")
+            lo = np.flatnonzero(bits).astype(np.uint32)
+            pos += 8192
+        out.append(hi | lo)
+    return np.concatenate(out) if out else np.zeros(0, np.uint32)
+
+
+def dump_record(res):
+    """What a caller of the timed path receives from one batch call: every result's cardinality, and
+    the values of DUMP_SAMPLE non-empty result bitmaps drawn with a fixed seed (the same ones on every
+    run that computes the same cardinalities; empty results would sample nothing)."""
+    cards = res.cardinalities()
+    live = np.flatnonzero(cards)
+    pick = np.sort(np.random.default_rng(len(res)).choice(live, size=min(DUMP_SAMPLE, len(live)), replace=False))
+    vals = []
+    for i in pick:
+        bm = res.download(int(i))
+        vals.append(portable_values(bm.serialize()))
+        bm.free()
+    return cards, pick, vals
+
+
+def write_dump(out_dir, records):
+    """DIR/<dataset>_<op>_{cardinality,sample_pairs,sample_offsets,sample_values}.npy, float64 (exact
+    for 32-bit values and the cardinalities).  A sampled bitmap with more values than its even share
+    of the budget keeps that many of them, evenly spaced: the same ones on every run."""
+    os.makedirs(out_dir, exist_ok=True)
+    fixed = sum(8 * (len(c) + 2 * len(p) + 1) + 4 * 128 for c, p, _ in records)   # + .npy headers
+    cap = (DUMP_BUDGET - fixed) // (8 * len(records) * DUMP_SAMPLE)
+    for k, (cards, pick, vals) in enumerate(records):
+        if not len(pick):
+            raise RuntimeError("--dump-outputs: every result of a batch call is empty, nothing to sample")
+        vals = [v if len(v) <= cap else v[np.linspace(0, len(v) - 1, cap).astype(np.int64)] for v in vals]
+        name = f"{DATASETS[k // len(OPS)]}_{OPS[k % len(OPS)]}"
+        offs = np.concatenate([[0], np.cumsum([len(v) for v in vals])])
+        flat = np.concatenate(vals) if vals else np.zeros(0)
+        for suffix, arr in (("cardinality", cards), ("sample_pairs", pick),
+                            ("sample_offsets", offs), ("sample_values", flat)):
+            np.save(os.path.join(out_dir, f"{name}_{suffix}.npy"), np.asarray(arr, dtype=np.float64))
+    log(f"dump: {len(records)} results written to {out_dir}")
 
 
 # ------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -256,6 +336,8 @@ def main():
     ap.add_argument("--zipf-bitmaps", type=int, default=200)
     ap.add_argument("--sharded-bitmaps", type=int, default=1000)
     ap.add_argument("--card-pairs", type=int, default=10 ** 4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline path's last-step results to DIR/<name>.npy")
     args = ap.parse_args()
     capture_stdout()
 
@@ -325,7 +407,7 @@ def main():
     succ_full = {ds: successive_pairs(len(blobs[ds])) for ds in DATASETS}
     succ = {ds: (succ_full[ds][0][rank::world].copy(), succ_full[ds][1][rank::world].copy()) for ds in DATASETS}
     ops_per_step = sum(len(full_pairs[ds][0]) for ds in DATASETS) * len(OPS)
-    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     d_chk = torch.zeros(1, dtype=torch.int64, device="cuda")              # device-resident checksum (u64)
 
     stats = {"algo_bytes": 0, "kernel_ms": 0.0, "launches": 0, "checksum": 0, "device_ms": 0.0}
@@ -345,14 +427,14 @@ def main():
         comm.allreduce_u64(d_chk.data_ptr(), 1)
         return res
 
-    def timed(pairset, steps, warmup, collect):
+    def timed(pairset, steps, warmup, collect, last=None):
         for _ in range(warmup):
             for r in step(pairset):
                 r.free()
         barrier()
         tot_ms = 0.0
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        for _ in range(steps):
+        for it in range(steps):
             flush_buf.zero_()            # flush L2 between timed iterations (not timed)
             barrier()
             e0.record(stream)
@@ -360,6 +442,7 @@ def main():
             e1.record(stream)
             torch.cuda.synchronize()
             tot_ms += e0.elapsed_time(e1)
+            keep = last is not None and it == steps - 1      # the last step's results, for --dump-outputs
             for k, r in enumerate(res):
                 if collect:
                     ms, cms, ab = r.op_stats()
@@ -372,7 +455,10 @@ def main():
                     pl[0] += cms
                     pl[1] += ms
                     pl[2] += ab
-                r.free()
+                if not keep:
+                    r.free()
+            if keep:
+                last[:] = res
             if collect:
                 stats["checksum"] = int(d_chk.item())
         barrier()
@@ -382,9 +468,14 @@ def main():
     if rank == 0:
         sampler.start()
     l0 = rb.kernel_launches()
-    tot_ms = timed(pairs, args.steps, args.warmup, True)
+    last = [] if args.dump_outputs and rank == 0 else None
+    tot_ms = timed(pairs, args.steps, args.warmup, True, last)
     gpu_launches = rb.kernel_launches() - l0
     clocks = sampler.stop() if rank == 0 else None
+    if last is not None:
+        write_dump(args.dump_outputs, [dump_record(r) for r in last])
+        for r in last:
+            r.free()
     value = ops_per_step * args.steps / (tot_ms * 1e-3)
     gold = golden_allpairs()
     headline_parity = gold is not None and stats["checksum"] == gold["bench_checksum_and_or_xor"]
@@ -392,7 +483,7 @@ def main():
         f"parity={headline_parity}")
 
     # ---- the literal configs[1] sweep: 199 successive pairs (latency-bound, reported beside)
-    succ_steps = max(args.steps, 20)
+    succ_steps = args.steps
     succ_ops = sum(len(succ_full[ds][0]) for ds in DATASETS) * len(OPS)
     succ_ms = timed(succ, succ_steps, args.warmup, False)
     succ_val = succ_ops * succ_steps / (succ_ms * 1e-3)

@@ -1,4 +1,4 @@
-"""croaring_b200 — B200-native Roaring set-algebra engine (hot path of CRoaring on sm_100a).
+"""croaring_b200 — H100-native Roaring set-algebra engine (hot path of CRoaring on sm_90a).
 
 The product is the C-ABI library libroaring_b200.so (include/roaring_b200.h); this package is
 its Python mirror (ctypes) plus workload I/O helpers.  See DESIGN.md / INTEGRATION.md.

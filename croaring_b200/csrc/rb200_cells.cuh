@@ -11,9 +11,8 @@ namespace rb200 {
 #endif
 #ifndef RB200_RANK_SCATTER
 // larger ones: 1 = accumulator + rank-scatter emission (rb200_device.cuh), 0 = accumulator + ordered
-// find-first-set emission.  Measured on B200 with class-ordered tickets (profiles/r2): rank-scatter
-// executes 20 % fewer instructions but is 3 % SLOWER per step (4.81 vs 4.67 ms of kernel time: its
-// 2-byte scattered loads / stores wait on the memory pipe), so the default stays 0.
+// find-first-set emission.  Rank-scatter executes fewer instructions, but its 2-byte scattered
+// loads / stores wait on the memory pipe, so the default stays 0.
 #define RB200_RANK_SCATTER 0
 #endif
 
@@ -76,8 +75,7 @@ cell_compute(uint32_t *acc, uint16_t *pre, int tA, int tB, const uint8_t *pa, co
     }
 
     // ---- array x array union / xor whose result is known to stay an array: warp merge path ---
-    // (measured on B200, weather_sept_85 all-pairs OR: staging limit 2032 values -> 1.41 ms,
-    //  1024 -> 1.50 ms, split merge up to 4064 -> 2.06 ms; the accumulator round trip wins above)
+    // (up to the staging limit; above it the accumulator round trip is cheaper than a split merge)
     // (lazy rules: only unions / xors of at most ARRAY_LAZY_LOWERBOUND values stay arrays)
     const bool lazy_eager = lazy && OP == OP_XOR && inplace_rules;  // container_lazy_ixor A,A is eager
     if ((op == OP_OR || op == OP_XOR) && tA == T_ARRAY && tB == T_ARRAY &&

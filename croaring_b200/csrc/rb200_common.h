@@ -115,11 +115,11 @@ struct OpStats {
 
 // Code-path classes of the pairwise work items.  k_compute_items is one large kernel (a code path
 // per cell family); when the warps of an SM run different families at the same time it is bound
-// by INSTRUCTION FETCH (ncu, profiles/r2: no_instruction stalls 6.3 per issued instruction), so
+// by INSTRUCTION FETCH (ncu: no_instruction stalls dominate), so
 // the tickets are handed out class by class: at any time almost every resident warp executes the
 // same few hundred instructions.  Heavy classes first (tail balance).
-// (measured with per-item clocks, tools/scale_probe.py: run cells through the accumulator cost
-//  100-450 k clocks each under load, 10-30x the average item — they go first)
+// (per-item clocks, tools/scale_probe.py: run cells through the accumulator cost an order of
+//  magnitude more than the average item under load — they go first)
 constexpr int CLS_RUN_ACC = 0;   // run cells through the accumulator
 constexpr int CLS_BR = 1;        // bitset x run
 constexpr int CLS_AA_ACC = 2;    // array x array through the accumulator (large unions / xors)

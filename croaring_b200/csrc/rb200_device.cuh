@@ -1,4 +1,4 @@
-// rb200_device.cuh — warp-level building blocks of the container x container grid (sm_100a).
+// rb200_device.cuh — warp-level building blocks of the container x container grid (sm_90a).
 //
 // One warp owns one 65536-bit accumulator `acc` (2048 x u32 = 8 KiB of shared memory) and
 // evaluates one grid cell on it:
@@ -306,8 +306,8 @@ __device__ __forceinline__ void acc_plain(uint32_t *p) {
 // acc op= {sorted u16 array}.  128-bit loads (8 values per lane); bits that fall in the same
 // 32-bit word are merged in registers before the shared-memory atomic.
 #ifndef RB200_APPLY_SPARSE_MAX
-#define RB200_APPLY_SPARSE_MAX 4097   // arrays below this many values set their bits one atomic per value (measured: merging same-word
-                                      // bits in registers first costs more instructions than it saves atomics: 4.31 -> 4.16 ms per step)
+#define RB200_APPLY_SPARSE_MAX 4097   // arrays below this many values set their bits one atomic per value (merging same-word
+                                      // bits in registers first costs more instructions than it saves atomics)
 #endif
 template <int MODE>
 __device__ __forceinline__ void acc_apply_array(uint32_t *acc, const uint8_t *src, uint32_t n,
@@ -631,9 +631,9 @@ __device__ __forceinline__ void acc_count(const uint32_t *acc, int lane, bool wa
 // owns one 128-bit group per stripe (conflict-free LDS.128, value order == lane order),
 // per-lane popcount -> warp scan -> every lane emits its bits at its offset, so a stripe's
 // output is one contiguous, mostly sector-coalesced range.
-// Measured alternatives (weather_sept_85 all-pairs OR, ncu): 64 stripes of one word per lane
-// 1.73 ms; this layout 1.31 ms; + cooperative emission of dense halves 1.34 ms; one 32-bit
-// find-first-set loop per lane 1.37 ms; four 32-bit loops 1.43 ms.
+// Alternatives tried on weather_sept_85 all-pairs OR, all slower than this layout: 64 stripes of
+// one word per lane; cooperative emission of dense halves; one or four 32-bit find-first-set
+// loops per lane.
 __device__ __forceinline__ uint32_t acc_emit_array(const uint32_t *acc, uint16_t *out, int lane) {
     uint32_t base = 0;
 #pragma unroll 1
@@ -667,8 +667,8 @@ __device__ __forceinline__ uint32_t acc_emit_array(const uint32_t *acc, uint16_t
 // value v is its rank in the accumulator: pre[v >> 7] (set bits before its 128-bit group, a
 // 512-entry table built with one warp scan per touched stripe) + the bits below it inside the
 // group.  Every input value computes that and stores ITSELF — no find-first-set loops, whose
-// trip count is the densest lane's (the hot spot of acc_emit_array on clustered data: 45 % of the
-// kernel's instructions in profiles/r1d), and the cardinality falls out of the table for free.
+// trip count is the densest lane's (the hot spot of acc_emit_array on clustered data), and the
+// cardinality falls out of the table for free.
 // Stripes outside [s0, s1) hold no bits and are neither zeroed, scanned nor read.
 __device__ __forceinline__ void acc_zero_span(uint32_t *acc, int lane, int s0, int s1) {
     const uint4 z = make_uint4(0, 0, 0, 0);
@@ -985,7 +985,7 @@ interval_cell(uint32_t *acc, int op, int tA, int tB, const uint8_t *pa, const ui
 }
 
 // ---------------------------------------------------------------- TMA bulk copies + mbarrier
-// Operand staging the Blackwell way: ONE elected thread issues cp.async.bulk (global -> shared,
+// Operand staging with the Hopper TMA unit: ONE elected thread issues cp.async.bulk (global -> shared,
 // whole containers, 16-byte granules) against an mbarrier; the bytes land asynchronously while the
 // other warps keep working on the previous batch, and nobody holds registers for loads in flight.
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -3,7 +3,7 @@
 // 1342) called on one pair of host bitmaps.
 //
 // The batched path costs a single pair three launches, four copies and two host round trips
-// (~100 us, all latency).  Here the host packs both operands into one pinned block, ONE
+// (all latency).  Here the host packs both operands into one pinned block, ONE
 // cudaMemcpyAsync moves it, ONE kernel — a single CTA, eight warps — plans the key merge
 // (src/roaring.c:742-768, 896-951 as binary-search ranks, like k_plan_pairs), evaluates the cells
 // with the very same cell_compute() as the batched kernel (one warp per cell, eight 8 KiB

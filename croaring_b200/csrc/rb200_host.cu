@@ -117,7 +117,7 @@ struct Ctx {
     // single-pair fused path (rb200_fused.cu): packed operands (pinned + device), mapped result block
     uint8_t *h_fused_in = nullptr, *d_fused_in = nullptr, *h_fused_out = nullptr, *d_fused_out = nullptr;
     uint32_t fused_seq = 0;
-    int sms = 148;
+    int sms = 132;
     std::multimap<size_t, void *> dpool, hpool;
     std::mutex alloc_mu;  // dpool / hpool are also used by the background downloader thread
     uint64_t last_algo_bytes = 0;
@@ -206,11 +206,14 @@ void *dev_alloc(size_t n) {
     void *p = nullptr;
     cudaError_t e = cudaMalloc(&p, b);
     if (e != cudaSuccess) {
-        // drop the cache and retry once
+        // drop the cache and retry once; the failure is reported through t_err, so it must not stay
+        // behind as the runtime's last error for the next launch check to find
+        (void)cudaGetLastError();
         for (auto &kv : g.dpool) cudaFree(kv.second);
         g.dpool.clear();
         e = cudaMalloc(&p, b);
         if (e != cudaSuccess) {
+            (void)cudaGetLastError();
             t_err = std::string("cudaMalloc: ") + cudaGetErrorString(e);
             return nullptr;
         }
@@ -244,6 +247,7 @@ void *pin_alloc(size_t n) {
     cudaError_t e = cudaHostAlloc(&p, b, cudaHostAllocDefault);
     if (moved) pthread_setaffinity_np(pthread_self(), sizeof(saved), &saved);
     if (e != cudaSuccess) {
+        (void)cudaGetLastError();   // reported through t_err, not left for the next launch check
         t_err = std::string("cudaHostAlloc: ") + cudaGetErrorString(e);
         return nullptr;
     }
@@ -1316,8 +1320,9 @@ struct PairBuf {
     uint64_t *d_off = nullptr;
     uint64_t W = 0, slab_bound = 0;
     // op: OP_* of the batch (OP_AND also for the cardinality-only sweeps, which need no slab)
+    // flip: B is the range bitmap of rb200_batch_flip (every container ONE run)
     bool build(const rb200_set *A, const rb200_set *B, const uint32_t *ia, const uint32_t *ib,
-               size_t np, int op, bool lazy = false) {
+               size_t np, int op, bool lazy = false, bool flip = false) {
         if (!ensure_mirrors(A) || !ensure_mirrors(B)) return false;
         if (np > 0xffffffffull) { t_err = "too many pairs in one batch (2^32 - 1 at most)"; return false; }
         const size_t o_off = 0, o_ia = al256(8 * (np + 1)), o_ib = o_ia + al256(4 * np);
@@ -1345,7 +1350,14 @@ struct PairBuf {
             // larger than either, so it fits min(8192, 2 * card_result); card_result <= cA + cB
             // (OR, XOR), <= min(cA, cB) (AND), <= cA (ANDNOT).  slot_bound() obeys the same limits.
             const uint64_t EA = A->h_ebytes[a], EB = B->h_ebytes[b];
-            if (lazy) {
+            if (flip) {
+                // the slots k_plan_pairs reserves: a copy of A's container (<= its effective bytes),
+                // a copy of a one-run range container (16), a matched cell (slot_bound_lazy with
+                // nB = 1: <= 8 KiB + 16 + twice A's stored bytes).  EB counts 8 KiB for every key
+                // the range covers, which for a range over the whole universe is 512 MiB per pair.
+                const uint64_t m = na < nb ? na : nb;
+                sb += 2 * EA + 16 * (uint64_t)nb + m * (uint64_t)(BITSET_BYTES + 16) + 512;
+            } else if (lazy) {
                 // lazy array x run unions stay runs (4 bytes per input value / run), flips add 8 KiB per key
                 const uint64_t m = na < nb ? na : nb;
                 sb += 3 * (EA + EB) + m * (uint64_t)BITSET_BYTES + 512;
@@ -1405,12 +1417,12 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     PairBuf pb;
     ItemsBuf ib_;
     rb200_set *R = nullptr;
-    bool ok = pb.build(A, B, ia, ib, np, op, (rules & RULES_LAZY) != 0);
+    bool ok = pb.build(A, B, ia, ib, np, op, (rules & RULES_LAZY) != 0, (rules & RULES_FLIP) != 0);
     // class-ordered tickets pay one more small kernel: only for batches that fill the GPU
     static const uint64_t order_min = []() { const char *e = getenv("RB200_ORDER_MIN"); return e ? (uint64_t)atoll(e) : 16384ull; }();
     // (tried in round 2: ONE launch with a CTA per pair doing plan -> cells -> finalize for small batches —
-    //  the 199-pair successive sweep took 84-174 us of device time per call instead of 53-126 us: a
-    //  pair's cells serialise on its 8 warps while the three-kernel path spreads them over the GPU)
+    //  the 199-pair successive sweep took more device time per call: a pair's cells serialise on
+    //  its 8 warps while the three-kernel path spreads them over the GPU)
     if (ok) ok = ib_.alloc(pb.W, pb.W >= order_min);
     if (ok) {
         R = set_new((uint32_t)np, pb.W, pb.slab_bound);
@@ -1433,8 +1445,8 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         // (32 x 8 KiB on one warp would be the tail of the launch)
         const uint64_t n_cont = A->n_containers + B->n_containers;
         const uint64_t avg_b = n_cont ? (A->slab_used + B->slab_used) / n_cont : 4096;
-        // (measured on the real-data suite, kernel ms per OR+XOR step at 4 / 8 / 16 / 32 items: 3.09 / 3.06 /
-        //  3.07 / 3.11; 1 item: 3.57 — RB200_COPY_TICKET overrides)
+        // (on the real-data suite 4-32 items per ticket are within noise of each other, 1 item is
+        //  clearly slower — RB200_COPY_TICKET overrides)
         static const int ct_env = []() { const char *e = getenv("RB200_COPY_TICKET"); return e ? std::min(32, std::max(1, atoi(e))) : 0; }();
         const int copy_ticket = ct_env ? ct_env : avg_b <= 256 ? 32 : avg_b <= 2048 ? 16 : 8;
         launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_stats, rules, copy_ticket, g.stream);
@@ -1996,10 +2008,10 @@ void bind_to_local_cpus() {
     for (int c : cpus) if (c < CPU_SETSIZE) CPU_SET(c, &set);
     pthread_setaffinity_np(pthread_self(), sizeof(set), &set);
 }
-// Host worker threads for materialisation.  Measured on the 2 x 32-core host of this pool
-// (profiles/r1c/e2e_threads.txt): the stream is PCIe bound from 8 threads on, 24 is the sweet spot,
-// 40+ threads LOSE 20-80 % (remote-socket traffic on the pinned staging buffers), so the default
-// is 24 threads bound to the CPUs of the GPU's NUMA node.  RB200_HOST_THREADS overrides.
+// Host worker threads for materialisation.  On a two-socket host the stream is PCIe bound well
+// before all cores are busy, and threads on the remote socket slow it down (remote-socket traffic
+// on the pinned staging buffers), so the default is 24 threads bound to the CPUs of the GPU's
+// NUMA node.  RB200_HOST_THREADS overrides.
 unsigned host_workers() {
     static unsigned T = 0;
     if (!T) {

@@ -1,4 +1,4 @@
-// rb200_kernels.cu — sm_100a kernels of the Roaring set-algebra hot path.
+// rb200_kernels.cu — sm_90a kernels of the Roaring set-algebra hot path.
 //
 //   k_plan_pairs      warp per bitmap pair: key merge by binary-search ranks (the reference's
 //                     two-pointer loops, src/roaring.c:742-768, 896-951) -> work items.
@@ -22,7 +22,7 @@ static inline int sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -240,10 +240,10 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
     // (small batches: tickets of 1 so that every warp of the grid gets work at once)
     // with an order list (big batches) the tickets walk the live items class by class
     // (tried: a lean kernel of its own for the pass-through class — 40 registers, no accumulator —
-    //  launched behind this one: 4.78 vs 4.53 ms per step, the copies no longer overlap the cells)
-    // Ticket granularity (measured, tools/scale_probe.py): cells take ONE item per ticket — four
-    // consecutive heavy cells on one warp were the tail of every launch (weather OR at 1/8 of the
-    // pairs: 363 -> 218 us) — pass-through copies 32, one per lane (below).
+    //  launched behind this one: slower, the copies no longer overlap the cells)
+    // Ticket granularity (tools/scale_probe.py): cells take ONE item per ticket — four
+    // consecutive heavy cells on one warp were the tail of every launch — pass-through copies 32,
+    // one per lane (below).
     unsigned long long n_cells = W, T = W;      // no order list (small batches): tickets of one item
     if (it.order) {
         unsigned long long live = 0;
@@ -265,8 +265,8 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
         if (lane == 0) next = atomicAdd(&st->work_counter, 1ull);
         if (tk >= n_cells) {
             // ---- pass-through ticket: copy_ticket (4 .. 32) items, ONE PER LANE through the dependent metadata chain
-            // (order -> item -> container -> payload address: ~3 us per item when a warp walked it
-            // item by item — the whole cost of the copy-heavy launches), then the warp copies the
+            // (order -> item -> container -> payload address: walked item by item by a warp, that
+            // chain was the whole cost of the copy-heavy launches), then the warp copies the
             // payloads, the first 512 bytes of four items in flight at a time
             const unsigned long long slot = n_cells + (tk - n_cells) * copy_ticket + lane;
             const bool valid = lane < copy_ticket && slot < W;

@@ -1,4 +1,4 @@
-// rb200_many.cu — N-way union (roaring_bitmap_or_many, src/roaring.c:775-790) on sm_100a.
+// rb200_many.cu — N-way union (roaring_bitmap_or_many, src/roaring.c:775-790) on sm_90a.
 //
 // The reference folds the inputs left to right with lazy cells (roaring_bitmap_lazy_or
 // :2509-2598, roaring_bitmap_lazy_or_inplace :2600-2682, container_lazy_or / container_lazy_ior

@@ -84,8 +84,8 @@ k_many2_count(SetView S, const uint32_t *__restrict__ idx, uint32_t n, uint32_t 
 // keys are distinct, so position <= key - first key: a galloping search from that bound, 1-3 probes
 // on dense directories — then a warp reads the <= 32 containers of (window, bitmap) in one
 // coalesced access and counts them with SHARED-memory atomics.  No global atomic anywhere
-// (the bitmap-major kernels above spend one L2 atomic per container: 1.7 + 3.3 ms on the 13 M
-// containers of config 3 at density 0.003; this form: see profiles/).
+// (the bitmap-major kernels above spend one L2 atomic per container, which dominates on the 13 M
+// containers of config 3 at density 0.003).
 constexpr int M2W_KEYS = 32, M2W_THREADS = 256;
 
 // live key span of the participants -> key_fill[0] = largest key, key_fill[1] = 65535 - smallest key
@@ -447,7 +447,7 @@ __device__ __forceinline__ unsigned long long block_min64(Many2Smem &sm, unsigne
 // TMA = true: operands staged by bulk copies (bitset-dominated inputs); false: direct global loads
 // (array-dominated inputs, where a bulk copy per small container costs more than it hides)
 #ifndef RB200_M2_PIPE
-#define RB200_M2_PIPE 1   // 1: warp-level full / empty mbarrier pipeline in the TMA path (no block barrier per half: 0.441 -> 0.423 ms at d = 0.3); 0: block barrier per half
+#define RB200_M2_PIPE 1   // 1: warp-level full / empty mbarrier pipeline in the TMA path (no block barrier per half); 0: block barrier per half
 #endif
 #ifndef RB200_M2_MINB
 #define RB200_M2_MINB 4   // resident CTAs per SM of the direct path (register budget 64 at 4)
@@ -574,8 +574,8 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
                 // small arrays: the 16-byte vectors of ALL of them as one flat list, a thread per vector
                 // (two in flight): every lane loads whatever the container sizes are — a warp per
                 // container left 18 of 32 lanes idle on the ~110-value arrays of the sparse densities
-                // (config 3, d = 0.003: 3.62 -> 2.50 ms; arrays that fill a warp's 32 lanes anyway stay
-                //  on the warp path below: flat for all sizes cost 1.15 -> 1.28 ms at d = 0.03)
+                // (arrays that fill a warp's 32 lanes anyway stay on the warp path below: the flat
+                //  list for all sizes was slower at d = 0.03)
                 const uint32_t V = sm.s_vend[M2_STAGE - 1];
                 for (uint32_t x0 = 4 * tid; x0 < V; x0 += 4 * M2_THREADS) {
                     // four CONSECUTIVE vectors per thread: one search, then a linear walk; all four loads in flight

@@ -274,8 +274,8 @@ RB_API int rb200_plan_key_ranges(const char *const *bufs, const size_t *lens, si
             rb200::set_error("plan_key_ranges: malformed portable bitmap at index " + std::to_string(b));
             return -1;
         }
-        // weight of a container = its bytes + a fixed per-container cost (k_or_many2 measured on config 3:
-        // ~0.4 ms per GB plus ~0.19 ns per container, i.e. a container costs as much as ~0.5 KiB)
+        // weight of a container = its bytes + a fixed per-container cost (k_or_many2 on config 3: a
+        // container costs about as much as 0.5 KiB of payload)
         for (uint32_t i = 0; i < ix.n; i++) hist[ix.key[i]] += (uint64_t)ix.size[i] + 512;
         if (ix.n) {
             any = true;

@@ -1,5 +1,5 @@
 /*
- * roaring_b200.h — C ABI of the B200-native Roaring set-algebra engine (libroaring_b200.so).
+ * roaring_b200.h — C ABI of the H100-native Roaring set-algebra engine (libroaring_b200.so).
  *
  * Plain C: only pointers, sizes and PODs cross this boundary; no torch / C++ / CUDA types.
  *
@@ -9,7 +9,7 @@
  * (paths relative to the reference tree).  They take and return host `roaring_bitmap_t`
  * objects in the reference's memory layout, so every other reference function
  * (roaring_bitmap_free, _contains, _portable_serialize, iterators ...) keeps working on what
- * they return.  The work itself is done by sm_100a CUDA kernels; there is NO CPU fallback:
+ * they return.  The work itself is done by sm_90a CUDA kernels; there is NO CPU fallback:
  * on a CUDA failure they return NULL / UINT64_MAX and rb200_last_error() says why.
  *
  * Part 2 (rb200_*) is the batched, device-resident form the GPU needs to be worth using:

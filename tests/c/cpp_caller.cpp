@@ -1,7 +1,7 @@
 // A C++ caller written against the REFERENCE's header-only wrapper (cpp/roaring/roaring.hh:
 // operator&, operator|, operator^, operator-, the compound assignments, and_cardinality,
-// fastunion).  tests/test_link_resolution.py links it with -lroaring_b200 ahead of -lroaring_ref
-// and checks which library the dynamic linker binds every roaring_bitmap_* symbol to; the calls
+// fastunion).  oracle/Makefile links it with -lroaring_b200 ahead of -lroaring_ref and
+// tests/test_link_resolution.py checks which library the dynamic linker binds every roaring_bitmap_* symbol to; the calls
 // sit behind an argument check so the symbols are referenced without anything being executed.
 #include <cstdio>
 

@@ -2,7 +2,7 @@
 # Host-side sanitizer pass (no GPU needed): rebuild rb200_host.cu / rb200_shard.cu with
 # -fsanitize=address,undefined, link them with the product's device objects into a scratch library
 # and run the CPU-executable paths (portable (de)serializer, blob algebra, mutation fuzz, host ABI
-# tests) against it.      bash tools/host_asan.sh > profiles/r2/host_asan.txt 2>&1
+# tests) against it.      bash tools/host_asan.sh > host_asan.txt 2>&1
 set -e
 ROOT=$(cd "$(dirname "$0")/.." && pwd)
 OUT=${TMPDIR:-/tmp}/rb200_asan
@@ -10,7 +10,7 @@ mkdir -p "$OUT"
 python -m croaring_b200.build > /dev/null            # the product's objects (device code)
 cd "$ROOT/croaring_b200/csrc"
 for f in rb200_host rb200_shard; do
-  nvcc -O1 -g -std=c++17 -gencode arch=compute_100a,code=sm_100a --expt-relaxed-constexpr -cudart static -DRB200_BUILDING_LIBRARY \
+  nvcc -O1 -g -std=c++17 -gencode arch=compute_90a,code=sm_90a --expt-relaxed-constexpr -cudart static -DRB200_BUILDING_LIBRARY \
        -Xcompiler -fPIC,-fvisibility=hidden,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer \
        -c $f.cu -o "$OUT/$f.o" 2>&1 | grep -v deprecated || true
 done

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """ncu CSV (dram__bytes_read/write.sum per k_compute_items launch of one bench step) ->
-profiles/roofline_traffic.json, the `traffic` field of bench.py's roofline object."""
+profiles/roofline_traffic.json (not committed), the `traffic` field of bench.py's roofline object."""
 import csv
 import json
 import sys

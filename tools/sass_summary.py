@@ -4,7 +4,7 @@
 paths the code uses (UBLKCP = cp.async.bulk / TMA bulk copy, SYNCS = mbarrier, ATOMS / ATOMG =
 shared / global atomics, POPC, REDUX, ...).
 
-    python tools/sass_summary.py > profiles/r2/sass_summary.txt
+    python tools/sass_summary.py > sass_summary.txt
 
 Rebuilds the product with `-Xptxas -v` and disassembles the objects with cuobjdump."""
 import collections
@@ -31,7 +31,7 @@ def main():
                          capture_output=True, text=True)
     text = log.stdout + log.stderr
     res = {}
-    pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_100a'\n(?:ptxas info\s*:\s*Function properties for [^\n]+\n)?"
+    pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_90a'\n(?:ptxas info\s*:\s*Function properties for [^\n]+\n)?"
                      r"\s*(?:ptxas info\s*:\s*)?(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
                      r"ptxas info\s*:\s*Used (\d+) registers(?:, used (\d+) barriers)?(?:, (\d+) bytes smem)?")
     for name, stack, ss, sl, regs, _bars, smem in pat.findall(text):
@@ -52,7 +52,7 @@ def main():
                 counts[cur][m.group(1)] += 1
                 counts[cur]["_total"] += 1
     print("# kernel: registers / stack / spill st+ld bytes / static smem | SASS instructions | mnemonic counts")
-    print("# (sm_100a, nvcc " + subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout.strip().splitlines()[-2].strip() + ")")
+    print("# (sm_90a, nvcc " + subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout.strip().splitlines()[-2].strip() + ")")
     for k in sorted(counts):
         r = res.get(k, {})
         c = counts[k]
