@@ -6,21 +6,11 @@
 
 namespace rb200 {
 
-#ifndef RB200_MERGE_LIMIT
-#define RB200_MERGE_LIMIT 2048   // array x array unions up to this many staged values take the merge path
-#endif
-#ifndef RB200_RANK_SCATTER
-// larger ones: 1 = accumulator + rank-scatter emission (rb200_device.cuh), 0 = accumulator + ordered
-// find-first-set emission.  Rank-scatter executes fewer instructions, but its 2-byte scattered
-// loads / stores wait on the memory pipe, so the default stays 0.
-#define RB200_RANK_SCATTER 0
-#endif
-
 // ------------------------------------------------------------------------------ grid cells
 // Evaluate one matched cell on the warp's accumulator and write the result payload.
 template <int OP, bool LAZY>
 __device__ __forceinline__ void
-cell_compute(uint32_t *acc, uint16_t *pre, int tA, int tB, const uint8_t *pa, const uint8_t *pb,
+cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb,
              uint32_t cA, uint32_t cB, uint32_t lA, uint32_t lB, uint8_t *out, uint32_t cap,
              int lane, int &otype, uint32_t &ocard, uint32_t &olen, unsigned int *err,
              int rules, bool unkA) {
@@ -75,55 +65,16 @@ cell_compute(uint32_t *acc, uint16_t *pre, int tA, int tB, const uint8_t *pa, co
     }
 
     // ---- array x array union / xor whose result is known to stay an array: warp merge path ---
-    // (up to the staging limit; above it the accumulator round trip is cheaper than a split merge)
+    // (cA + cB <= MAX_ARRAY: the type rule makes the result an array whatever its cardinality)
     // (lazy rules: only unions / xors of at most ARRAY_LAZY_LOWERBOUND values stay arrays)
     const bool lazy_eager = lazy && OP == OP_XOR && inplace_rules;  // container_lazy_ixor A,A is eager
-    if ((op == OP_OR || op == OP_XOR) && tA == T_ARRAY && tB == T_ARRAY &&
-        ((cA + 7) & ~7u) + ((cB + 7) & ~7u) <= (uint32_t)RB200_MERGE_LIMIT &&
+    if ((op == OP_OR || op == OP_XOR) && tA == T_ARRAY && tB == T_ARRAY && cA + cB <= (uint32_t)MAX_ARRAY &&
         (!lazy || lazy_eager || (cA + cB <= 1024u && !(rules & RULES_CONV)))) {
         if (round16(2 * (cA + cB)) > cap) { if (lane == 0) atomicExch(err, 1u); otype = 0; return; }
         const uint32_t n = (op == OP_OR) ? merge_arrays<false>(acc, pa, cA, pb, cB, out, lane)
                                          : merge_arrays<true>(acc, pa, cA, pb, cB, out, lane);
         otype = n ? T_ARRAY : 0;  // cA + cB <= 4096 -> array (mixed_union.c:162-176, mixed_xor.c:196-205)
         ocard = olen = n;
-        return;
-    }
-
-    // ---- larger array x array unions / symmetric differences: accumulator + rank-scatter -------
-    if (RB200_RANK_SCATTER && !lazy && (op == OP_OR || op == OP_XOR) && tA == T_ARRAY && tB == T_ARRAY) {
-        const uint16_t *a16 = reinterpret_cast<const uint16_t *>(pa), *b16 = reinterpret_cast<const uint16_t *>(pb);
-        const uint32_t vlo = min((uint32_t)a16[0], (uint32_t)b16[0]);
-        const uint32_t vhi = max((uint32_t)a16[cA - 1], (uint32_t)b16[cB - 1]);
-        const int s0 = (int)(vlo >> 12), s1 = (int)(vhi >> 12) + 1;   // stripes of 4096 values that can hold a bit
-        acc_zero_span(acc, lane, s0, s1);
-        __syncwarp();
-        acc_apply_array<0>(acc, pa, cA, lane);
-        __syncwarp();
-        if (op == OP_OR) acc_apply_array<0>(acc, pb, cB, lane);
-        else acc_apply_array<1>(acc, pb, cB, lane);
-        __syncwarp();
-        const int card = acc_prefix_span(acc, pre, lane, s0, s1);
-        __syncwarp();
-        if (card == 0) { otype = 0; ocard = olen = 0; return; }
-        const int t = decide_type(op, tA, tB, cA, cB, lA, lB, card, 0);   // array x array: never a run
-        if (stored_bytes(t, t == T_BITSET ? 1024u : (uint32_t)card) > cap) { if (lane == 0) atomicExch(err, 1u); otype = 0; return; }
-        if (t == T_BITSET) {
-            // stripes outside the span were not zeroed: complete the accumulator before the copy
-            acc_zero_span(acc, lane, 0, s0);
-            acc_zero_span(acc, lane, s1, 16);
-            __syncwarp();
-            acc_store_bitset(acc, out, lane);
-        } else if (op == OP_OR) {
-            rank_store_array<false>(acc, pre, pa, cA, reinterpret_cast<uint16_t *>(out), lane);
-            rank_store_array<false>(acc, pre, pb, cB, reinterpret_cast<uint16_t *>(out), lane);
-        } else {
-            rank_store_array<true>(acc, pre, pa, cA, reinterpret_cast<uint16_t *>(out), lane);
-            rank_store_array<true>(acc, pre, pb, cB, reinterpret_cast<uint16_t *>(out), lane);
-        }
-        __syncwarp();
-        otype = t;
-        ocard = (uint32_t)card;
-        olen = t == T_BITSET ? 1024u : (uint32_t)card;
         return;
     }
 

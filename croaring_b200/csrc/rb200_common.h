@@ -122,7 +122,7 @@ struct OpStats {
 //  magnitude more than the average item under load — they go first)
 constexpr int CLS_RUN_ACC = 0;   // run cells through the accumulator
 constexpr int CLS_BR = 1;        // bitset x run
-constexpr int CLS_AA_ACC = 2;    // array x array through the accumulator (large unions / xors)
+constexpr int CLS_AA_ACC = 2;    // array x array through the accumulator (unions / xors above 4096 values)
 constexpr int CLS_BA = 3;        // bitset x array (either side)
 constexpr int CLS_BB = 4;        // bitset x bitset
 constexpr int CLS_AA = 5;        // array x array: filter / merge path

@@ -662,47 +662,6 @@ __device__ __forceinline__ uint32_t acc_emit_array(const uint32_t *acc, uint16_t
     return base;
 }
 
-// ---- rank-scatter emission of array x array unions / symmetric differences -------------------
-// For a result that is an ARRAY built from two ARRAY inputs, the output position of an input
-// value v is its rank in the accumulator: pre[v >> 7] (set bits before its 128-bit group, a
-// 512-entry table built with one warp scan per touched stripe) + the bits below it inside the
-// group.  Every input value computes that and stores ITSELF — no find-first-set loops, whose
-// trip count is the densest lane's (the hot spot of acc_emit_array on clustered data), and the
-// cardinality falls out of the table for free.
-// Stripes outside [s0, s1) hold no bits and are neither zeroed, scanned nor read.
-__device__ __forceinline__ void acc_zero_span(uint32_t *acc, int lane, int s0, int s1) {
-    const uint4 z = make_uint4(0, 0, 0, 0);
-    for (int i = s0; i < s1; i++) reinterpret_cast<uint4 *>(acc)[i * 32 + lane] = z;
-}
-// exclusive prefix popcount per 128-bit group over stripes [s0, s1); returns the cardinality
-__device__ __forceinline__ int acc_prefix_span(const uint32_t *acc, uint16_t *pre, int lane, int s0, int s1) {
-    uint32_t base = 0;
-    for (int it = s0; it < s1; it++) {
-        const uint32_t c = popc4(reinterpret_cast<const uint4 *>(acc)[it * 32 + lane]);
-        const uint32_t incl = warp_incl_scan(c, lane);
-        pre[it * 32 + lane] = (uint16_t)(base + incl - c);   // read only for groups that hold a bit: < 65536
-        base += __shfl_sync(FULLMASK, incl, 31);
-    }
-    return (int)base;
-}
-// out[rank(v)] = v for every value of the sorted array `src` (CHECK: only if its bit survived)
-template <bool CHECK>
-__device__ __forceinline__ void rank_store_array(const uint32_t *acc, const uint16_t *pre, const uint8_t *src,
-                                                 uint32_t n, uint16_t *out, int lane) {
-    const uint16_t *arr = reinterpret_cast<const uint16_t *>(src);
-    for (uint32_t i = lane; i < n; i += 32) {
-        const uint32_t v = arr[i], w = v >> 5, g = w >> 2, k = w & 3;
-        const uint4 q = reinterpret_cast<const uint4 *>(acc)[g];
-        const uint32_t word = k == 0 ? q.x : (k == 1 ? q.y : (k == 2 ? q.z : q.w));
-        if (CHECK && !((word >> (v & 31)) & 1u)) continue;
-        uint32_t r = pre[g] + __popc(word & ((1u << (v & 31)) - 1u));
-        r += k > 0 ? __popc(q.x) : 0;
-        r += k > 1 ? __popc(q.y) : 0;
-        r += k > 2 ? __popc(q.z) : 0;
-        out[r] = (uint16_t)v;
-    }
-}
-
 // acc -> run list {start, length-1}: pass 1 writes run starts, pass 2 run ends, pass 3 turns
 // ends into lengths.  Returns the number of runs.
 static __device__ __noinline__ uint32_t acc_emit_runs(const uint32_t *acc, uint16_t *out, int lane) {
@@ -764,14 +723,6 @@ __device__ __forceinline__ uint32_t filter_array(const uint8_t *src, uint32_t n,
     return cnt;
 }
 
-// Union / symmetric difference of two sorted u16 arrays WITHOUT the bitset round trip
-// (array_container_union / xor, src/array_util.c:1104,1198 — here a warp merge path).
-// Both inputs are staged in the low 4 KiB of the warp's accumulator, the output in the high
-// 4 KiB, so it needs round8(n) + round8(m) <= 2048.  Every lane owns one contiguous slice of
-// the merged sequence (diagonal binary search), runs the sequential merge twice (count, then
-// write at its scanned offset) and the warp copies the staged result out with 128-bit stores.
-// Duplicates (a value present in both inputs) are adjacent in the merged order: OR keeps the
-// first, XOR drops both.
 // global -> shared staging of a u16 range (128-bit when the source is 16-byte aligned)
 __device__ __forceinline__ void stage_u16(uint16_t *dst, const uint8_t *src, uint32_t n, int lane) {
     if ((reinterpret_cast<uintptr_t>(src) & 15) == 0) {
@@ -783,65 +734,106 @@ __device__ __forceinline__ void stage_u16(uint16_t *dst, const uint8_t *src, uin
     }
 }
 
+// Union / symmetric difference of two sorted u16 arrays with n + m <= 4096 values, the cells whose
+// result the type rule makes an array (array_container_union / xor, src/array_util.c:1104,1198),
+// as a windowed warp merge path: no accumulator round trip and no find-first-set emission.
+// Both inputs are staged once in the warp's shared block, a at 0 and b at round8(n); the 128-bit
+// staging reaches u16 index round8(n) + round8(m) <= 4104.  The merged sequence is produced in
+// windows of 32 * MERGE_PER_LANE positions: every lane finds the split of its diagonal (merge-path
+// search between the window's start split and MERGE_PER_LANE more values per lane before it),
+// merges its values in registers and decides which survive.  Duplicates (a value present in both
+// inputs) are adjacent in the merged order: OR keeps the first, XOR drops both.  A warp scan places
+// the survivors in the window buffer (u16 index MERGE_WBUF, past the staging) and the warp stores
+// them at the running output offset.  The buffer mirrors the output from the last 16-byte boundary,
+// so the stores are whole 128-bit words; the partial last word carries into the next window.
+constexpr uint32_t MERGE_PER_LANE = 8, MERGE_WIN = 32 * MERGE_PER_LANE;
+constexpr uint32_t MERGE_WBUF = 4104;
+// per-warp shared block: the 8 KiB accumulator, then room for the merge's window buffer (9 KiB)
+constexpr int WARP_SMEM_WORDS = ACC_WORDS + 256;
+static_assert(2 * MERGE_WBUF + 2 * (MERGE_WIN + 8) <= 4 * WARP_SMEM_WORDS, "merge window buffer");
+
+// Not inlined: the cell kernel's other paths then keep their register allocation (measured faster
+// than the inlined merge on the headline workload).
 template <bool IS_XOR>
-__device__ __forceinline__ uint32_t merge_arrays(uint32_t *acc, const uint8_t *pa, uint32_t n,
-                                                 const uint8_t *pb, uint32_t m, uint8_t *out,
-                                                 int lane) {
+static __device__ __noinline__ uint32_t merge_arrays(uint32_t *acc, const uint8_t *pa, uint32_t n,
+                                                     const uint8_t *pb, uint32_t m, uint8_t *out,
+                                                     int lane) {
     uint16_t *sa = reinterpret_cast<uint16_t *>(acc);
     uint16_t *sb = sa + ((n + 7) & ~7u);
-    uint16_t *so = reinterpret_cast<uint16_t *>(acc) + 2048;
+    uint16_t *wb = sa + MERGE_WBUF;
+    uint16_t *o16 = reinterpret_cast<uint16_t *>(out);
+    const bool vec = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
     stage_u16(sa, pa, n, lane);
     stage_u16(sb, pb, m, lane);
     __syncwarp();
-    const uint32_t T = n + m, per = (T + 31) >> 5;
-    const uint32_t d0 = min((uint32_t)lane * per, T), d1 = min(d0 + per, T);
-    // merge-path split: i0 = how many of the first d0 merged elements come from a (ties: a first)
-    uint32_t lo = d0 > m ? d0 - m : 0u, hi = min(d0, n);
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (sa[mid] <= sb[d0 - 1 - mid]) lo = mid + 1;
-        else hi = mid;
-    }
-    const uint32_t i0 = lo, j0 = d0 - lo;
-    const uint32_t NONE = 0x10000u;
-    uint32_t prev0 = NONE + 1;  // element at merged position d0-1 (none for d0 == 0)
-    if (d0 > 0) {
-        const uint32_t pa_ = i0 > 0 ? sa[i0 - 1] : 0u, pb_ = j0 > 0 ? sb[j0 - 1] : 0u;
-        prev0 = (i0 > 0 && j0 > 0) ? max(pa_, pb_) : (i0 > 0 ? pa_ : pb_);
-    }
-    uint32_t off = 0, count = 0;
+    const uint32_t T = n + m, NONE = 0x10000u;   // NONE: past the end of an input, above every value
+    uint32_t is = 0;                             // split at the window start: values taken from a
+    uint32_t last = NONE + 1;                    // merged value before the window (none yet)
+    uint32_t base = 0;                           // values written so far
 #pragma unroll 1
-    for (int pass = 0; pass < 2; pass++) {
-        uint32_t i = i0, j = j0, prev = prev0, c = 0;
+    for (uint32_t w0 = 0; w0 < T; w0 += MERGE_WIN) {
+        const uint32_t d = w0 + lane * MERGE_PER_LANE;
+        // i = how many of the first d merged values come from a (ties: a first); lanes past the end
+        // get lo = d - m > n, i.e. both inputs exhausted
+        uint32_t lo = max(is, d > m ? d - m : 0u), hi = min(is + lane * MERGE_PER_LANE, n);
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (sa[mid] <= sb[d - 1 - mid]) lo = mid + 1;
+            else hi = mid;
+        }
+        uint32_t i = lo, j = d - lo;
         uint32_t ai = i < n ? sa[i] : NONE, bj = j < m ? sb[j] : NONE;
-        for (uint32_t p = d0; p < d1; p++) {
+        // the lane's merged values, two u16 per word; keep bit k: value k survives.  The bits that
+        // need a neighbour outside the lane (bit 0, and for XOR also the last) are decided after it.
+        uint32_t xp[MERGE_PER_LANE / 2];
+        uint32_t x0 = NONE, x1 = NONE, p1 = NONE, p2 = NONE;   // values 0, 1, k-1, k-2
+        unsigned keep = 0;
+#pragma unroll
+        for (int k = 0; k < (int)MERGE_PER_LANE; k++) {
             const bool take_a = ai <= bj;
-            const uint32_t x = take_a ? ai : bj;
+            const uint32_t v = take_a ? ai : bj;
             if (take_a) { i++; ai = i < n ? sa[i] : NONE; }
             else { j++; bj = j < m ? sb[j] : NONE; }
-            const bool emit = IS_XOR ? (x != prev && x != min(ai, bj)) : (x != prev);
-            if (emit) {
-                if (pass == 1) so[off + c] = (uint16_t)x;
-                c++;
-            }
-            prev = x;
+            if (k & 1) xp[k >> 1] |= v << 16;
+            else xp[k >> 1] = v & 0xffffu;
+            if (k == 0) x0 = v;
+            if (k == 1) x1 = v;
+            if (!IS_XOR && k >= 1) keep |= (unsigned)(v < NONE && v != p1) << k;
+            if (IS_XOR && k >= 2) keep |= (unsigned)(p1 < NONE && p1 != p2 && p1 != v) << (k - 1);
+            p2 = p1;
+            p1 = v;
         }
-        if (pass == 0) {
-            const uint32_t incl = warp_incl_scan(c, lane);
-            off = incl - c;
-            count = __shfl_sync(FULLMASK, incl, 31);
+        // neighbours across the lane and window boundaries: the previous lane's last value, and the
+        // next merged value (read from the inputs) for XOR's look-ahead
+        uint32_t prev = __shfl_up_sync(FULLMASK, p1, 1);
+        if (lane == 0) prev = last;
+        last = __shfl_sync(FULLMASK, p1, 31);
+        is = __shfl_sync(FULLMASK, i, 31);
+        keep |= (unsigned)(x0 < NONE && x0 != prev && (!IS_XOR || x0 != x1));
+        if (IS_XOR) keep |= (unsigned)(p1 < NONE && p1 != p2 && p1 != min(ai, bj)) << (MERGE_PER_LANE - 1);
+        const uint32_t c = __popc(keep);
+        const uint32_t incl = warp_incl_scan(c, lane);
+        const uint32_t total = __shfl_sync(FULLMASK, incl, 31);
+        const uint32_t head = base & 7u;   // wb[t] mirrors out[(base & ~7) + t]
+        uint32_t o = head + incl - c;
+#pragma unroll
+        for (int k = 0; k < (int)MERGE_PER_LANE; k++)
+            if ((keep >> k) & 1u) wb[o++] = (uint16_t)(xp[k >> 1] >> (16 * (k & 1)));
+        __syncwarp();
+        if (vec) {
+            uint4 *dst = reinterpret_cast<uint4 *>(o16 + (base - head));
+            for (uint32_t v = lane; v < (head + total + 7) / 8; v += 32)
+                dst[v] = reinterpret_cast<const uint4 *>(wb)[v];
+        } else {
+            for (uint32_t v = lane; v < total; v += 32) o16[base + v] = wb[head + v];
         }
+        __syncwarp();
+        const uint32_t end = head + total;
+        if (lane == 0 && (end & 7u)) reinterpret_cast<uint4 *>(wb)[0] = reinterpret_cast<const uint4 *>(wb)[end >> 3];
+        __syncwarp();
+        base += total;
     }
-    __syncwarp();
-    if ((reinterpret_cast<uintptr_t>(out) & 15) == 0) {
-        for (uint32_t i = lane; i < (count + 7) / 8; i += 32)
-            reinterpret_cast<uint4 *>(out)[i] = reinterpret_cast<const uint4 *>(so)[i];
-    } else {
-        uint16_t *o16 = reinterpret_cast<uint16_t *>(out);
-        for (uint32_t i = lane; i < count; i += 32) o16[i] = so[i];
-    }
-    __syncwarp();
-    return count;
+    return base;
 }
 
 // ---------------------------------------------------------------- interval (run) algebra

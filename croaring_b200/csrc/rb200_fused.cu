@@ -26,8 +26,7 @@ __device__ __forceinline__ uint32_t lb_u16(const uint16_t *a, uint32_t n, uint32
 }
 
 struct FusedSmem {
-    uint32_t acc[FUSED_WARPS][ACC_WORDS];
-    uint16_t pre[FUSED_WARPS][512];
+    uint32_t acc[FUSED_WARPS][WARP_SMEM_WORDS];   // accumulator + merge window (rb200_device.cuh)
     uint16_t keys[FUSED_MAX_ITEMS];          // keys of A then B
     uint32_t i_slot[FUSED_MAX_ITEMS], i_cap[FUSED_MAX_ITEMS], i_ocard[FUSED_MAX_ITEMS], i_olen[FUSED_MAX_ITEMS];
     uint16_t i_ca[FUSED_MAX_ITEMS], i_cb[FUSED_MAX_ITEMS], i_key[FUSED_MAX_ITEMS];
@@ -129,7 +128,7 @@ k_pair_fused(const uint8_t *__restrict__ in, uint8_t *out, uint32_t out_bytes, i
             const uint32_t ca = sm.i_ca[item], cb = sm.i_cb[item];
             int cell_rules = rules;
             if ((rules & RULES_INPLACE) && c_shared[ca]) cell_rules &= ~RULES_INPLACE;   // roaring.c:1085-1088
-            cell_compute<OP, false>(sm.acc[wid], sm.pre[wid], c_type[ca], c_type[cb], in + c_off[ca], in + c_off[cb],
+            cell_compute<OP, false>(sm.acc[wid], c_type[ca], c_type[cb], in + c_off[ca], in + c_off[cb],
                                     c_card[ca], c_card[cb], c_len[ca], c_len[cb], dst, sm.i_cap[item], lane, otype,
                                     ocard, olen, &sm.err, cell_rules, false);
         } else {

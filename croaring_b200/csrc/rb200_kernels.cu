@@ -47,13 +47,16 @@ __device__ __forceinline__ uint32_t upper_bound_u16(const uint16_t *a, uint32_t 
 }
 
 // code-path class of a matched cell (see rb200_common.h CLS_*); mirrors the branches of cell_compute
-__device__ __forceinline__ int cell_class(int op, int tA, int tB, uint32_t cA, uint32_t cB, uint32_t lA, uint32_t lB) {
+__device__ __forceinline__ int cell_class(int op, int rules, int tA, int tB, uint32_t cA, uint32_t cB, uint32_t lA,
+                                          uint32_t lB) {
     const bool bA = tA == T_BITSET, bB = tB == T_BITSET;
     if (bA && bB) return CLS_BB;
     if (bA || bB) return (bA ? tB : tA) == T_ARRAY ? CLS_BA : CLS_BR;
     if (tA == T_ARRAY && tB == T_ARRAY) {
         if (op == OP_AND || op == OP_ANDNOT) return CLS_AA;
-        return ((cA + 7) & ~7u) + ((cB + 7) & ~7u) <= (uint32_t)RB200_MERGE_LIMIT ? CLS_AA : CLS_AA_ACC;
+        const bool lazy = (rules & RULES_LAZY) != 0, lazy_eager = lazy && op == OP_XOR && (rules & RULES_INPLACE);
+        return cA + cB <= (uint32_t)MAX_ARRAY && (!lazy || lazy_eager || (cA + cB <= 1024u && !(rules & RULES_CONV)))
+                   ? CLS_AA : CLS_AA_ACC;
     }
     return (tA == T_RUN ? lA : cA) + (tB == T_RUN ? lB : cB) <= 512u ? CLS_RUN_IV : CLS_RUN_ACC;
 }
@@ -99,7 +102,7 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
                             cap = (rules & RULES_LAZY)
                                       ? slot_bound_lazy(A.c_type[ca], B.c_type[cb], cA, cB, A.c_len[ca], B.c_len[cb])
                                       : slot_bound(op, A.c_type[ca], B.c_type[cb], cA, cB, A.c_len[ca], B.c_len[cb]);
-                            cls = cell_class(op, A.c_type[ca], B.c_type[cb], cA, cB, A.c_len[ca], B.c_len[cb]);
+                            cls = cell_class(op, rules, A.c_type[ca], B.c_type[cb], cA, cB, A.c_len[ca], B.c_len[cb]);
                         }
                     } else if (op != OP_AND && !card_only) {
                         kind = K_COPY_A;
@@ -230,11 +233,9 @@ template <int OP, bool LAZY>
 __global__ void __launch_bounds__(128, RB200_CI_MINBLOCKS)
 k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
                 uint64_t slab_cap, OpStats *st, int rules, int copy_ticket) {
-    __shared__ __align__(16) uint32_t s_acc[4][ACC_WORDS];
-    __shared__ __align__(16) uint16_t s_pre[4][512];   // rank-scatter prefix table (rb200_device.cuh)
+    __shared__ __align__(16) uint32_t s_acc[4][WARP_SMEM_WORDS];   // accumulator + merge window (rb200_device.cuh)
     const int lane = threadIdx.x & 31;
     uint32_t *acc = s_acc[threadIdx.x >> 5];
-    uint16_t *pre = s_pre[threadIdx.x >> 5];
     // dynamic scheduling: a ticket is TICKET consecutive items; the next ticket is requested
     // before the current one is processed so its latency hides behind the work.
     // (small batches: tickets of 1 so that every warp of the grid gets work at once)
@@ -355,7 +356,7 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
                 int cell_rules = rules;
                 if ((rules & (RULES_INPLACE | RULES_LAZY)) == RULES_INPLACE && A.c_src[ca] == SRC_SHARED)
                     cell_rules &= ~RULES_INPLACE;
-                cell_compute<OP, LAZY>(acc, pre, A.c_type[ca], B.c_type[cb], A.payload + A.c_off[ca],
+                cell_compute<OP, LAZY>(acc, A.c_type[ca], B.c_type[cb], A.payload + A.c_off[ca],
                              B.payload + B.c_off[cb], rawA & CARD_MASK, B.c_card[cb] & CARD_MASK,
                              A.c_len[ca], B.c_len[cb], slab + off, cap, lane, otype, ocard, olen,
                              &st->error, cell_rules, (rawA & CARD_UNKNOWN) != 0);
