@@ -132,8 +132,51 @@ constexpr int CLS_NONE = 0xff;
 constexpr int N_CLS = 8;
 
 // Key-major index of one many-way union (rb200_many2.cu): built per call on the device.
+//
+// Index entry of one participating container, 16 bytes:
+//   {payload offset / 16 (low 32 bits), input position, c_len, type | TF_* flags | (payload offset / 16) >> 32 << 8}
+constexpr uint32_t TF_FULL_RUN = 16, TF_FULL_BITSET = 32;   // the type takes the low 4 bits, the flags 2 more
+__host__ __device__ __forceinline__ uint32_t m2_tf(uint32_t type, uint32_t len, uint32_t card) {
+    uint32_t f = type;
+    if (type == T_RUN && len == 1 && card == 65536) f |= TF_FULL_RUN;
+    if (type == T_BITSET && card == 65536) f |= TF_FULL_BITSET;
+    return f;
+}
+__host__ __device__ __forceinline__ uint4 m2_entry(uint64_t off, uint32_t pos, uint32_t len, uint32_t tf) {
+    const uint64_t o16 = off >> 4;
+    return make_uint4((uint32_t)o16, pos, len, tf | (uint32_t)(o16 >> 32) << 8);
+}
+__host__ __device__ __forceinline__ uint64_t m2_entry_off(uint4 e) {
+    return (((uint64_t)(e.w >> 8) << 32) | e.x) << 4;
+}
+__host__ __device__ __forceinline__ uint32_t m2_entry_tf(uint4 e) { return e.w & 0xffu; }
+
+// Per-key counter of the index build (key_cu): participants in the high 32 bits, weight (stored
+// bytes) in the low 32 bits in units of 16 << w_shift bytes.  w_shift is the smallest shift that
+// keeps n * 2^13 >> w_shift below 2^32 (2^13 x 16 bytes is the largest container, a run container
+// of 32768 runs); it is 0 below 2^19 inputs.  Weights are rounded up (m2_weight), so a small
+// container still weighs at least one unit; one container weighs at most 2^(13 - w_shift) units, so
+// a key's weight stays below n * 2^(13 - w_shift) < 2^32 and never carries into its count.  The
+// weight only steers how keys are split into work units, never what they compute.
+__host__ __device__ __forceinline__ unsigned long long m2_cu(uint32_t count, uint32_t weight) {
+    return ((unsigned long long)count << 32) | weight;
+}
+__host__ __device__ __forceinline__ uint32_t m2_weight(uint32_t b16, uint32_t w_shift) {   // b16: 16-byte units
+    return (b16 + (1u << w_shift) - 1) >> w_shift;
+}
+__host__ __device__ __forceinline__ uint32_t m2_cu_count(unsigned long long cu) { return (uint32_t)(cu >> 32); }
+__host__ __device__ __forceinline__ uint32_t m2_cu_weight_kib(unsigned long long cu, uint32_t w_shift) {
+    return (uint32_t)(((cu & 0xffffffffull) << w_shift) >> 6);
+}
+inline uint32_t m2_weight_shift(uint64_t n) {   // n < 2^32
+    uint32_t s = 0;
+    while (((n << 13) >> s) >> 32) s++;
+    return s;
+}
+
 struct Many2Index {
-    unsigned long long *key_cu;  // [65536] participants << 40 | stored bytes / 16   (zero on entry)
+    unsigned long long *key_cu;  // [65536] m2_cu(participants, weight)   (zero on entry)
+    uint32_t w_shift;       // weight unit of key_cu: 16 << w_shift bytes
     uint32_t *key_count;    // [65536] participants per key (decoded by k_many2_scan)
     uint32_t *key_fill;     // [65536] fill cursors                    (zero on entry)
     uint32_t *key_start;    // [65536] first index entry of the key
@@ -144,7 +187,7 @@ struct Many2Index {
     unsigned long long *fold_first, *fold_second;   // [nk] order statistics of the fold (k_many2_fold)
     uint32_t *fold_F, *fold_L;                      // [nk]
     uint32_t *unit_ki;      // [max_units] work unit -> live key index
-    uint4 *ent;             // [entries] {payload offset / 16, input position, c_len, type | full flags}
+    uint4 *ent;             // [entries] m2_entry(payload offset, input position, c_len, type | flags)
 };
 
 // ---- single-pair fused path (rb200_fused.cu): packed input block (host-pinned -> device) and
@@ -189,15 +232,12 @@ void launch_pack(const SetView &S, uint32_t n, int elide, uint64_t *bytes, uint3
 void launch_pack_copy(const SetView &S, uint32_t n, int elide, const uint64_t *off, const uint64_t *beg,
                       SetOut out, cudaStream_t s);
 
-// or_many: mark -> compact keys -> reduce per key
+// xor_many: mark -> compact keys (then launch_xor_many)
 void launch_many_mark(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t key_lo,
                       uint32_t key_hi, uint32_t *flags /*65536*/, cudaStream_t s);
 void launch_many_compact(const uint32_t *flags, uint16_t *keys_out, OpStats *st, cudaStream_t s);
-void launch_or_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
-                    uint32_t want_slices, uint32_t *scratch_acc, uint32_t *scratch_tickets,
-                    uint32_t scratch_keys, SetOut out, uint32_t *card_per_key /*65536 or null*/,
-                    OpStats *st, int sms, cudaStream_t s);
 
+// or_many: key-major index, then one pass over the payloads (rb200_many2.cu)
 void launch_or_many2(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t key_lo, uint32_t key_hi,
                      const Many2Index &ix, uint32_t max_units, uint32_t *scratch, uint32_t *tickets,
                      uint32_t scratch_slots, SetOut out, uint32_t *card_per_key, OpStats *st, int sms,

@@ -52,7 +52,6 @@ constexpr uint8_t FLAG_COW = 1, FLAG_FROZEN = 2;  // roaring_types.h:46-49
 constexpr uint32_t SERIAL_COOKIE_NO_RUN = 12346, SERIAL_COOKIE = 12347;  // roaring_array.h:35-40
 constexpr int32_t NO_OFFSET_THRESHOLD = 4;
 constexpr uint32_t M2_SCRATCH_SLOTS = 2048, M2_SCRATCH_WORDS = 2 * ACC_WORDS + 32;  // rb200_many2.cu split keys
-constexpr uint32_t MANY_SCRATCH_KEYS = 4096;  // keys that may be split over several CTAs in or_many
 
 // ------------------------------------------------------------------ host allocation hooks
 // If the reference library is loaded in this process (drop-in deployment) every host object we
@@ -107,11 +106,10 @@ struct Ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evk0 = nullptr, evk1 = nullptr;
     OpStats *d_stats = nullptr;
     OpStats *h_stats = nullptr;  // pinned
-    uint32_t *d_flags = nullptr;   // 65536 key flags (or_many)
+    uint32_t *d_flags = nullptr;   // 65536 key flags (xor_many)
     uint16_t *d_keys = nullptr;    // 65536 compacted keys
     uint32_t *d_cardkey = nullptr; // 65536 per-key cardinalities
-    uint32_t *d_many_acc = nullptr, *d_many_tickets = nullptr;  // split-key scratch (kept zeroed)
-    // second-generation or_many (rb200_many2.cu): per-key tables + split-key scratch (kept zeroed)
+    // or_many (rb200_many2.cu): per-key tables + split-key scratch (kept zeroed)
     uint32_t *d_m2_tables = nullptr;   // 14 x 65536 u32: key_cu(2) | fill | count | units16 | fill | start | slices | scratch | unit_first | fold_first(2) | fold_second(2) | fold_F | fold_L
     uint32_t *d_m2_scratch = nullptr, *d_m2_tickets = nullptr;
     // single-pair fused path (rb200_fused.cu): packed operands (pinned + device), mapped result block
@@ -173,10 +171,6 @@ bool ctx_init(int device = -1) {
     CK(cudaMalloc(&g.d_flags, 65536 * sizeof(uint32_t)));
     CK(cudaMalloc(&g.d_keys, 65536 * sizeof(uint16_t)));
     CK(cudaMalloc(&g.d_cardkey, 65536 * sizeof(uint32_t)));
-    CK(cudaMalloc(&g.d_many_acc, (size_t)MANY_SCRATCH_KEYS * BITSET_BYTES));
-    CK(cudaMalloc(&g.d_many_tickets, MANY_SCRATCH_KEYS * sizeof(uint32_t)));
-    CK(cudaMemset(g.d_many_acc, 0, (size_t)MANY_SCRATCH_KEYS * BITSET_BYTES));
-    CK(cudaMemset(g.d_many_tickets, 0, MANY_SCRATCH_KEYS * sizeof(uint32_t)));
     CK(cudaMalloc(&g.d_m2_tables, 14 * 65536 * sizeof(uint32_t)));
     CK(cudaMalloc(&g.d_m2_scratch, (size_t)M2_SCRATCH_SLOTS * M2_SCRATCH_WORDS * sizeof(uint32_t)));
     CK(cudaMalloc(&g.d_m2_tickets, M2_SCRATCH_SLOTS * sizeof(uint32_t)));
@@ -1534,7 +1528,7 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
     return ok ? 0 : -1;
 }
 
-// Sharded form: after k_or_many the per-key cardinalities of [span_lo, span_hi] are all-reduced
+// Sharded form: after k_or_many2 the per-key cardinalities of [span_lo, span_hi] are all-reduced
 // across the communicator ON THE DEVICE (one ncclAllReduce on the library stream), then that
 // span alone (4 * K bytes) is read back.
 struct ShardArgs {
@@ -1559,12 +1553,17 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     if (reject_lazy(S, "or_many")) return nullptr;
     if (!ensure_mirrors(S)) return nullptr;
     if (idx == nullptr) n = S->n_bitmaps;
+    // the index (rb200_many2.cu) holds input positions, per-key segments and counts in 32 bits; its
+    // entry buffer is sized for every container of the inputs (the host has no per-bitmap keys to
+    // count only those of [key_lo, key_hi]), so the container limit covers them all
+    if (n > 0xffffffffu) { t_err = "or_many: more than 2^32 - 1 inputs"; return nullptr; }
     uint64_t tot = 0;
     for (size_t i = 0; i < n; i++) {
         const uint32_t b = idx ? idx[i] : (uint32_t)i;
         if (b >= S->n_bitmaps) { t_err = "or_many: index out of range"; return nullptr; }
         tot += S->h_cnt[b];
     }
+    if (tot > 0xffffffffu) { t_err = "or_many: the inputs carry more than 2^32 - 1 containers (every key counts, whatever the key range)"; return nullptr; }
     uint64_t maxk = key_lo <= key_hi ? (uint64_t)key_hi - key_lo + 1 : 0;
     if (tot < maxk) maxk = tot;
     rb200_set *R = set_new(1, maxk, maxk * BITSET_BYTES);
@@ -1584,10 +1583,7 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     cudaEvent_t evc0 = nullptr, evc1 = nullptr;
     if (ok && want_ck) { h_ck = (uint32_t *)pin_alloc(65536 * 4); ok = h_ck != nullptr; }
     if (ok && sh) { evc0 = ev_get(); evc1 = ev_get(); ok = evc0 && evc1; }
-    static const bool env_v1 = []() { const char *e = getenv("RB200_OR_MANY"); return e && !strcmp(e, "v1"); }();
-    // the index packs payload offsets / 16 into 32 bits and participants per key into 24
-    const bool use_v1 = env_v1 || S->slab_used >= (64ull << 30) || n >= (1u << 22);
-    // index of the second-generation kernel: entries + work-unit table from the device pool
+    // index: entries + work-unit table from the device pool
     uint64_t tot_kib = 0;
     for (size_t i = 0; i < n; i++) tot_kib += (S->h_bytes[idx ? idx[i] : i] >> 10) + 1;
     const uint64_t max_units = std::max<uint64_t>(1, std::min<uint64_t>(tot, std::min<uint64_t>(65536, tot) + tot_kib / 32 + 1));
@@ -1596,13 +1592,14 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     const size_t tab_bytes = m2_chunks > 1 && m2_chunks <= M2W_MAX_CHUNKS ? (size_t)2048 * m2_chunks * 32 * 4 : 0;
     const size_t e_bytes = al256(16 * tot) + al256(4 * max_units) + al256(tab_bytes);
     uint8_t *d_index = nullptr;
-    if (ok && !use_v1) { d_index = (uint8_t *)dev_alloc(e_bytes); ok = d_index != nullptr; }
-    if (ok && !use_v1) {
+    if (ok) { d_index = (uint8_t *)dev_alloc(e_bytes); ok = d_index != nullptr; }
+    if (ok) {
         cudaEventRecord(g.ev0, g.stream);
         ok = stats_reset();
         const SetView vs = S->view();
         Many2Index ix;
         ix.key_cu = (unsigned long long *)g.d_m2_tables;          // [0, 2): zeroed per call
+        ix.w_shift = m2_weight_shift(n);
         ix.key_fill = g.d_m2_tables + 2 * 65536;                  // [2, 3): zeroed per call
         ix.key_count = g.d_m2_tables + 3 * 65536;
         ix.key_start = g.d_m2_tables + 4 * 65536;
@@ -1627,30 +1624,10 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         const bool window_index = m2_chunks <= M2W_MAX_CHUNKS && n > 0 && (win_env >= 0 ? win_env != 0 : (tot >= 64 * (uint64_t)n));
         cudaMemsetAsync(g.d_m2_tables, 0, 3 * 65536 * sizeof(uint32_t), g.stream);
         if (want_ck) cudaMemsetAsync(g.d_cardkey, 0, 65536 * 4, g.stream);
-        launch_or_many2(vs, d_idx, (uint32_t)n, key_lo, key_hi, ix, (uint32_t)std::min<uint64_t>(max_units, 0xffffffffu),
+        launch_or_many2(vs, d_idx, (uint32_t)n, key_lo, key_hi, ix, (uint32_t)max_units,
                         g.d_m2_scratch, g.d_m2_tickets, M2_SCRATCH_SLOTS, R->out(), want_ck ? g.d_cardkey : nullptr,
                         g.d_stats, g.sms, g.stream, g.evk0, use_tma, window_index,
                         (uint32_t *)(d_index + al256(16 * tot) + al256(4 * max_units)));
-    }
-    if (ok && use_v1) {
-        cudaEventRecord(g.ev0, g.stream);
-        ok = stats_reset();
-        const SetView vs = S->view();
-        launch_many_mark(vs, d_idx, (uint32_t)n, key_lo, key_hi, g.d_flags, g.stream);
-        launch_many_compact(g.d_flags, g.d_keys, g.d_stats, g.stream);
-        if (want_ck) cudaMemsetAsync(g.d_cardkey, 0, 65536 * 4, g.stream);
-        cudaEventRecord(g.evk0, g.stream);
-        // few keys x many bitmaps: split every key over several CTAs (partial unions merged in a
-        // global scratch accumulator); the estimate of the key count is the largest directory
-        uint32_t nk_est = 1;
-        for (size_t i = 0; i < n; i++) nk_est = std::max(nk_est, S->h_cnt[idx ? idx[i] : i]);
-        uint32_t slices = (uint32_t)((4ull * g.sms + nk_est - 1) / nk_est);
-        slices = std::min<uint32_t>(slices, 16u);
-        slices = std::min<uint32_t>(slices, (uint32_t)(n / 32));
-        if (slices < 1) slices = 1;
-        launch_or_many(vs, d_idx, (uint32_t)n, g.d_keys, slices, g.d_many_acc, g.d_many_tickets,
-                       MANY_SCRATCH_KEYS, R->out(), want_ck ? g.d_cardkey : nullptr, g.d_stats,
-                       g.sms, g.stream);
     }
     if (ok) {
         cudaEventRecord(g.evk1, g.stream);

@@ -6,7 +6,7 @@
 //                   work units: a key whose participants weigh more than SLICE_BYTES is split
 //                   into several units (slices of its participant list) merged through a global
 //                   scratch accumulator
-//   k_many2_fill    index entries {input position, container, type|flags}, grouped by key
+//   k_many2_fill    index entries (m2_entry, rb200_common.h), grouped by key
 //                   (order inside a key is arbitrary: nothing below needs it)
 //   k_or_many2      work unit = (key, slice): the participants' payloads are staged into shared
 //                   memory by TMA bulk copies (cp.async.bulk + one mbarrier per half of a 64 KiB
@@ -42,23 +42,18 @@ constexpr int M2_THREADS = 256;
 constexpr int M2_STAGE = 256;                    // index entries staged per round
 constexpr uint32_t M2_SLICE_BYTES = 384u << 10;  // payload bytes per work unit before a key is split
 constexpr uint32_t M2_MAX_SLICES = 64;
-constexpr uint32_t TF_FULL_RUN = 16, TF_FULL_BITSET = 32;
 constexpr uint32_t POS_NONE = 0xffffffffu;
 #ifndef RB200_M2_FLAT_VECS
 #define RB200_M2_FLAT_VECS 513
 #endif
+// Arrays of at least RB200_M2_MERGE_MIN values would merge same-word bits before the atomic.  Only
+// arrays below 8 * M2_FLAT_VECS values reach that test, so with this default the merging arm never
+// runs; deleting it still changes how the direct path of k_or_many2 is compiled and made that path
+// ~4 % slower on configs[2] (H100 80GB HBM3, 700 W), so it stays until the flat list is retuned.
 #ifndef RB200_M2_MERGE_MIN
-#define RB200_M2_MERGE_MIN 100000   // arrays of at least this many values merge same-word bits before the atomic
+#define RB200_M2_MERGE_MIN 100000
 #endif
 constexpr uint32_t M2_FLAT_VECS = RB200_M2_FLAT_VECS;   // arrays below this many 16-byte vectors go through the flat list
-
-__device__ __forceinline__ uint32_t entry_tf(const SetView &S, uint32_t c) {
-    const uint32_t t = S.c_type[c], l = S.c_len[c], cd = S.c_card[c] & CARD_MASK;
-    uint32_t f = t;
-    if (t == T_RUN && l == 1 && cd == 65536) f |= TF_FULL_RUN;
-    if (t == T_BITSET && cd == 65536) f |= TF_FULL_BITSET;
-    return f;
-}
 
 // ------------------------------------------------------------------------------ index
 __global__ void __launch_bounds__(128)
@@ -73,8 +68,8 @@ k_many2_count(SetView S, const uint32_t *__restrict__ idx, uint32_t n, uint32_t 
         for (uint32_t c = lane; c < nc; c += 32) {
             const uint32_t k = S.c_key[c0 + c];
             if (k < key_lo || k > key_hi) continue;
-            // one atomic per container: participants in the high 24 bits, stored bytes / 16 in the low 40
-            atomicAdd(ix.key_cu + k, (1ull << 40) | (unsigned long long)(round16(stored_bytes(S.c_type[c0 + c], S.c_len[c0 + c])) >> 4));
+            // one atomic per container
+            atomicAdd(ix.key_cu + k, m2_cu(1, m2_weight(round16(stored_bytes(S.c_type[c0 + c], S.c_len[c0 + c])) >> 4, ix.w_shift)));
         }
     }
 }
@@ -185,17 +180,13 @@ k_many2_window(SetView S, const uint32_t *__restrict__ idx, uint32_t n, uint32_t
                 atomicAdd(&s_cnt[k - k0], 1u);
                 atomicAdd(&s_b16[k - k0], round16(stored_bytes(t, l)) >> 4);
             } else {
-                const uint32_t cd = S.c_card[cix] & CARD_MASK;
-                uint32_t f = t;
-                if (t == T_RUN && l == 1 && cd == 65536) f |= TF_FULL_RUN;
-                if (t == T_BITSET && cd == 65536) f |= TF_FULL_BITSET;
                 const uint32_t slot = s_start[k - k0] + atomicAdd(&s_cnt[k - k0], 1u);
-                ix.ent[slot] = make_uint4((uint32_t)(S.c_off[cix] >> 4), base + q, l, f);
+                ix.ent[slot] = m2_entry(S.c_off[cix], base + q, l, m2_tf(t, l, S.c_card[cix] & CARD_MASK));
             }
         }
         __syncthreads();
         if (!FILL && tid < M2W_KEYS && k0 + tid <= 65535u) {
-            const unsigned long long packed = ((unsigned long long)s_cnt[tid] << 40) | s_b16[tid];
+            const unsigned long long packed = m2_cu(s_cnt[tid], m2_weight(s_b16[tid], ix.w_shift));
             if (nchunks == 1) {
                 ix.key_cu[k0 + tid] = packed;
             } else {
@@ -208,10 +199,10 @@ k_many2_window(SetView S, const uint32_t *__restrict__ idx, uint32_t n, uint32_t
 }
 
 // single CTA, 1024 threads: tiles of 4096 keys, 4 consecutive keys per thread (coalesced), running carries
-__device__ __forceinline__ uint32_t key_units(unsigned long long cu, uint32_t slice_kib) {
-    const uint32_t c = (uint32_t)(cu >> 40);
+__device__ __forceinline__ uint32_t key_units(unsigned long long cu, uint32_t w_shift, uint32_t slice_kib) {
+    const uint32_t c = m2_cu_count(cu);
     if (!c) return 0;
-    const uint32_t kib = (uint32_t)((cu & ((1ull << 40) - 1)) >> 6);
+    const uint32_t kib = m2_cu_weight_kib(cu, w_shift);
     uint32_t s = (kib + slice_kib - 1) / slice_kib;
     const uint32_t by_cnt = (c + 3) >> 2;
     if (s > by_cnt) s = by_cnt;
@@ -233,8 +224,8 @@ k_many2_scan(Many2Index ix, uint32_t scratch_slots, uint32_t max_units, uint32_t
     for (uint32_t t = 0; t < ntiles; t++) {
         const ulonglong2 *p = reinterpret_cast<const ulonglong2 *>(ix.key_cu + t * 4096 + tid * 4);
         const ulonglong2 a = p[0], b = p[1];
-        const unsigned long long M = (1ull << 40) - 1;
-        w16 += (uint32_t)((a.x & M) >> 6) + (uint32_t)((a.y & M) >> 6) + (uint32_t)((b.x & M) >> 6) + (uint32_t)((b.y & M) >> 6);   // KiB, to stay inside 32 bits
+        const uint32_t ws = ix.w_shift;
+        w16 += m2_cu_weight_kib(a.x, ws) + m2_cu_weight_kib(a.y, ws) + m2_cu_weight_kib(b.x, ws) + m2_cu_weight_kib(b.y, ws);   // KiB, to stay inside 32 bits
     }
     w16 = __reduce_add_sync(FULLMASK, w16);
     if (lane == 0) s_w[wid][0] = w16;
@@ -268,8 +259,8 @@ k_many2_scan(Many2Index ix, uint32_t scratch_slots, uint32_t max_units, uint32_t
         uint32_t cnt = 0, live = 0, units = 0, nsplit = 0;
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            c[k] = (uint32_t)(cu[k] >> 40);
-            s[k] = key_units(cu[k], slice_kib);
+            c[k] = m2_cu_count(cu[k]);
+            s[k] = key_units(cu[k], ix.w_shift, slice_kib);
             cnt += c[k];
             live += c[k] ? 1u : 0u;
             units += s[k];
@@ -333,8 +324,8 @@ k_many2_fill(SetView S, const uint32_t *__restrict__ idx, uint32_t n, uint32_t k
             const uint32_t k = S.c_key[c0 + c];
             if (k < key_lo || k > key_hi) continue;
             const uint32_t slot = ix.key_start[k] + atomicAdd(ix.key_fill + k, 1u);
-            // {payload offset / 16, input position, length, type flags}: ONE 16-byte store
-            ix.ent[slot] = make_uint4((uint32_t)(S.c_off[c0 + c] >> 4), i, S.c_len[c0 + c], entry_tf(S, c0 + c));
+            const uint32_t l = S.c_len[c0 + c];
+            ix.ent[slot] = m2_entry(S.c_off[c0 + c], i, l, m2_tf(S.c_type[c0 + c], l, S.c_card[c0 + c] & CARD_MASK));   // ONE 16-byte store
         }
     }
 }
@@ -356,7 +347,7 @@ k_many2_fold(Many2Index ix, const OpStats *st) {
         unsigned long long m1 = ~0ull, m2 = ~0ull;
         for (uint32_t e = lane; e < m; e += 32) {
             const uint4 en = ix.ent[e0 + e];
-            const unsigned long long v = ((unsigned long long)en.y << 8) | en.w;
+            const unsigned long long v = ((unsigned long long)en.y << 8) | m2_entry_tf(en);
             if (v < m1) { m2 = m1; m1 = v; }
             else if (v < m2) m2 = v;
         }
@@ -380,14 +371,14 @@ k_many2_fold(Many2Index ix, const OpStats *st) {
             for (uint32_t e = lane; e < m; e += 32) {
                 const uint4 en = ix.ent[e0 + e];
                 const uint32_t p = en.y;
-                if (p > inplace_from && (en.w & TF_FULL_RUN)) f = min(f, p);
+                if (p > inplace_from && (m2_entry_tf(en) & TF_FULL_RUN)) f = min(f, p);
             }
             F = __reduce_min_sync(FULLMASK, f);
             uint32_t l = 0;   // position + 1, 0 = none
             for (uint32_t e = lane; e < m; e += 32) {
                 const uint4 en = ix.ent[e0 + e];
                 const uint32_t p = en.y;
-                if (p > inplace_from && p < F && (en.w & 15) == T_BITSET) l = max(l, p + 1);
+                if (p > inplace_from && p < F && (m2_entry_tf(en) & 15) == T_BITSET) l = max(l, p + 1);
             }
             l = __reduce_max_sync(FULLMASK, l);
             if (l) L = l - 1;
@@ -409,8 +400,8 @@ struct Many2Smem {
     uint32_t acc[ACC_WORDS];    // union of the inputs up to L (or of all of them when L is not needed)
     uint32_t acc2[ACC_WORDS];   // union of the inputs after L
     uint64_t bar[2];            // mbarriers of the two halves: "the bytes have landed"
-    uint64_t ebar[2];           // RB200_M2_PIPE: "all eight warps are done with the half"
-    uint32_t h_last[2];         // RB200_M2_PIPE: the half holds the last entries of the round
+    uint64_t ebar[2];           // mbarriers of the two halves: "all eight warps are done with the half"
+    uint32_t h_last[2];         // the half holds the last entries of the round
     uint16_t h_bs[2][M2_HALF_ENTRIES], h_ar[2][M2_HALF_ENTRIES];   // staged bitsets / arrays+runs of a half (entry ids)
     uint32_t h_soff[M2_STAGE];  // byte offset of a staged entry inside its half
     uint32_t h_nbs[2], h_nar[2], h_big[2];
@@ -446,9 +437,6 @@ __device__ __forceinline__ unsigned long long block_min64(Many2Smem &sm, unsigne
 
 // TMA = true: operands staged by bulk copies (bitset-dominated inputs); false: direct global loads
 // (array-dominated inputs, where a bulk copy per small container costs more than it hides)
-#ifndef RB200_M2_PIPE
-#define RB200_M2_PIPE 1   // 1: warp-level full / empty mbarrier pipeline in the TMA path (no block barrier per half); 0: block barrier per half
-#endif
 #ifndef RB200_M2_MINB
 #define RB200_M2_MINB 4   // resident CTAs per SM of the direct path (register budget 64 at 4)
 #endif
@@ -469,7 +457,7 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
         mbar_fence_init();
     }
     uint32_t ph0 = 0, ph1 = 0;   // phase parity of the two staging halves (every thread tracks both)
-    uint32_t fills0 = 0, fills1 = 0;   // RB200_M2_PIPE: fills issued per half (thread 0)
+    uint32_t fills0 = 0, fills1 = 0;   // fills issued per half (thread 0)
     __syncthreads();
     if (tid == 0) sm.unit = (uint32_t)atomicAdd(&st->work_counter2, 1ull);
     for (;;) {
@@ -528,8 +516,8 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
             uint32_t my_vec = 0;
             if (tid < M2_STAGE && e < s_hi) {
                 const uint4 en = ix.ent[e0 + e];
-                const uint32_t tf = en.w, p = en.y;
-                sm.s_off[tid] = (unsigned long long)en.x << 4;
+                const uint32_t tf = m2_entry_tf(en), p = en.y;
+                sm.s_off[tid] = m2_entry_off(en);
                 sm.s_len[tid] = en.z;
                 sm.s_pos[tid] = p;
                 sm.s_tf[tid] = (uint8_t)tf;
@@ -618,7 +606,6 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
                 }
                 continue;
             }
-#if RB200_M2_PIPE
             // ---- two-half pipeline without block-wide barriers: thread 0 is the producer (packs entries
             // into a half, arms its "full" mbarrier with the byte count, issues the bulk copies); every
             // warp consumes a half as soon as its bytes have landed and then arrives on the half's
@@ -702,93 +689,6 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
                 __syncwarp();
                 if (last) break;
             }
-#else
-            // ---- two-half pipeline: thread 0 packs the next entries of the round into a half and
-            // issues their bulk copies; everybody consumes the other half meanwhile
-            uint32_t next = 0;   // next entry of the round to stage (thread 0's cursor, kept uniform)
-            auto issue = [&](int h) {
-                // (executed by every thread so that `next` stays uniform; only thread 0 touches the
-                //  tables, the barrier and the copy engine)
-                uint32_t bytes = 0, nbs = 0, nar = 0, big = POS_NONE;
-                while (next < R && nbs + nar < M2_HALF_ENTRIES) {
-                    const uint32_t tf = sm.s_tf[next], t = tf & 15;
-                    const uint32_t sz = (tf & TF_FULL_RUN) ? 0u : round16(stored_bytes((int)t, sm.s_len[next]));
-                    if (sz > M2_HALF) {   // an oversized run container (unoptimised input): straight from global
-                        if (nbs + nar == 0 && big == POS_NONE) { big = next; next++; }
-                        break;
-                    }
-                    if (bytes + sz > M2_HALF) break;
-                    if (tid == 0) {
-                        sm.h_soff[next] = bytes;
-                        if (sz) {
-                            if (t == T_BITSET) sm.h_bs[h][nbs] = (uint16_t)next;
-                            else sm.h_ar[h][nar] = (uint16_t)next;
-                        }
-                    }
-                    if (sz) { if (t == T_BITSET) nbs++; else nar++; }
-                    bytes += sz;
-                    next++;
-                }
-                if (tid == 0) {
-                    sm.h_nbs[h] = nbs;
-                    sm.h_nar[h] = nar;
-                    sm.h_big[h] = big;
-                    mbar_arrive_expect_tx(&sm.bar[h], bytes);
-                    for (uint32_t k = 0; k < nbs; k++) {
-                        const uint32_t q = sm.h_bs[h][k];
-                        bulk_copy_g2s(ring[h] + sm.h_soff[q], S.payload + sm.s_off[q], BITSET_BYTES, &sm.bar[h]);
-                    }
-                    for (uint32_t k = 0; k < nar; k++) {
-                        const uint32_t q = sm.h_ar[h][k];
-                        bulk_copy_g2s(ring[h] + sm.h_soff[q], S.payload + sm.s_off[q],
-                                      round16(stored_bytes(sm.s_tf[q] & 15, sm.s_len[q])), &sm.bar[h]);
-                    }
-                }
-            };
-            uint32_t staged = 0;      // halves issued and not yet consumed
-            issue(0);
-            staged++;
-            if (next < R) { issue(1); staged++; }
-            int h = 0;
-            while (staged) {
-                mbar_wait(&sm.bar[h], h ? ph1 : ph0);
-                if (h) ph1 ^= 1; else ph0 ^= 1;
-                // bitsets of the half: registers <- shared (all of them are <= L), two at a time
-                const uint32_t nbs = sm.h_nbs[h], nar = sm.h_nar[h];
-                for (uint32_t j = 0; j < nbs; j += 2) {
-                    const uint4 *s0 = reinterpret_cast<const uint4 *>(ring[h] + sm.h_soff[sm.h_bs[h][j]]);
-                    const uint4 a0 = s0[tid], b0 = s0[tid + M2_THREADS];
-                    r0.x |= a0.x; r0.y |= a0.y; r0.z |= a0.z; r0.w |= a0.w;
-                    r1.x |= b0.x; r1.y |= b0.y; r1.z |= b0.z; r1.w |= b0.w;
-                    if (j + 1 < nbs) {
-                        const uint4 *s1 = reinterpret_cast<const uint4 *>(ring[h] + sm.h_soff[sm.h_bs[h][j + 1]]);
-                        const uint4 a1 = s1[tid], b1 = s1[tid + M2_THREADS];
-                        r0.x |= a1.x; r0.y |= a1.y; r0.z |= a1.z; r0.w |= a1.w;
-                        r1.x |= b1.x; r1.y |= b1.y; r1.z |= b1.z; r1.w |= b1.w;
-                    }
-                }
-                // arrays and runs: one warp per container, shared-memory atomics on the accumulator
-                for (uint32_t j = wid; j < nar; j += M2_THREADS / 32) {
-                    const uint32_t q = sm.h_ar[h][j];
-                    uint32_t *dst = (L != POS_NONE && sm.s_pos[q] > L) ? sm.acc2 : sm.acc;
-                    const uint8_t *p = ring[h] + sm.h_soff[q];
-                    if ((sm.s_tf[q] & 15) == T_ARRAY) acc_apply_array_s<0>(dst, p, sm.s_len[q], lane);
-                    else acc_apply_runs_s<0, true>(dst, p, sm.s_len[q], lane);
-                }
-                const uint32_t big = sm.h_big[h];
-                if (big != POS_NONE) {   // oversized run container: every warp takes a share, from global
-                    uint32_t *dst = (L != POS_NONE && sm.s_pos[big] > L) ? sm.acc2 : sm.acc;
-                    const uint32_t nr = sm.s_len[big], per_w = (nr + M2_THREADS / 32 - 1) / (M2_THREADS / 32);
-                    const uint32_t r_lo = min((uint32_t)wid * per_w, nr), r_hi = min(r_lo + per_w, nr);
-                    if (r_hi > r_lo)
-                        acc_apply_runs<0, true>(dst, S.payload + sm.s_off[big] + 4ull * r_lo, r_hi - r_lo, lane);
-                }
-                __syncthreads();   // the half is free again
-                staged--;
-                if (next < R) { issue(h); staged++; }
-                h ^= 1;
-            }
-#endif
         }
         __syncthreads();
         anyfull = __syncthreads_or(anyfull);

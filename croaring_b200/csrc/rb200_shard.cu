@@ -4,7 +4,7 @@
 //     the process — torch's — or the system one), so libroaring_b200.so has no link-time
 //     dependency on it and single-GPU users never load it.  The only collective of the path is
 //     ONE ncclAllReduce(sum) over the per-key result cardinalities uint32[K] (K = keys between the
-//     first and the last live key), issued on the library's stream right behind k_or_many — the
+//     first and the last live key), issued on the library's stream right behind k_or_many2 — the
 //     counters never leave the device before they are reduced.
 //   * Host-side key-range planning and slicing of portable-serialized bitmaps
 //     (format: /root/reference/src/roaring_array.c:469-531), plain C ABI, no CUDA involved:

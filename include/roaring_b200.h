@@ -372,7 +372,7 @@ int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_
 uint64_t rb200_last_algorithmic_bytes(void);
 /* Device time (ms) of the last batch / many op, measured with CUDA events on its stream. */
 float rb200_last_device_ms(void);
-/* Device time (ms) of the grid-cell kernel (k_compute_items / k_card_items / k_or_many) alone. */
+/* Device time (ms) of the grid-cell kernel (k_compute_items / k_card_items / k_or_many2) alone. */
 float rb200_last_compute_ms(void);
 /* Bytes copied device->host by the last rb200_set_download* call (directory + payload slab). */
 uint64_t rb200_last_download_bytes(void);

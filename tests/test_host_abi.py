@@ -97,6 +97,12 @@ int main() {
     return bad;
 }
 '''
+    out = _run_probe(src)
+    assert out.returncode == 0, out.stdout
+
+
+def _run_probe(src):
+    """Compile a host-side probe against the library's headers with nvcc and run it."""
     import tempfile
     with tempfile.TemporaryDirectory() as td:
         cu = os.path.join(td, "probe.cu")
@@ -105,8 +111,79 @@ int main() {
         subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-std=c++17", "--expt-relaxed-constexpr",
                                "-gencode", "arch=compute_90a,code=sm_90a",
                                "-I", os.path.join(ROOT, "croaring_b200", "csrc"), cu, "-o", exe])
-        out = subprocess.run([exe], capture_output=True, text=True)
-        assert out.returncode == 0, out.stdout
+        return subprocess.run([exe], capture_output=True, text=True)
+
+
+def test_many2_index_formats_round_trip():
+    """The N-way union's index entry (m2_entry) and per-key counter (m2_cu) are host+device helpers:
+    payload offsets of 64 GiB and more, every type / flag combination, participant counts above 2^24
+    and weights at every w_shift boundary survive packing and unpacking."""
+    src = r'''
+#include "rb200_common.h"
+#include <cstdio>
+using namespace rb200;
+int bad = 0;
+#define CHECK(c) do { if (!(c)) { printf("FAIL line %d: %s\n", __LINE__, #c); bad++; } } while (0)
+int main() {
+    const uint64_t offs[] = {0, (1ull << 36) - 16, 1ull << 36, (1ull << 40) + 16, (1ull << 60) - 16};
+    const uint32_t poss[] = {0, 1, (1u << 24) + 1, 0xffffffffu};
+    for (uint64_t off : offs)
+        for (uint32_t pos : poss)
+            for (uint32_t t = T_BITSET; t <= T_RUN; t++)
+                for (uint32_t fl = 0; fl < 4; fl++) {
+                    const uint32_t tf = t | (fl & 1 ? TF_FULL_RUN : 0) | (fl & 2 ? TF_FULL_BITSET : 0);
+                    const uint4 e = m2_entry(off, pos, 4096, tf);
+                    CHECK(m2_entry_off(e) == off);
+                    CHECK(m2_entry_tf(e) == tf);
+                    CHECK(e.y == pos && e.z == 4096);
+                    const unsigned long long v = ((unsigned long long)e.y << 8) | m2_entry_tf(e);   // k_many2_fold's order key
+                    CHECK((uint32_t)(v >> 8) == pos && (uint32_t)(v & 0xff) == tf);
+                }
+    CHECK(m2_tf(T_RUN, 1, 65536) == (T_RUN | TF_FULL_RUN));
+    CHECK(m2_tf(T_BITSET, 1024, 65536) == (T_BITSET | TF_FULL_BITSET));
+    CHECK(m2_tf(T_RUN, 2, 65535) == T_RUN && m2_tf(T_BITSET, 1024, 65535) == T_BITSET);
+    CHECK(m2_tf(T_ARRAY, 4096, 4096) == T_ARRAY);
+
+    const uint32_t counts[] = {0, 1, (1u << 24) - 1, 1u << 24, (1u << 24) + 1, 0xffffffffu};
+    for (uint32_t c : counts)
+        for (uint32_t w : {0u, 1u, 0x12345678u, 0xffffffffu}) {
+            const unsigned long long cu = m2_cu(c, w);
+            CHECK(m2_cu_count(cu) == c && (uint32_t)cu == w);
+        }
+    // w_shift: the smallest shift that keeps n * 2^13 >> w_shift below 2^32; 0 below 2^19 inputs
+    const uint64_t ns[] = {1, (1u << 19) - 1, 1u << 19, (1u << 19) + 1, 1u << 20, (1u << 24) + 1, (1u << 25) - 1,
+                           1u << 25, 0xffffffffu};
+    for (uint64_t n : ns) {
+        const uint32_t s = m2_weight_shift(n);
+        CHECK(((n << 13) >> s) < (1ull << 32));
+        CHECK(s == 0 || ((n << 13) >> (s - 1)) >= (1ull << 32));
+        CHECK((s == 0) == (n < (1u << 19)));
+        // n inputs each bringing the largest container (2^13 x 16 bytes) to one key, one atomic each:
+        // the weights never carry into the count
+        CHECK(m2_weight(1u << 13, s) == (1u << 13) >> s);
+        const unsigned long long tot = n * m2_cu(1, m2_weight(1u << 13, s));
+        CHECK(m2_cu_count(tot) == n);
+        CHECK((uint32_t)tot == (uint32_t)(n * ((1u << 13) >> s)));
+        if (n < (1u << 25)) CHECK(m2_cu_weight_kib(tot, s) == n * 128);   // 128 KiB each
+        // n inputs of one 16-byte unit each (arrays of <= 8 values) still weigh something, so such a
+        // key is split over work units as it was with exact weights
+        const unsigned long long small = n * m2_cu(1, m2_weight(1, s));
+        CHECK(m2_cu_count(small) == n && (uint32_t)small == n);
+    }
+    for (uint32_t s = 0; s <= 13; s++) {   // every w_shift an n < 2^32 can need
+        CHECK(m2_weight(0, s) == 0);
+        CHECK(m2_weight(1, s) == 1);   // rounded up: a small container keeps a nonzero weight
+        CHECK(m2_weight((1u << s) + 1, s) == 2);
+        CHECK(m2_weight(1u << 21, s) == (1u << 21) >> s);   // a window's sum: 256 of the largest containers
+    }
+    CHECK(m2_weight_shift((1u << 24) + 1) == 6);
+    CHECK(m2_cu_weight_kib(m2_cu(3, 64 * 5), 0) == 5);   // w_shift 0: the weight is stored bytes / 16
+    printf("bad=%d\n", bad);
+    return bad;
+}
+'''
+    out = _run_probe(src)
+    assert out.returncode == 0, out.stdout
 
 
 def test_compute_fails_loudly_without_gpu():

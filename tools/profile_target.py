@@ -3,7 +3,7 @@
 
   pairs   : weather_sept_85 all-pairs OR  (k_plan_pairs, k_compute_items, k_finalize_pairs)
   card    : config[3] shape: bitset-heavy and_cardinality, 2000 pairs (k_card_items)
-  many    : or_many over weather_sept_85 + a dense synthetic set (k_or_many)
+  many    : or_many over weather_sept_85 + a dense synthetic set (k_many2_*, k_or_many2)
 """
 import sys
 import os
