@@ -82,6 +82,49 @@ struct SetOut {
     uint8_t *payload;
 };
 
+// Cell descriptor of one pairwise work item: everything k_compute_items needs to run the cell or
+// the pass-through copy, so that a warp fetches one 32-byte record instead of walking
+// item -> container -> payload.  Two uint4:
+//   a = {A payload offset / 16, B payload offset / 16, output slot offset / 16  (low 32 bits each), item id}
+//   b.x  cA as stored (CARD_UNKNOWN included)
+//   b.y  cB (17 bits) | tA << 17 | tB << 19 | kind << 21 | SHARED left << 23 | (A offset / 16) >> 32 << 24
+//   b.z  lA | lB << 16   (at most 32768 runs or 4096 values)
+//   b.w  slot capacity / 16 (16 bits) | (B offset / 16) >> 32 << 16 | (slot offset / 16) >> 32 << 24
+// Offsets are 16-byte aligned and below 2^44 bytes (16 TiB, more than any device allocation); the
+// capacity is at most 4 x 65536 bytes (slot_bound_lazy of two run containers).  A pass-through item
+// keeps its source container (of A or B, by kind) in the A fields and leaves the B fields zero;
+// a hole is all zero (kind K_HOLE).
+struct CellDesc {
+    uint64_t offA, offB, off;   // payload offsets of A / B (or the copy's source), output slot offset
+    uint32_t item, cA, cB, lA, lB, cap;
+    uint32_t tA, tB, kind;
+    bool shared;                // the in-place twins' left container is SHARED: take the functional cell
+};
+__host__ __device__ __forceinline__ void cd_pack(const CellDesc &d, uint4 &a, uint4 &b) {
+    const uint64_t oA = d.offA >> 4, oB = d.offB >> 4, oO = d.off >> 4;
+    a = make_uint4((uint32_t)oA, (uint32_t)oB, (uint32_t)oO, d.item);
+    b = make_uint4(d.cA,
+                   d.cB | d.tA << 17 | d.tB << 19 | d.kind << 21 | (d.shared ? 1u : 0u) << 23 | (uint32_t)(oA >> 32) << 24,
+                   d.lA | d.lB << 16, (d.cap >> 4) | (uint32_t)(oB >> 32) << 16 | (uint32_t)(oO >> 32) << 24);
+}
+__host__ __device__ __forceinline__ CellDesc cd_unpack(uint4 a, uint4 b) {
+    CellDesc d;
+    d.offA = ((uint64_t)(b.y >> 24) << 32 | a.x) << 4;
+    d.offB = ((uint64_t)((b.w >> 16) & 0xffu) << 32 | a.y) << 4;
+    d.off = ((uint64_t)(b.w >> 24) << 32 | a.z) << 4;
+    d.item = a.w;
+    d.cA = b.x;
+    d.cB = b.y & 0x1ffffu;
+    d.tA = (b.y >> 17) & 3u;
+    d.tB = (b.y >> 19) & 3u;
+    d.kind = (b.y >> 21) & 3u;
+    d.shared = (b.y >> 23) & 1u;
+    d.lA = b.z & 0xffffu;
+    d.lB = b.z >> 16;
+    d.cap = (b.w & 0xffffu) << 4;
+    return d;
+}
+
 // Work items of one batched pairwise op (SoA, W entries; items of pair p occupy
 // [item_off[p], item_off[p+1]) in key order with holes).
 struct Items {
@@ -90,9 +133,9 @@ struct Items {
     uint32_t *ca;        // container index in A (K_COMPUTE, K_COPY_A)
     uint32_t *cb;        // container index in B (K_COMPUTE, K_COPY_B)
     uint64_t *slot_off;  // byte offset of the output slot in the result slab
-    uint32_t *slot_cap;  // bytes reserved (upper bound on the result payload, 16-B multiple)
     uint8_t *cls;        // code-path class of the item (CLS_*), CLS_NONE for holes
-    uint32_t *order;     // item ids sorted by class (null: tickets walk the items in place)
+    uint4 *desc;         // [2 W] cell descriptors in item order (cd_pack; null: cardinality-only sweeps)
+    uint4 *desc_cls;     // [2 W] the live items' descriptors sorted by class (null: tickets walk desc)
     uint8_t *otype;      // result container type (0 = dropped)
     uint32_t *ocard;     // result cardinality
     uint32_t *olen;      // result length (array values / runs)

@@ -1273,15 +1273,16 @@ struct ItemsBuf {
     uint8_t *block = nullptr;
     size_t bytes = 0;
     Items it;
-    // order_min: batches with at least that many item slots get the class-ordered ticket list
-    bool alloc(uint64_t W, bool with_order = false) {
+    // with_desc: cell descriptors (k_compute_items); with_order: batches with at least order_min item
+    // slots also get them sorted by class
+    bool alloc(uint64_t W, bool with_desc, bool with_order) {
         size_t o = 0;
         const size_t o_off = o; o += al256(8 * W);
-        const size_t o_order = o; if (with_order) o += al256(4 * W);
+        const size_t o_desc = o; if (with_desc) o += al256(32 * W);
+        const size_t o_dcls = o; if (with_order) o += al256(32 * W);
         const size_t o_cls = o; if (with_order) o += al256(W);
         const size_t o_ca = o; o += al256(4 * W);
         const size_t o_cb = o; o += al256(4 * W);
-        const size_t o_cap = o; o += al256(4 * W);
         const size_t o_ocard = o; o += al256(4 * W);
         const size_t o_olen = o; o += al256(4 * W);
         const size_t o_key = o; o += al256(2 * W);
@@ -1291,11 +1292,11 @@ struct ItemsBuf {
         block = (uint8_t *)dev_alloc(bytes);
         if (!block) return false;
         it.slot_off = (uint64_t *)(block + o_off);
-        it.order = with_order ? (uint32_t *)(block + o_order) : nullptr;
+        it.desc = with_desc ? (uint4 *)(block + o_desc) : nullptr;
+        it.desc_cls = with_order ? (uint4 *)(block + o_dcls) : nullptr;
         it.cls = with_order ? block + o_cls : nullptr;
         it.ca = (uint32_t *)(block + o_ca);
         it.cb = (uint32_t *)(block + o_cb);
-        it.slot_cap = (uint32_t *)(block + o_cap);
         it.ocard = (uint32_t *)(block + o_ocard);
         it.olen = (uint32_t *)(block + o_olen);
         it.key = (uint16_t *)(block + o_key);
@@ -1417,7 +1418,7 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     // (tried in round 2: ONE launch with a CTA per pair doing plan -> cells -> finalize for small batches —
     //  the 199-pair successive sweep took more device time per call: a pair's cells serialise on
     //  its 8 warps while the three-kernel path spreads them over the GPU)
-    if (ok) ok = ib_.alloc(pb.W, pb.W >= order_min);
+    if (ok) ok = ib_.alloc(pb.W, true, pb.W >= order_min);
     if (ok) {
         R = set_new((uint32_t)np, pb.W, pb.slab_bound);
         ok = R != nullptr;
@@ -1497,7 +1498,7 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
     ItemsBuf ib_;
     uint64_t *d_out = nullptr, *h_out = nullptr;
     bool ok = pb.build(A, B, ia, ib, np, OP_AND);
-    if (ok) ok = ib_.alloc(pb.W);
+    if (ok) ok = ib_.alloc(pb.W, false, false);
     if (ok) { d_out = (uint64_t *)dev_alloc(8 * np); h_out = (uint64_t *)pin_alloc(8 * np); ok = d_out && h_out; }
     if (ok) {
         cudaEventRecord(g.ev0, g.stream);
