@@ -6,6 +6,11 @@
 
 namespace rb200 {
 
+#ifndef RB200_FILTER_GLOBAL_MAX
+#define RB200_FILTER_GLOBAL_MAX 192   // AND / ANDNOT of an array below this many values with a bitset tests the bits
+                                      // in global memory instead of copying the bitset into the accumulator
+#endif
+
 // ------------------------------------------------------------------------------ grid cells
 // Evaluate one matched cell on the warp's accumulator and write the result payload.
 template <int OP, bool LAZY>
@@ -18,6 +23,7 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
     constexpr int op = OP;
     const bool inplace_rules = (rules & RULES_INPLACE) != 0;
     constexpr bool lazy = LAZY && (OP == OP_OR || OP == OP_XOR);
+    constexpr uint32_t AV = (OP == OP_OR || OP == OP_XOR) ? APPLY_VECS_OR : APPLY_VECS;   // array rasterise batch
     if (!lazy && (tA == T_RUN || tB == T_RUN) && tA != T_BITSET && tB != T_BITSET &&
         (tA == T_RUN ? lA : cA) + (tB == T_RUN ? lB : cB) <= 512u) {
         if (interval_cell(acc, op, tA, tB, pa, pb, cA, cB, lA, lB, out, cap, lane, otype, ocard, olen))
@@ -34,16 +40,18 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
         const uint8_t *po = arrA ? pb : pa;
         const uint32_t lo = arrA ? lB : lA;
         uint32_t n;
-        // (the filter writes only the values it keeps: at most min(cA, cB) of them)
+        // (the filter writes only the values it keeps: at most min(cA, cB) of them, in whole 16-byte
+        //  words, and the slot is a multiple of 16 bytes)
         if (2 * min(cA, cB) > cap) { if (lane == 0) atomicExch(err, 1u); otype = 0; return; }
-        if (to == T_BITSET && narr < 192) {  // few probes: test the bits where they are
-            n = filter_array<false, true>(parr, narr, reinterpret_cast<const uint32_t *>(po),
-                                          reinterpret_cast<uint16_t *>(out), lane);
-        } else {
-            acc_load(acc, to, po, lo, lane);
-            n = filter_array<false, true>(parr, narr, acc, reinterpret_cast<uint16_t *>(out), lane);
-            __syncwarp();
+        uint16_t *o16 = reinterpret_cast<uint16_t *>(out), *wb = reinterpret_cast<uint16_t *>(acc) + MERGE_WBUF;
+        if (to == T_BITSET && narr < (uint32_t)RB200_FILTER_GLOBAL_MAX) {  // few probes: test the bits where they are
+            n = filter_array<false, true>(parr, narr, reinterpret_cast<const uint32_t *>(po), o16, wb, lane, false);
+        } else {   // a bitset's copy and the array's loads share one trip
+            if (to == T_BITSET) acc_copy_bitset_async(acc, po, lane);
+            else acc_load<AV>(acc, to, po, lo, lane);
+            n = filter_array<false, true>(parr, narr, acc, o16, wb, lane, to == T_BITSET);
         }
+        __syncwarp();
         otype = n ? T_ARRAY : 0;
         ocard = olen = n;
         return;
@@ -51,14 +59,15 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
     if (op == OP_ANDNOT && tA == T_ARRAY) {
         uint32_t n;
         if (2 * cA > cap) { if (lane == 0) atomicExch(err, 1u); otype = 0; return; }
-        if (tB == T_BITSET && cA < 192) {
-            n = filter_array<true, true>(pa, cA, reinterpret_cast<const uint32_t *>(pb),
-                                         reinterpret_cast<uint16_t *>(out), lane);
+        uint16_t *o16 = reinterpret_cast<uint16_t *>(out), *wb = reinterpret_cast<uint16_t *>(acc) + MERGE_WBUF;
+        if (tB == T_BITSET && cA < (uint32_t)RB200_FILTER_GLOBAL_MAX) {
+            n = filter_array<true, true>(pa, cA, reinterpret_cast<const uint32_t *>(pb), o16, wb, lane, false);
         } else {
-            acc_load(acc, tB, pb, lB, lane);
-            n = filter_array<true, true>(pa, cA, acc, reinterpret_cast<uint16_t *>(out), lane);
-            __syncwarp();
+            if (tB == T_BITSET) acc_copy_bitset_async(acc, pb, lane);
+            else acc_load<AV>(acc, tB, pb, lB, lane);
+            n = filter_array<true, true>(pa, cA, acc, o16, wb, lane, tB == T_BITSET);
         }
+        __syncwarp();
         otype = n ? T_ARRAY : 0;
         ocard = olen = n;
         return;
@@ -88,8 +97,21 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
             default: card = acc_bitset_op_bitset<OP_ANDNOT>(acc, pa, pb, lane); break;
         }
         __syncwarp();
+    } else if ((tA == T_BITSET && tB == T_ARRAY) || (tA == T_ARRAY && tB == T_BITSET)) {
+        // bitset with an array (AND and A x B ANDNOT took the filter above): the bitset is copied into
+        // the accumulator by cp.async and the array applied on top, its first loads issued before the
+        // copy is waited for, so both arrive in the same trip.  A x B unions / xors run as B op A,
+        // the same set.
+        const bool arrA = tA == T_ARRAY;
+        const uint8_t *parr = arrA ? pa : pb;
+        const uint32_t narr = arrA ? cA : cB;
+        acc_copy_bitset_async(acc, arrA ? pb : pa, lane);
+        if (op == OP_OR) acc_apply_array<0, APPLY_WAIT, AV>(acc, parr, narr, lane);
+        else if (op == OP_XOR) acc_apply_array<1, APPLY_WAIT, AV>(acc, parr, narr, lane);
+        else if (op == OP_ANDNOT) acc_apply_array<2, APPLY_WAIT, AV>(acc, parr, narr, lane);
+        __syncwarp();
     } else {
-        acc_load(acc, tA, pa, lA, lane);
+        acc_load<AV>(acc, tA, pa, lA, lane);
         if (tB == T_BITSET) {
             switch (op) {
                 case OP_AND: acc_op_bitset<OP_AND>(acc, pb, lane); break;
@@ -100,9 +122,9 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
         } else if (tB == T_ARRAY) {
             switch (op) {
                 case OP_AND: acc_and_array(acc, pb, cB, lane); break;  // not reached (filter path)
-                case OP_OR: acc_apply_array<0>(acc, pb, cB, lane); break;
-                case OP_XOR: acc_apply_array<1>(acc, pb, cB, lane); break;
-                default: acc_apply_array<2>(acc, pb, cB, lane); break;
+                case OP_OR: acc_apply_array<0, APPLY_NONE, AV>(acc, pb, cB, lane); break;
+                case OP_XOR: acc_apply_array<1, APPLY_NONE, AV>(acc, pb, cB, lane); break;
+                default: acc_apply_array<2, APPLY_NONE, AV>(acc, pb, cB, lane); break;
             }
         } else {
             switch (op) {

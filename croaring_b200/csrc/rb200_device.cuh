@@ -27,6 +27,8 @@ __device__ __forceinline__ unsigned lanemask_lt() {
     return m;
 }
 
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
 __device__ __forceinline__ int popc4(const uint4 &q) {
     return __popc(q.x) + __popc(q.y) + __popc(q.z) + __popc(q.w);
 }
@@ -271,16 +273,27 @@ __device__ __forceinline__ void acc_zero(uint32_t *acc, int lane) {
     for (int i = 0; i < 16; i++) reinterpret_cast<uint4 *>(acc)[i * 32 + lane] = z;
 }
 
+// Bitset -> accumulator as 16 cp.async.cg copies of 16 bytes per lane: one trip to L2, no registers
+// held.  The copies are only issued here; acc_async_wait() waits for them, so a caller can issue the
+// loads of the cell's other operand in between and have both arrive in the same trip.
+// acc_async_wait() waits for ALL of the thread's outstanding cp.async groups: in k_compute_items that
+// includes the prefetch of the next cell's descriptor, which only makes that wait a little earlier
+// (the descriptor slot is read after the loop's own wait + __syncwarp, never before).
+__device__ __forceinline__ void acc_copy_bitset_async(uint32_t *acc, const uint8_t *src, int lane) {
+    const uint32_t d = smem_u32(acc) + 16u * lane;
+    const uint4 *s = reinterpret_cast<const uint4 *>(src) + lane;
+#pragma unroll
+    for (int i = 0; i < 16; i++)
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d + 512u * i), "l"(s + 32 * i) : "memory");
+    asm volatile("cp.async.commit_group;\n" ::: "memory");
+}
+__device__ __forceinline__ void acc_async_wait() {
+    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    __syncwarp();
+}
 __device__ __forceinline__ void acc_copy_bitset(uint32_t *acc, const uint8_t *src, int lane) {
-    const uint4 *s = reinterpret_cast<const uint4 *>(src);
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        uint4 q[8];
-#pragma unroll
-        for (int i = 0; i < 8; i++) q[i] = __ldg(s + (h * 8 + i) * 32 + lane);
-#pragma unroll
-        for (int i = 0; i < 8; i++) reinterpret_cast<uint4 *>(acc)[(h * 8 + i) * 32 + lane] = q[i];
-    }
+    acc_copy_bitset_async(acc, src, lane);
+    acc_async_wait();
 }
 
 __device__ __forceinline__ void acc_store_bitset(const uint32_t *acc, uint8_t *dst, int lane) {
@@ -309,12 +322,49 @@ __device__ __forceinline__ void acc_plain(uint32_t *p) {
 #define RB200_APPLY_SPARSE_MAX 4097   // arrays below this many values set their bits one atomic per value (merging same-word
                                       // bits in registers first costs more instructions than it saves atomics)
 #endif
-template <int MODE>
-__device__ __forceinline__ void acc_apply_array(uint32_t *acc, const uint8_t *src, uint32_t n,
+// Up to VECS vectors per lane (256 values each) are loaded before the first atomic, so an array of up
+// to 256 * VECS values costs one trip to L2.  PRE runs between the first loads and the first atomic:
+// APPLY_ZERO clears the accumulator (rasterising into a fresh one), APPLY_WAIT waits for an
+// acc_copy_bitset_async issued by the caller (the bitset and the array arrive in the same trip).
+constexpr int APPLY_NONE = 0, APPLY_ZERO = 1, APPLY_WAIT = 2;
+#ifndef RB200_APPLY_VECS
+#define RB200_APPLY_VECS 2      // AND / ANDNOT cells, and_cardinality, conversions
+#endif
+#ifndef RB200_APPLY_VECS_OR
+#define RB200_APPLY_VECS_OR 1   // union / xor cells: more registers there spill in the cell kernel's main loop
+#endif                          // (measured slower on every union / xor launch of the headline workload)
+constexpr uint32_t APPLY_VECS = RB200_APPLY_VECS, APPLY_VECS_OR = RB200_APPLY_VECS_OR;
+template <int MODE, int PRE = APPLY_NONE, uint32_t VECS = APPLY_VECS>
+__device__ __forceinline__ void acc_apply_array(uint32_t *acc, const uint8_t *__restrict__ src, uint32_t n,
                                                 int lane) {
     const uint4 *v4 = reinterpret_cast<const uint4 *>(src);
     const uint32_t nvec = (n + 7) >> 3;
-    if (n < (uint32_t)RB200_APPLY_SPARSE_MAX) {    // sparse: one atomic per value, no merging
+    if (PRE == APPLY_NONE && n >= (uint32_t)RB200_APPLY_SPARSE_MAX) {   // dense: same-word bits merged first
+        for (uint32_t i = lane; i < nvec; i += 32) {
+            const uint4 q = __ldg(v4 + i);
+            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+            const uint32_t left = n - i * 8;           // values valid in this vector (>= 1)
+            uint32_t cur_w = (w[0] & 0xffffu) >> 5, cur_m = 0;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
+                const uint32_t wi = v >> 5, bit = 1u << (v & 31);
+                if (k == 0 || k < (int)left) {         // k == 0 is always valid
+                    if (wi != cur_w) {
+                        acc_atom<MODE>(acc + cur_w, cur_m);
+                        cur_w = wi;
+                        cur_m = bit;
+                    } else {
+                        cur_m |= bit;
+                    }
+                }
+            }
+            acc_atom<MODE>(acc + cur_w, cur_m);
+        }
+        return;
+    }
+    // sparse: one atomic per value, no merging
+    if (VECS == 1 && PRE == APPLY_NONE) {   // one vector per lane in flight (k_or_many2, where more registers spill)
         for (uint32_t i = lane; i < nvec; i += 32) {
             const uint4 q = __ldg(v4 + i);
             const uint32_t w[4] = {q.x, q.y, q.z, q.w};
@@ -327,27 +377,32 @@ __device__ __forceinline__ void acc_apply_array(uint32_t *acc, const uint8_t *sr
         }
         return;
     }
-    for (uint32_t i = lane; i < nvec; i += 32) {
-        const uint4 q = __ldg(v4 + i);
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-        const uint32_t left = n - i * 8;           // values valid in this vector (>= 1)
-        uint32_t cur_w = (w[0] & 0xffffu) >> 5, cur_m = 0;
+    uint32_t i0 = 0;
+    do {
+        uint4 q[VECS];
 #pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
-            const uint32_t wi = v >> 5, bit = 1u << (v & 31);
-            if (k == 0 || k < (int)left) {         // k == 0 is always valid
-                if (wi != cur_w) {
-                    acc_atom<MODE>(acc + cur_w, cur_m);
-                    cur_w = wi;
-                    cur_m = bit;
-                } else {
-                    cur_m |= bit;
-                }
+        for (uint32_t u = 0; u < VECS; u++) {
+            const uint32_t i = i0 + 32 * u + lane;
+            if (i < nvec) q[u] = __ldg(v4 + i);
+        }
+        if (PRE == APPLY_ZERO && i0 == 0) { acc_zero(acc, lane); __syncwarp(); }
+        if (PRE == APPLY_WAIT && i0 == 0) acc_async_wait();
+#pragma unroll 1
+        for (uint32_t u = 0; u < VECS; u++) {   // one vector per pass, the next ones moved down
+            const uint32_t i = i0 + 32 * u + lane;
+            if (i >= nvec) break;
+            const uint32_t w[4] = {q[0].x, q[0].y, q[0].z, q[0].w};
+#pragma unroll
+            for (uint32_t r = 0; r + 1 < VECS; r++) q[r] = q[r + 1];
+            const uint32_t left = n - i * 8;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
+                if (k < (int)left) acc_atom<MODE>(acc + (v >> 5), 1u << (v & 31));
             }
         }
-        acc_atom<MODE>(acc + cur_w, cur_m);
-    }
+        i0 += 32 * VECS;
+    } while (i0 < nvec);
 }
 
 // one 16-byte vector (8 values, `left` of them valid, >= 1) of a sorted array into the accumulator
@@ -379,35 +434,6 @@ __device__ __forceinline__ void acc_or_vec_sparse(uint32_t *acc, uint4 q, uint32
     for (int k = 0; k < 8; k++) {
         const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
         if (k < (int)left) atomicOr(acc + (v >> 5), 1u << (v & 31));
-    }
-}
-
-// same with the first vector of every lane already loaded by the caller (several containers in flight)
-template <int MODE>
-__device__ __forceinline__ void acc_apply_array_first(uint32_t *acc, const uint8_t *src, uint32_t n, uint4 q,
-                                                      int lane) {
-    const uint4 *v4 = reinterpret_cast<const uint4 *>(src);
-    const uint32_t nvec = (n + 7) >> 3;
-    for (uint32_t i = lane; i < nvec; i += 32) {
-        if (i != (uint32_t)lane) q = __ldg(v4 + i);
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-        const uint32_t left = n - i * 8;
-        uint32_t cur_w = (w[0] & 0xffffu) >> 5, cur_m = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
-            const uint32_t wi = v >> 5, bit = 1u << (v & 31);
-            if (k == 0 || k < (int)left) {
-                if (wi != cur_w) {
-                    acc_atom<MODE>(acc + cur_w, cur_m);
-                    cur_w = wi;
-                    cur_m = bit;
-                } else {
-                    cur_m |= bit;
-                }
-            }
-        }
-        acc_atom<MODE>(acc + cur_w, cur_m);
     }
 }
 
@@ -507,22 +533,24 @@ static __device__ __noinline__ void acc_and_array(uint32_t *acc, const uint8_t *
 }
 
 // Rasterise any container into the (private) accumulator.
+template <uint32_t VECS = APPLY_VECS>
 __device__ __forceinline__ void acc_load(uint32_t *acc, int type, const uint8_t *src,
                                          uint32_t len, int lane) {
     if (type == T_BITSET) {
         acc_copy_bitset(acc, src, lane);
+    } else if (type == T_ARRAY) {
+        acc_apply_array<0, APPLY_ZERO, VECS>(acc, src, len, lane);   // the array's loads overlap the clearing
     } else {
         acc_zero(acc, lane);
         __syncwarp();
-        if (type == T_ARRAY) acc_apply_array<0>(acc, src, len, lane);
-        else acc_apply_runs<0, false>(acc, src, len, lane);
+        acc_apply_runs<0, false>(acc, src, len, lane);
     }
     __syncwarp();
 }
 
 // acc = acc OP bitset(src), returns nothing (cardinality is taken by acc_count)
 template <int OP>
-__device__ __forceinline__ void acc_op_bitset(uint32_t *acc, const uint8_t *src, int lane) {
+__device__ __forceinline__ void acc_op_bitset(uint32_t *acc, const uint8_t *__restrict__ src, int lane) {
     const uint4 *s = reinterpret_cast<const uint4 *>(src);
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -700,34 +728,127 @@ static __device__ __noinline__ uint32_t acc_emit_runs(const uint32_t *acc, uint1
     return nr;
 }
 
-// Filter a sorted array through a bit test (array_bitset_container_intersection /
-// _andnot, src/containers/mixed_intersection.c:19-58, mixed_andnot.c:24-38): ballot compaction.
-template <bool NEG, bool WRITE>
-__device__ __forceinline__ uint32_t filter_array(const uint8_t *src, uint32_t n,
-                                                 const uint32_t *bits, uint16_t *out, int lane) {
-    const uint16_t *arr = reinterpret_cast<const uint16_t *>(src);
-    uint32_t cnt = 0;
-    for (uint32_t base = 0; base < n; base += 32) {
-        const uint32_t i = base + lane;
-        bool keep = false;
-        uint16_t v = 0;
-        if (i < n) {
-            v = arr[i];
-            const bool hit = (bits[v >> 5] >> (v & 31)) & 1u;
-            keep = NEG ? !hit : hit;
-        }
-        const unsigned m = __ballot_sync(FULLMASK, keep);
-        if (WRITE && keep) out[cnt + __popc(m & lanemask_lt())] = v;
-        cnt += __popc(m);
+// ---------------------------------------------------------------- ordered u16 output through a window
+// Both the array filter and the array merge path produce their output 32 lanes x 8 candidate values
+// at a time, in order.  A warp scan places the survivors in a shared window buffer `wb` that mirrors
+// the output from the last 16-byte boundary below `base`, and the warp stores it as whole 128-bit
+// words (u16 stores when `out` is not 16-byte aligned); the partial last word carries into the next
+// window.  Every lane brings its 8 candidates in xp (value k in half k & 1 of word k >> 1) and a
+// keep mask; returns base + the number kept.  The buffer holds 8 + 256 values.
+__device__ __forceinline__ uint32_t window_store(uint16_t *wb, uint16_t *__restrict__ out, bool vec, uint32_t base,
+                                                 const uint32_t (&xp)[4], unsigned keep, int lane) {
+    const uint32_t c = __popc(keep);
+    const uint32_t incl = warp_incl_scan(c, lane);
+    const uint32_t total = __shfl_sync(FULLMASK, incl, 31);
+    if (total == 0) return base;
+    const uint32_t head = base & 7u;   // wb[t] mirrors out[(base & ~7) + t]
+    uint32_t o = head + incl - c;
+#pragma unroll
+    for (int k = 0; k < 8; k++)
+        if ((keep >> k) & 1u) wb[o++] = (uint16_t)(xp[k >> 1] >> (16 * (k & 1)));
+    __syncwarp();
+    if (vec) {
+        uint4 *dst = reinterpret_cast<uint4 *>(out + (base - head));
+        for (uint32_t v = lane; v < (head + total + 7) / 8; v += 32)
+            dst[v] = reinterpret_cast<const uint4 *>(wb)[v];
+    } else {
+        for (uint32_t v = lane; v < total; v += 32) out[base + v] = wb[head + v];
     }
-    return cnt;
+    __syncwarp();
+    const uint32_t end = head + total;
+    if (lane == 0 && (end & 7u)) reinterpret_cast<uint4 *>(wb)[0] = reinterpret_cast<const uint4 *>(wb)[end >> 3];
+    __syncwarp();
+    return base + total;
 }
 
-// global -> shared staging of a u16 range (128-bit when the source is 16-byte aligned)
-__device__ __forceinline__ void stage_u16(uint16_t *dst, const uint8_t *src, uint32_t n, int lane) {
+// Filter a sorted array through a bit test (array_bitset_container_intersection /
+// _andnot, src/containers/mixed_intersection.c:19-58, mixed_andnot.c:24-38).
+// 128-bit loads, 8 values per lane; FILTER_VECS vectors per lane (256 values each) are loaded before
+// any bit is tested or any value stored, so an array of up to 256 * FILTER_VECS values waits on L2 once.  With WRITE
+// the survivors go out through window_store (wb: the warp's window buffer); without, they are only
+// counted.  wait_bits: `bits` is the accumulator and an acc_copy_bitset_async into it is in flight —
+// the wait goes after the array's first loads, so both arrive in the same trip.  `out` never aliases
+// the operands: it is a result slot (slab, or mapped host memory for k_pair_fused).
+#ifndef RB200_FILTER_VECS
+#define RB200_FILTER_VECS 2
+#endif
+constexpr uint32_t FILTER_VECS = RB200_FILTER_VECS;
+#ifndef RB200_FILTER_SCALAR_MAX
+#define RB200_FILTER_SCALAR_MAX 32   // arrays of at most this many values take the one-u16-per-lane loop: one load
+#endif                               // trip as well, and one ballot instead of the window store's scan
+template <bool NEG, bool WRITE>
+__device__ __forceinline__ uint32_t filter_array(const uint8_t *__restrict__ src, uint32_t n,
+                                                 const uint32_t *__restrict__ bits, uint16_t *__restrict__ out,
+                                                 uint16_t *wb, int lane, bool wait_bits = false) {
+    if ((reinterpret_cast<uintptr_t>(src) & 15) || n <= (uint32_t)RB200_FILTER_SCALAR_MAX) {
+        // unaligned source or few values: one u16 per lane, ballot compaction
+        if (wait_bits) acc_async_wait();
+        const uint16_t *arr = reinterpret_cast<const uint16_t *>(src);
+        uint32_t cnt = 0;
+        for (uint32_t base = 0; base < n; base += 32) {
+            const uint32_t i = base + lane;
+            bool keep = false;
+            uint16_t v = 0;
+            if (i < n) {
+                v = arr[i];
+                const bool hit = (bits[v >> 5] >> (v & 31)) & 1u;
+                keep = NEG ? !hit : hit;
+            }
+            const unsigned m = __ballot_sync(FULLMASK, keep);
+            if (WRITE && keep) out[cnt + __popc(m & lanemask_lt())] = v;
+            cnt += __popc(m);
+        }
+        return cnt;
+    }
+    const uint4 *v4 = reinterpret_cast<const uint4 *>(src);
+    const uint32_t nvec = (n + 7) >> 3;
+    const bool vec = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    uint32_t base = 0, cnt = 0, i0 = 0;
+    do {
+        uint4 q[FILTER_VECS];
+#pragma unroll
+        for (uint32_t u = 0; u < FILTER_VECS; u++) {
+            const uint32_t i = i0 + 32 * u + lane;
+            if (i < nvec) q[u] = __ldg(v4 + i);
+        }
+        if (wait_bits && i0 == 0) acc_async_wait();
+        // (one vector per pass, the next ones moved down: one copy of the bit tests and the window
+        //  store instead of FILTER_VECS)
+#pragma unroll 1
+        for (uint32_t u = 0; u < FILTER_VECS && i0 + 32 * u < nvec; u++) {   // warp-uniform
+            const uint32_t i = i0 + 32 * u + lane;
+            const uint32_t xp[4] = {q[0].x, q[0].y, q[0].z, q[0].w};
+#pragma unroll
+            for (uint32_t r = 0; r + 1 < FILTER_VECS; r++) q[r] = q[r + 1];
+            unsigned keep = 0;
+            if (i < nvec) {
+                const uint32_t left = n - i * 8;
+#pragma unroll
+                for (int k = 0; k < 8; k++) {
+                    const uint32_t v = (xp[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+                    const bool hit = (bits[v >> 5] >> (v & 31)) & 1u;
+                    keep |= (unsigned)((NEG ? !hit : hit) && k < (int)left) << k;
+                }
+            }
+            if (WRITE) base = window_store(wb, out, vec, base, xp, keep, lane);
+            else cnt += __popc(keep);
+        }
+        i0 += 32 * FILTER_VECS;
+    } while (i0 < nvec);
+    return WRITE ? base : __reduce_add_sync(FULLMASK, cnt);
+}
+
+// global -> shared staging of a u16 range (dst 16-byte aligned).  A 16-byte aligned source is copied
+// by cp.async.cg, 16 bytes per copy, all of them issued at once and none waited for here: the caller
+// issues every range it needs and then waits once (acc_async_wait), so they arrive in one trip to L2.
+// An unaligned source is copied one u16 per lane, synchronously.
+__device__ __forceinline__ void stage_u16_async(uint16_t *dst, const uint8_t *src, uint32_t n, int lane) {
     if ((reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+        const uint32_t d = smem_u32(dst);
+        const uint4 *s = reinterpret_cast<const uint4 *>(src);
         for (uint32_t i = lane; i < (n + 7) / 8; i += 32)
-            reinterpret_cast<uint4 *>(dst)[i] = __ldg(reinterpret_cast<const uint4 *>(src) + i);
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d + 16u * i), "l"(s + i) : "memory");
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
     } else {
         const uint16_t *s16 = reinterpret_cast<const uint16_t *>(src);
         for (uint32_t i = lane; i < n; i += 32) dst[i] = s16[i];
@@ -737,15 +858,14 @@ __device__ __forceinline__ void stage_u16(uint16_t *dst, const uint8_t *src, uin
 // Union / symmetric difference of two sorted u16 arrays with n + m <= 4096 values, the cells whose
 // result the type rule makes an array (array_container_union / xor, src/array_util.c:1104,1198),
 // as a windowed warp merge path: no accumulator round trip and no find-first-set emission.
-// Both inputs are staged once in the warp's shared block, a at 0 and b at round8(n); the 128-bit
-// staging reaches u16 index round8(n) + round8(m) <= 4104.  The merged sequence is produced in
+// Both inputs are staged once in the warp's shared block by cp.async, a at 0 and b at round8(n), both
+// copies in flight together; the 128-bit staging reaches u16 index round8(n) + round8(m) <= 4104.  The merged sequence is produced in
 // windows of 32 * MERGE_PER_LANE positions: every lane finds the split of its diagonal (merge-path
 // search between the window's start split and MERGE_PER_LANE more values per lane before it),
 // merges its values in registers and decides which survive.  Duplicates (a value present in both
-// inputs) are adjacent in the merged order: OR keeps the first, XOR drops both.  A warp scan places
-// the survivors in the window buffer (u16 index MERGE_WBUF, past the staging) and the warp stores
-// them at the running output offset.  The buffer mirrors the output from the last 16-byte boundary,
-// so the stores are whole 128-bit words; the partial last word carries into the next window.
+// inputs) are adjacent in the merged order: OR keeps the first, XOR drops both.  window_store places
+// the survivors in the window buffer (u16 index MERGE_WBUF, past the staging; the array filter uses
+// the same buffer) and stores them at the running output offset as whole 128-bit words.
 constexpr uint32_t MERGE_PER_LANE = 8, MERGE_WIN = 32 * MERGE_PER_LANE;
 constexpr uint32_t MERGE_WBUF = 4104;
 // per-warp shared block: the 8 KiB accumulator, then room for the merge's window buffer (9 KiB)
@@ -763,9 +883,9 @@ static __device__ __noinline__ uint32_t merge_arrays(uint32_t *acc, const uint8_
     uint16_t *wb = sa + MERGE_WBUF;
     uint16_t *o16 = reinterpret_cast<uint16_t *>(out);
     const bool vec = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
-    stage_u16(sa, pa, n, lane);
-    stage_u16(sb, pb, m, lane);
-    __syncwarp();
+    stage_u16_async(sa, pa, n, lane);
+    stage_u16_async(sb, pb, m, lane);
+    acc_async_wait();   // both inputs in one trip (also waits for the next cell's descriptor prefetch)
     const uint32_t T = n + m, NONE = 0x10000u;   // NONE: past the end of an input, above every value
     uint32_t is = 0;                             // split at the window start: values taken from a
     uint32_t last = NONE + 1;                    // merged value before the window (none yet)
@@ -811,27 +931,7 @@ static __device__ __noinline__ uint32_t merge_arrays(uint32_t *acc, const uint8_
         is = __shfl_sync(FULLMASK, i, 31);
         keep |= (unsigned)(x0 < NONE && x0 != prev && (!IS_XOR || x0 != x1));
         if (IS_XOR) keep |= (unsigned)(p1 < NONE && p1 != p2 && p1 != min(ai, bj)) << (MERGE_PER_LANE - 1);
-        const uint32_t c = __popc(keep);
-        const uint32_t incl = warp_incl_scan(c, lane);
-        const uint32_t total = __shfl_sync(FULLMASK, incl, 31);
-        const uint32_t head = base & 7u;   // wb[t] mirrors out[(base & ~7) + t]
-        uint32_t o = head + incl - c;
-#pragma unroll
-        for (int k = 0; k < (int)MERGE_PER_LANE; k++)
-            if ((keep >> k) & 1u) wb[o++] = (uint16_t)(xp[k >> 1] >> (16 * (k & 1)));
-        __syncwarp();
-        if (vec) {
-            uint4 *dst = reinterpret_cast<uint4 *>(o16 + (base - head));
-            for (uint32_t v = lane; v < (head + total + 7) / 8; v += 32)
-                dst[v] = reinterpret_cast<const uint4 *>(wb)[v];
-        } else {
-            for (uint32_t v = lane; v < total; v += 32) o16[base + v] = wb[head + v];
-        }
-        __syncwarp();
-        const uint32_t end = head + total;
-        if (lane == 0 && (end & 7u)) reinterpret_cast<uint4 *>(wb)[0] = reinterpret_cast<const uint4 *>(wb)[end >> 3];
-        __syncwarp();
-        base += total;
+        base = window_store(wb, o16, vec, base, xp, keep, lane);
     }
     return base;
 }
@@ -980,7 +1080,6 @@ interval_cell(uint32_t *acc, int op, int tA, int tB, const uint8_t *pa, const ui
 // Operand staging with the Hopper TMA unit: ONE elected thread issues cp.async.bulk (global -> shared,
 // whole containers, 16-byte granules) against an mbarrier; the bytes land asynchronously while the
 // other warps keep working on the previous batch, and nobody holds registers for loads in flight.
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }

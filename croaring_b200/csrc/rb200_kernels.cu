@@ -478,9 +478,9 @@ __device__ __forceinline__ uint32_t cell_and_card(uint32_t *acc, int tA, int tB,
         const uint32_t lo = arrA ? lB : lA;
         if (to == T_BITSET)
             return filter_array<false, false>(parr, narr, reinterpret_cast<const uint32_t *>(po),
-                                              nullptr, lane);
+                                              nullptr, nullptr, lane);
         acc_load(acc, to, po, lo, lane);
-        const uint32_t n = filter_array<false, false>(parr, narr, acc, nullptr, lane);
+        const uint32_t n = filter_array<false, false>(parr, narr, acc, nullptr, nullptr, lane);
         __syncwarp();
         return n;
     }

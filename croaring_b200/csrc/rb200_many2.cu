@@ -601,7 +601,7 @@ k_or_many2(SetView S, Many2Index ix, uint32_t n, uint32_t *__restrict__ scratch,
                     const uint32_t q = sm.ar_list[j];
                     uint32_t *dst = (L != POS_NONE && sm.s_pos[q] > L) ? sm.acc2 : sm.acc;
                     const uint8_t *p = S.payload + sm.s_off[q];
-                    if ((sm.s_tf[q] & 15) == T_ARRAY) acc_apply_array<0>(dst, p, sm.s_len[q], lane);
+                    if ((sm.s_tf[q] & 15) == T_ARRAY) acc_apply_array<0, APPLY_NONE, 1>(dst, p, sm.s_len[q], lane);
                     else acc_apply_runs<0, true>(dst, p, sm.s_len[q], lane);
                 }
                 continue;
