@@ -106,6 +106,8 @@ def lib():
     sig("rb200_set_run_optimize", _P, _P, C.c_int)
     sig("rb200_set_to_uint32", C.c_int, _P, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.POINTER(C.c_uint64)))
     sig("rb200_values_free", None, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64))
+    sig("rb200_set_from_uint32", _P, _P, _P, C.c_size_t)
+    sig("rb200_set_from_uint32_device", _P, _P, _P, C.c_size_t)
     sig("rb200_set_serialize", C.c_int, _P, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)),
         C.POINTER(C.POINTER(C.c_uint64)))
     sig("rb200_serialized_free", None, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64))
@@ -489,6 +491,16 @@ def batch_op_host(op, a, b):
     return [Bitmap(out[i]) for i in range(n)]
 
 
+def _values_u32(a):
+    """1-D integer values as a contiguous uint32 array (refused if any lies outside [0, 2^32))."""
+    a = np.asarray(a)
+    if a.ndim != 1 or (a.size and a.dtype.kind not in "iu"):
+        raise RB200Error(f"values must be 1-D integer arrays, got {a.dtype} with shape {a.shape}")
+    if a.size and a.dtype != np.uint32 and (int(a.min()) < 0 or int(a.max()) > 0xFFFFFFFF):
+        raise RB200Error("values must lie in [0, 2^32)")
+    return np.ascontiguousarray(a, dtype=np.uint32)
+
+
 class DeviceSet:
     """An ordered collection of bitmaps resident in HBM (rb200_set_t*)."""
 
@@ -519,6 +531,45 @@ class DeviceSet:
         arr = (C.c_char_p * n)(*blobs)
         lens = (C.c_size_t * n)(*[len(b) for b in blobs])
         return cls(lib().rb200_set_upload_frozen(arr, lens, n))
+
+    @classmethod
+    def from_values(cls, values, offsets=None):
+        """roaring_bitmap_of_ptr of every bitmap, built on the device (no run containers: chain
+        .run_optimize() for those).  values: a list of 1-D integer arrays, one per bitmap; or one flat
+        uint32 array with n + 1 offsets (the layout of to_uint32_arrays); or a CUDA torch tensor of
+        int32 / uint32 values with offsets as a CUDA or CPU tensor, read in place on the library stream
+        (order its writes before the call, e.g. by building it on the stream given to set_stream)."""
+        if getattr(values, "is_cuda", False):
+            return cls._from_device_values(values, offsets)
+        if offsets is None:
+            arrays = [np.asarray(a).reshape(-1) for a in values]
+            offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
+            np.cumsum([a.size for a in arrays], out=offs[1:])
+            flat = _values_u32(np.concatenate(arrays) if arrays else np.zeros(0, np.uint32))
+        else:
+            flat = _values_u32(values)
+            offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
+            if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
+                raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
+        return cls(lib().rb200_set_from_uint32(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+
+    @classmethod
+    def _from_device_values(cls, values, offsets):
+        import torch
+        if values.dtype not in (torch.int32, torch.uint32) or values.dim() != 1 or not values.is_contiguous():
+            raise RB200Error("device values must be a contiguous 1-D int32 / uint32 CUDA tensor")
+        if offsets is None:
+            raise RB200Error("device values need offsets")
+        offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
+        if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
+            raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
+        last = int(offs[-1].item())
+        if last < 0 or last > values.numel():
+            raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
+        offs = offs.to(values.device).contiguous()
+        if offs is not offsets:   # copied here: on the stream the library reads on
+            torch.cuda.current_stream(values.device).synchronize()
+        return cls(lib().rb200_set_from_uint32_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
 
     def free(self):
         if self.ptr:

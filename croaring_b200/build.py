@@ -12,7 +12,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libroaring_b200.so")
-SOURCES = ["rb200_kernels.cu", "rb200_many.cu", "rb200_many2.cu", "rb200_convert.cu", "rb200_host.cu", "rb200_shard.cu", "rb200_fused.cu"]
+SOURCES = ["rb200_kernels.cu", "rb200_many.cu", "rb200_many2.cu", "rb200_convert.cu", "rb200_build.cu", "rb200_host.cu", "rb200_shard.cu",
+           "rb200_fused.cu"]
 HEADERS = ["rb200_common.h", "rb200_device.cuh", "rb200_cells.cuh", "rb200_internal.h", os.path.join("..", "..", "include", "roaring_b200.h")]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper) only

@@ -154,6 +154,7 @@ struct OpStats {
     unsigned int units;               // or_many: number of (key, slice) work units
     unsigned int cls_count[8];        // pairwise ops: live work items per code-path class
     unsigned int cls_cursor[8];       //               fill cursors of k_order_items
+    unsigned long long payload_bytes; // set builders: container_size_in_bytes of every container, summed
 };
 
 // Code-path classes of the pairwise work items.  k_compute_items is one large kernel (a code path
@@ -311,6 +312,24 @@ void launch_values_measure(const SetView &S, uint32_t nb, uint64_t *bm_vals, uin
                            uint64_t *c_start, uint32_t *c_bitmap, cudaStream_t s);
 void launch_values_write(const SetView &S, uint32_t nb, const uint64_t *bm_off, const uint64_t *c_start,
                          const uint32_t *c_bitmap, uint64_t nc, uint32_t *out, cudaStream_t s);
+// per bitmap of a produced set: bm_card, bm_bytes, bm_ebytes from its container directory
+void launch_bitmap_figures(SetOut out, uint32_t nb, const OpStats *st, cudaStream_t s);
+
+// roaring_bitmap_of_ptr over a batch (rb200_build.cu).  v: values, off: n + 1 offsets, N = off[n].
+uint64_t build_tile_count(uint64_t N);
+void launch_build_measure(const uint32_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
+                          uint32_t *unsorted, cudaStream_t s);
+void launch_build_emit(const uint32_t *v, const uint64_t *off, uint32_t n, uint64_t N, const uint64_t *tile_base,
+                       uint16_t *c_key, uint64_t *c_pos, cudaStream_t s);
+void launch_build_slots(const uint64_t *c_pos, uint64_t nc, uint64_t N, uint64_t *slot, cudaStream_t s);
+void launch_build_bitmaps(const uint64_t *off, uint32_t n, const uint64_t *c_pos, uint64_t nc, uint32_t *bm_beg,
+                          uint32_t *bm_cnt, cudaStream_t s);
+void launch_build_write(const uint32_t *v, const uint64_t *c_pos, uint64_t nc, uint64_t N, SetOut out,
+                        uint64_t slab_cap, OpStats *st, cudaStream_t s);
+bool build_scan(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *out, uint64_t n, cudaStream_t s);
+bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint32_t *in, uint32_t *out, const uint64_t *off,
+                      uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s);
+
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
                      uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
                      int sms, cudaStream_t s);

@@ -392,6 +392,61 @@ void ev_put(cudaEvent_t e) {
     g.evpool.push_back(e);
 }
 
+// Host bytes -> one device buffer as a stream through two pinned chunks on the library stream: the
+// copy of one chunk overlaps the memcpy into the other.  put() appends (src == nullptr: zeros),
+// flush() sends the rest.  The chunks go back to the pool when the stager is destroyed, so it must
+// outlive a synchronisation of the stream after the last flush.
+struct H2DStager {
+    static constexpr size_t CH = (size_t)32 << 20;
+    uint8_t *dst, *chunk[2];
+    cudaEvent_t cev[2] = {nullptr, nullptr};
+    bool cev_used[2] = {false, false};
+    bool ok;
+    int cur = 0;
+    size_t used = 0;
+    uint64_t base = 0;
+    explicit H2DStager(uint8_t *d) : dst(d) {
+        chunk[0] = (uint8_t *)pin_alloc(CH);
+        chunk[1] = (uint8_t *)pin_alloc(CH);
+        ok = chunk[0] && chunk[1];
+        for (int k = 0; k < 2 && ok; k++) ok = cudaEventCreateWithFlags(&cev[k], cudaEventDisableTiming) == cudaSuccess;
+    }
+    ~H2DStager() {
+        for (int k = 0; k < 2; k++) if (cev[k]) cudaEventDestroy(cev[k]);
+        pin_free(chunk[0], CH);
+        pin_free(chunk[1], CH);
+    }
+    bool flush() {
+        if (used) {
+            if (cudaMemcpyAsync(dst + base, chunk[cur], used, cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
+                return false;
+            cudaEventRecord(cev[cur], g.stream);
+            cev_used[cur] = true;
+        }
+        base += used;
+        used = 0;
+        cur ^= 1;
+        if (cev_used[cur]) cudaEventSynchronize(cev[cur]);
+        return true;
+    }
+    bool put(const void *src, size_t n) {
+        const uint8_t *p = (const uint8_t *)src;
+        while (n) {
+            if (used == CH && !flush()) return false;
+            const size_t take = std::min(CH - used, n);
+            if (p) {
+                memcpy(chunk[cur] + used, p, take);
+                p += take;
+            } else {
+                memset(chunk[cur] + used, 0, take);
+            }
+            used += take;
+            n -= take;
+        }
+        return true;
+    }
+};
+
 // Wait for the op that produced `cs` (if it is still in flight) and take over its counters.
 // false: the op failed (t_err says why); the set must not be used.
 bool resolve(const rb200_set *cs) {
@@ -1095,12 +1150,8 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
     uint32_t *h_bc = (uint32_t *)pin_alloc(8 * (n ? n : 1));
     uint8_t *d_raw = (uint8_t *)dev_alloc(raw_total ? raw_total : 16);
     uint64_t *d_src = (uint64_t *)dev_alloc(8 * (nc ? nc : 1));
-    const size_t CH = (size_t)32 << 20;
-    uint8_t *chunk[2] = {(uint8_t *)pin_alloc(CH), (uint8_t *)pin_alloc(CH)};
-    cudaEvent_t cev[2] = {nullptr, nullptr};
-    bool cev_used[2] = {false, false};
-    bool ok = h_tab && d_tab && h_bc && d_raw && d_src && chunk[0] && chunk[1];
-    for (int k = 0; k < 2 && ok; k++) ok = cudaEventCreateWithFlags(&cev[k], cudaEventDisableTiming) == cudaSuccess;
+    H2DStager stage(d_raw);
+    bool ok = h_tab && d_tab && h_bc && d_raw && d_src && stage.ok;
     if (ok) {
         uint64_t ro = 0, so = 0, cb = 0;
         for (size_t i = 0; i < n; i++) {
@@ -1125,37 +1176,9 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
               (cudaMemcpyAsync(s->d_dir + s->L.o_beg, h_bc, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
                cudaMemcpyAsync(s->d_dir + s->L.o_cnt, h_bc + n, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess));
         // raw bytes as one stream through the two pinned chunks
-        int cur = 0;
-        size_t used = 0;
-        uint64_t base = 0;
-        auto flush = [&]() -> bool {
-            if (used) {
-                if (cudaMemcpyAsync(d_raw + base, chunk[cur], used, cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
-                    return false;
-                cudaEventRecord(cev[cur], g.stream);
-                cev_used[cur] = true;
-            }
-            base += used;
-            used = 0;
-            cur ^= 1;
-            if (cev_used[cur]) cudaEventSynchronize(cev[cur]);
-            return true;
-        };
-        for (size_t i = 0; i < n && ok; i++) {
-            size_t done = 0;
-            const size_t padded = (lens[i] + 15) & ~(size_t)15;
-            while (done < padded && ok) {
-                if (used == CH) ok = flush();
-                const size_t room = CH - used, want = padded - done;
-                const size_t take = room < want ? room : want;
-                const size_t real = done < lens[i] ? std::min(take, lens[i] - done) : 0;
-                if (real) memcpy(chunk[cur] + used, bufs[i] + done, real);
-                if (take > real) memset(chunk[cur] + used + real, 0, take - real);
-                used += take;
-                done += take;
-            }
-        }
-        if (ok) ok = flush();
+        for (size_t i = 0; i < n && ok; i++)
+            ok = stage.put(bufs[i], lens[i]) && stage.put(nullptr, ((lens[i] + 15) & ~(size_t)15) - lens[i]);
+        if (ok) ok = stage.flush();
     }
     if (ok) {
         ok = stats_reset();
@@ -1184,9 +1207,6 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
         cudaStreamSynchronize(g.stream);
     }
     if (ok) s->mirrors_pending = n > 0;   // exact per-bitmap bytes / effective bytes: k_deser_bitmap_cards wrote them
-    for (int k = 0; k < 2; k++) if (cev[k]) cudaEventDestroy(cev[k]);
-    pin_free(chunk[0], CH);
-    pin_free(chunk[1], CH);
     pin_free(h_tab, tb);
     pin_free(h_bc, 8 * (n ? n : 1));
     dev_free(d_tab, tb);
@@ -2797,6 +2817,224 @@ int rb200_set_to_uint32(const rb200_set_t *S, uint32_t **vals, uint64_t **off_ou
 }
 
 void rb200_values_free(uint32_t *vals, uint64_t *off) { rb200_serialized_free((char *)vals, off, nullptr); }
+
+// Arguments of rb200_set_from_uint32*: n < 2^32 bitmaps; n + 1 offsets, off[0] == 0, non-decreasing.
+static bool check_bitmap_count(size_t n) {
+    if (n <= 0xffffffffull) return true;
+    t_err = "set_from_uint32: " + std::to_string((uint64_t)n) + " bitmaps, at most 2^32 - 1 fit in a set";
+    return false;
+}
+static bool check_value_offsets(const uint64_t *off, size_t n) {
+    if (!check_bitmap_count(n)) return false;
+    if (!off) { t_err = "set_from_uint32: offsets are NULL"; return false; }
+    if (off[0] != 0) {
+        t_err = "set_from_uint32: offsets must start at 0 (off[0] = " + std::to_string(off[0]) + ")";
+        return false;
+    }
+    for (size_t i = 0; i < n; i++)
+        if (off[i + 1] < off[i]) {
+            t_err = "set_from_uint32: offsets decrease at bitmap " + std::to_string((uint64_t)i) + " (off[" +
+                    std::to_string((uint64_t)i) + "] = " + std::to_string(off[i]) + ", off[" +
+                    std::to_string((uint64_t)i + 1) + "] = " + std::to_string(off[i + 1]) + ")";
+            return false;
+        }
+    return true;
+}
+
+// roaring_bitmap_of_ptr of every bitmap (rb200_build.cu).  Values come from the host (h_vals, staged
+// through pinned chunks) or from the device (d_in, read in place); h_off are checked offsets.
+static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in, const uint64_t *h_off, size_t n) {
+    const uint64_t N = h_off[n];
+    const uint64_t ntiles = build_tile_count(N);
+    if (ntiles >= (1ull << 31) - 1) { t_err = "set_from_uint32: too many values for one call"; return nullptr; }
+    uint64_t *d_off = (uint64_t *)dev_alloc(8 * (n + 1));
+    uint32_t *d_vals = h_vals ? (uint32_t *)dev_alloc(4 * N) : nullptr, *d_sorted = nullptr;
+    uint64_t *d_tcnt = (uint64_t *)dev_alloc(8 * (ntiles + 1)), *d_tbase = (uint64_t *)dev_alloc(8 * (ntiles + 1));
+    uint32_t *d_flag = (uint32_t *)dev_alloc(4);
+    uint64_t *h_meta = (uint64_t *)pin_alloc(16);
+    uint64_t *d_cpos = nullptr, *d_slot = nullptr;
+    int *d_rel = nullptr;
+    void *d_temp = nullptr;
+    size_t temp_bytes = 0, scan_bytes = 0, rel_bytes = 0;
+    uint64_t nc = 0;
+    rb200_set *s = nullptr;
+    bool ok = d_off && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
+              cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    if (ok && h_vals && N) {
+        H2DStager stage((uint8_t *)d_vals);
+        ok = stage.ok && stage.put(h_vals, 4 * N) && stage.flush();
+        ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
+    }
+    const uint32_t *src = h_vals ? d_vals : d_in;
+    // container starts per tile, scanned; the total is the container count if the values are sorted
+    auto measure = [&]() -> bool {
+        size_t b = 0;
+        if (!build_scan(nullptr, &b, d_tcnt, d_tbase, ntiles + 1, g.stream)) return false;
+        if (b > temp_bytes) {
+            dev_free(d_temp, temp_bytes);
+            temp_bytes = b;
+            if (!(d_temp = dev_alloc(temp_bytes))) return false;
+        }
+        scan_bytes = b;
+        launch_build_measure(src, d_off, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
+        return build_scan(d_temp, &scan_bytes, d_tcnt, d_tbase, ntiles + 1, g.stream) &&
+               cudaMemcpyAsync(h_meta, d_tbase + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+               cudaMemcpyAsync(h_meta + 1, d_flag, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+               cudaStreamSynchronize(g.stream) == cudaSuccess;
+    };
+    ok = ok && cudaMemsetAsync(d_flag, 0, 4, g.stream) == cudaSuccess &&
+         cudaMemsetAsync(d_tcnt + ntiles, 0, 8, g.stream) == cudaSuccess && measure();
+    const uint32_t unsorted = ok ? (uint32_t)h_meta[1] : 0u;
+    if (ok && (unsorted & 2u)) {
+        t_err = "set_from_uint32: a bitmap of 2^31 values or more is not sorted; pass it sorted";
+        ok = false;
+    }
+    if (ok && unsorted) {
+        // segmented sort into scratch (the input stays as it was), in calls of < 2^31 values each;
+        // a bitmap too large for one call is sorted already (else the flag above) and is copied
+        struct Chunk { uint64_t s0, s1; bool copy; };
+        std::vector<Chunk> chunks;
+        const uint64_t LIM = (1ull << 31) - 1;
+        for (uint64_t s0 = 0; s0 < n;) {
+            uint64_t s1 = s0;
+            while (s1 < n && h_off[s1 + 1] - h_off[s0] <= LIM && s1 - s0 < LIM - 1) s1++;
+            if (s1 == s0) { chunks.push_back({s0, s0 + 1, true}); s0++; continue; }
+            chunks.push_back({s0, s1, false});
+            s0 = s1;
+        }
+        size_t sort_bytes = 0;
+        uint64_t max_seg = 0;
+        for (const Chunk &c : chunks) {
+            const uint64_t items = h_off[c.s1] - h_off[c.s0];
+            if (c.copy || !items) continue;
+            size_t b = 0;
+            if (!build_sort_chunk(nullptr, &b, src, nullptr, nullptr, h_off[c.s0], items, (uint32_t)(c.s1 - c.s0),
+                                  nullptr, g.stream)) { ok = false; break; }
+            sort_bytes = std::max(sort_bytes, b);
+            max_seg = std::max(max_seg, c.s1 - c.s0);
+        }
+        if (ok && sort_bytes > temp_bytes) {
+            dev_free(d_temp, temp_bytes);
+            temp_bytes = sort_bytes;
+            ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
+        }
+        rel_bytes = 4 * (max_seg + 1);
+        ok = ok && (d_sorted = (uint32_t *)dev_alloc(4 * N)) && (d_rel = (int *)dev_alloc(rel_bytes));
+        for (size_t k = 0; k < chunks.size() && ok; k++) {
+            const Chunk &c = chunks[k];
+            const uint64_t first = h_off[c.s0], items = h_off[c.s1] - first;
+            if (!items) continue;
+            if (c.copy) {
+                ok = cudaMemcpyAsync(d_sorted + first, src + first, 4 * items, cudaMemcpyDeviceToDevice, g.stream) ==
+                     cudaSuccess;
+            } else {
+                size_t b = temp_bytes;
+                ok = build_sort_chunk(d_temp, &b, src, d_sorted, d_off + c.s0, first, items, (uint32_t)(c.s1 - c.s0),
+                                      d_rel, g.stream);
+            }
+        }
+        if (ok) {
+            src = d_sorted;
+            ok = measure();
+            if (!ok && t_err.empty()) t_err = "set_from_uint32: segmented sort failed";
+        }
+    }
+    if (ok) {
+        nc = h_meta[0];
+        if (nc > 0xffffffffull) { t_err = "set_from_uint32: more than 2^32 - 1 containers"; ok = false; }
+    }
+    // every container stores at most 2 bytes per input value (an array 2 d <= 2 count, a bitset needs
+    // d > 4096, so 8192 < 2 count) plus its 16-byte padding
+    if (ok) ok = (s = set_new((uint32_t)n, nc, 2 * N + 16 * nc + 16)) != nullptr;
+    if (ok && nc) {
+        size_t b = 0;
+        ok = (d_cpos = (uint64_t *)dev_alloc(8 * nc)) && (d_slot = (uint64_t *)dev_alloc(8 * nc)) &&
+             build_scan(nullptr, &b, d_slot, s->out().c_off, nc, g.stream);
+        if (ok && b > temp_bytes) {
+            dev_free(d_temp, temp_bytes);
+            temp_bytes = b;
+            ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
+        }
+        if (ok) {
+            launch_build_emit(src, d_off, (uint32_t)n, N, d_tbase, s->out().c_key, d_cpos, g.stream);
+            launch_build_slots(d_cpos, nc, N, d_slot, g.stream);
+            b = temp_bytes;
+            ok = build_scan(d_temp, &b, d_slot, s->out().c_off, nc, g.stream);
+        }
+    }
+    if (ok) {
+        ok = stats_reset();
+        if (n && !nc) ok = ok && cudaMemsetAsync(s->out().bm_cnt, 0, 4 * n, g.stream) == cudaSuccess &&
+                           cudaMemsetAsync(s->out().bm_beg, 0, 4 * n, g.stream) == cudaSuccess;
+        if (nc) launch_build_bitmaps(d_off, (uint32_t)n, d_cpos, nc, s->out().bm_beg, s->out().bm_cnt, g.stream);
+        launch_build_write(src, d_cpos, nc, N, s->out(), s->slab_cap, g.d_stats, g.stream);
+        launch_bitmap_figures(s->out(), (uint32_t)n, g.d_stats, g.stream);
+        ok = ok && stats_fetch();
+        cudaError_t e = cudaStreamSynchronize(g.stream);
+        if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+            t_err = std::string("set_from_uint32: ") + cudaGetErrorString(e);
+            ok = false;
+        } else if (ok && g.h_stats->error) {
+            t_err = "internal: result slab bound exceeded";
+            ok = false;
+        }
+    } else {
+        cudaStreamSynchronize(g.stream);
+    }
+    if (ok) {
+        s->n_containers = nc;
+        s->slab_used = g.h_stats->slab_cursor;
+        s->portable_bytes = g.h_stats->payload_bytes;
+        s->mirrors_pending = n > 0;   // containers / bytes / effective bytes per bitmap: k_deser_bitmap_cards wrote them
+    }
+    dev_free(d_off, 8 * (n + 1));
+    dev_free(d_vals, 4 * N);
+    dev_free(d_sorted, 4 * N);
+    dev_free(d_tcnt, 8 * (ntiles + 1));
+    dev_free(d_tbase, 8 * (ntiles + 1));
+    dev_free(d_flag, 4);
+    dev_free(d_cpos, 8 * nc);
+    dev_free(d_slot, 8 * nc);
+    dev_free(d_temp, temp_bytes);
+    dev_free(d_rel, rel_bytes);
+    pin_free(h_meta, 16);
+    if (!ok) {
+        if (t_err.empty()) t_err = "set_from_uint32 failed";
+        set_delete(s);
+        return nullptr;
+    }
+    return s;
+}
+
+rb200_set_t *rb200_set_from_uint32(const uint32_t *vals, const uint64_t *off, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!check_value_offsets(off, n)) return nullptr;   // before any CUDA call
+    if (!vals && off[n]) { t_err = "set_from_uint32: values are NULL"; return nullptr; }
+    if (!ctx_init()) return nullptr;
+    static const uint32_t none = 0;
+    return from_uint32_impl(vals ? vals : &none, nullptr, off, n);
+}
+
+rb200_set_t *rb200_set_from_uint32_device(const uint32_t *d_vals, const uint64_t *d_off, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!check_bitmap_count(n)) return nullptr;
+    if (!d_off) { t_err = "set_from_uint32_device: offsets are NULL"; return nullptr; }
+    if (!ctx_init()) return nullptr;
+    // the offsets are checked on the host before any kernel reads values through them
+    uint64_t *h_off = (uint64_t *)pin_alloc(8 * (n + 1));
+    if (!h_off) return nullptr;
+    rb200_set *s = nullptr;
+    if (cudaMemcpyAsync(h_off, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
+        cudaStreamSynchronize(g.stream) != cudaSuccess) {
+        (void)cudaGetLastError();
+        t_err = "set_from_uint32_device: offsets are not readable device memory of the library's device";
+    } else if (check_value_offsets(h_off, n)) {
+        if (!d_vals && h_off[n]) t_err = "set_from_uint32_device: values are NULL";
+        else s = from_uint32_impl(nullptr, d_vals, h_off, n);
+    }
+    pin_free(h_off, 8 * (n + 1));
+    return s;
+}
 
 // Device-side portable serialization of every bitmap of a set + one D2H copy.
 // *buf is pinned host memory owned by the library (release with rb200_serialized_free);

@@ -1463,6 +1463,11 @@ void launch_deserialize(const uint8_t *raw, const uint64_t *roff, const uint64_t
 }  // namespace rb200
 
 namespace rb200 {
+void launch_bitmap_figures(SetOut out, uint32_t nb, const OpStats *st, cudaStream_t s) {
+    if (!nb) return;
+    k_deser_bitmap_cards<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(out, nb, st);
+    g_launches++;
+}
 void launch_pack_scan(const uint64_t *bytes, const uint32_t *cnts, uint32_t n, uint64_t *off,
                       uint64_t *beg, cudaStream_t s) {
     k_pack_scan<<<1, 1024, 0, s>>>(bytes, cnts, n, off, beg);

@@ -358,6 +358,13 @@ rb200_set_t *rb200_set_upload_frozen(const char *const *bufs, const size_t *lens
 rb200_set_t *rb200_set_run_optimize(const rb200_set_t *s, int mode);
 int rb200_set_to_uint32(const rb200_set_t *s, uint32_t **vals, uint64_t **off);
 void rb200_values_free(uint32_t *vals, uint64_t *off);
+/* The reference's roaring_bitmap_of_ptr, src/roaring.c:195, for every bitmap of a batch, built on the device:
+ * bitmap i = of_ptr(off[i+1] - off[i], vals + off[i]), i < n — values in any order, duplicates
+ * allowed (the layout rb200_set_to_uint32 returns).  Returns a new resident set, NULL on error.
+ * _device: vals / off in device memory of the library's device, read on the library stream and
+ * not modified (the caller orders its writes before the call). */
+rb200_set_t *rb200_set_from_uint32(const uint32_t *vals, const uint64_t *off, size_t n);
+rb200_set_t *rb200_set_from_uint32_device(const uint32_t *d_vals, const uint64_t *d_off, size_t n);
 
 /* Free n host bitmaps (e.g. the results of rb200_set_download_all) using several threads. */
 void rb200_bitmaps_free(roaring_bitmap_t **bitmaps, size_t n);
