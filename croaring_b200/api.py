@@ -148,6 +148,19 @@ def lib():
     sig("rb200_or_many_sharded", _P, _P, _P, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, _P,
         _P, C.POINTER(C.c_uint64))
     sig("rb200_last_collective_ms", C.c_float)
+    sig("rb200_set64_upload_serialized", _P, _P, _P, C.c_size_t)
+    sig("rb200_set64_upload", _P, _P, C.c_size_t)
+    sig("rb200_set64_from_uint64", _P, _P, _P, C.c_size_t)
+    sig("rb200_set64_from_uint64_device", _P, _P, _P, C.c_size_t)
+    sig("rb200_set64_free", None, _P)
+    sig("rb200_set64_count", C.c_size_t, _P)
+    sig("rb200_set64_cardinalities", C.c_int, _P, _P)
+    sig("rb200_set64_batch_op", _P, C.c_int, _P, _P, _P, _P, C.c_size_t)
+    sig("rb200_set64_batch_and_cardinality", C.c_int, _P, _P, _P, _P, C.c_size_t, _P)
+    sig("rb200_set64_run_optimize", _P, _P, C.c_int)
+    sig("rb200_set64_serialize", C.c_int, _P, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)),
+        C.POINTER(C.POINTER(C.c_uint64)))
+    sig("rb200_set64_download_all", C.c_int, _P, _P)
     _lib = L
     return L
 
@@ -798,3 +811,121 @@ class DeviceSet:
         if lib().rb200_set_download_all(self.ptr, out) != 0:
             raise RB200Error(last_error())
         return [Bitmap(out[i]) for i in range(n)]
+
+
+def _values_u64(a):
+    """1-D integer values as a contiguous uint64 array (refused if any lies outside [0, 2^64))."""
+    a = np.asarray(a)
+    if a.ndim != 1 or (a.size and a.dtype.kind not in "iu"):
+        raise RB200Error(f"values must be 1-D integer arrays, got {a.dtype} with shape {a.shape}")
+    if a.size and a.dtype.kind == "i" and int(a.min()) < 0:
+        raise RB200Error("values must lie in [0, 2^64)")
+    return np.ascontiguousarray(a, dtype=np.uint64)
+
+
+def _serialized(fn, ptr, n):
+    buf = C.c_void_p()
+    off = C.POINTER(C.c_uint64)()
+    ln = C.POINTER(C.c_uint64)()
+    if fn(ptr, C.byref(buf), C.byref(off), C.byref(ln)) != 0:
+        raise RB200Error(last_error())
+    out = [C.string_at(buf.value + off[i], ln[i]) for i in range(n)]
+    lib().rb200_serialized_free(buf, off, ln)
+    return out
+
+
+class DeviceSet64:
+    """An ordered collection of 64-bit bitmaps (roaring64_bitmap_t) resident in HBM (rb200_set64_t*)."""
+
+    def __init__(self, ptr):
+        if not ptr:
+            raise RB200Error(last_error() or "null set")
+        self.ptr = ptr
+
+    @classmethod
+    def from_serialized(cls, blobs):
+        """blobs: list of roaring64_bitmap_portable_serialize bytes."""
+        arr, lens, n = _blob_args(blobs)
+        return cls(lib().rb200_set64_upload_serialized(arr, lens, n))
+
+    @classmethod
+    def from_values(cls, values, offsets=None):
+        """roaring64_bitmap_of_ptr of every bitmap, built on the device (no run containers: chain
+        .run_optimize() for those).  values: a list of 1-D integer arrays, one per bitmap; or one flat
+        array with n + 1 offsets; or a CUDA torch tensor of int64 / uint64 values (its bits read as
+        uint64) with offsets as a CUDA or CPU tensor, read in place on the library stream."""
+        if getattr(values, "is_cuda", False):
+            return cls._from_device_values(values, offsets)
+        if offsets is None:
+            arrays = [np.asarray(a).reshape(-1) for a in values]
+            offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
+            np.cumsum([a.size for a in arrays], out=offs[1:])
+            flat = _values_u64(np.concatenate([_values_u64(a) for a in arrays]) if arrays else np.zeros(0, np.uint64))
+        else:
+            flat = _values_u64(values)
+            offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
+            if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
+                raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
+        return cls(lib().rb200_set64_from_uint64(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+
+    @classmethod
+    def _from_device_values(cls, values, offsets):
+        import torch
+        if values.dtype not in (torch.int64, torch.uint64) or values.dim() != 1 or not values.is_contiguous():
+            raise RB200Error("device values must be a contiguous 1-D int64 / uint64 CUDA tensor")
+        if offsets is None:
+            raise RB200Error("device values need offsets")
+        offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
+        if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
+            raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
+        last = int(offs[-1].item())
+        if last < 0 or last > values.numel():
+            raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
+        offs = offs.to(values.device).contiguous()
+        if offs is not offsets:   # copied here: on the stream the library reads on
+            torch.cuda.current_stream(values.device).synchronize()
+        return cls(lib().rb200_set64_from_uint64_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
+
+    def free(self):
+        if self.ptr:
+            lib().rb200_set64_free(self.ptr)
+        self.ptr = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+    def __len__(self):
+        return int(lib().rb200_set64_count(self.ptr))
+
+    def op(self, op, other, ia, ib):
+        """result[k] = self[ia[k]] op other[ib[k]] as a new DeviceSet64 (op: and / or / xor / andnot)."""
+        ia, ib = _u32(ia), _u32(ib)
+        assert ia.shape == ib.shape
+        code = OPS[op] if isinstance(op, str) else op
+        return DeviceSet64(lib().rb200_set64_batch_op(code, self.ptr, other.ptr, ia.ctypes.data, ib.ctypes.data,
+                                                      ia.size))
+
+    def and_cardinality(self, other, ia, ib):
+        ia, ib = _u32(ia), _u32(ib)
+        out = np.zeros(ia.size, dtype=np.uint64)
+        if lib().rb200_set64_batch_and_cardinality(self.ptr, other.ptr, ia.ctypes.data, ib.ctypes.data, ia.size,
+                                                   out.ctypes.data) != 0:
+            raise RB200Error(last_error())
+        return out
+
+    def cardinalities(self):
+        out = np.zeros(len(self), dtype=np.uint64)
+        if lib().rb200_set64_cardinalities(self.ptr, out.ctypes.data) != 0:
+            raise RB200Error(last_error())
+        return out
+
+    def run_optimize(self, mode=1):
+        """mode 1: roaring64_bitmap_run_optimize of every bitmap; mode 0: the run containers removed."""
+        return DeviceSet64(lib().rb200_set64_run_optimize(self.ptr, int(mode)))
+
+    def serialize_all(self):
+        """roaring64_bitmap_portable_serialize bytes of every bitmap, written on the device, one D2H."""
+        return _serialized(lib().rb200_set64_serialize, self.ptr, len(self))

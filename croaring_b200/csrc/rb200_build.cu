@@ -16,6 +16,10 @@
 //   k_build_bitmaps  bm_beg / bm_cnt by binary search of the bitmap's first position
 //   k_build_write    warp per container: distinct low halves compacted by ballot + scan into an
 //                    array, or OR-ed into the warp's 8 KiB accumulator and stored as a bitset
+// roaring64_bitmap_of_ptr (src/roaring64.c:523-620) adds through the same container_add per 48-bit
+// key, so a 64-bit batch is first split into high-32 buckets (k_build_measure<uint64_t> counts them
+// and flags unsorted input, k_build64_split writes the low halves and the bucket starts) and every
+// bucket is then one sorted segment of the 32-bit steps above.
 // CUB (NVIDIA's library shipped with the toolkit) is used for the sort and the two scans only, and
 // only in this file.
 #include <cub/device/device_scan.cuh>
@@ -67,20 +71,26 @@ __device__ __forceinline__ void tile_bitmaps(const uint64_t *__restrict__ off, u
 
 // Position p (< N) of bitmap *b (advanced from the previous position of this thread): does it start
 // a container (first value of its bitmap or a new high half), and do the values decrease there?
-__device__ __forceinline__ bool position_starts(const uint32_t *__restrict__ v, const uint64_t *__restrict__ off,
-                                                uint32_t &b, uint32_t b_hi, uint64_t p, uint32_t &x, bool &decreases) {
+// T = uint32_t: the high half is the 16-bit key of a container; T = uint64_t: the high 32 bits of a
+// 64-bit value, the bucket of roaring64's portable format.
+template <typename T>
+__device__ __forceinline__ bool position_starts(const T *__restrict__ v, const uint64_t *__restrict__ off,
+                                                uint32_t &b, uint32_t b_hi, uint64_t p, T &x, bool &decreases) {
+    constexpr int HALF = 4 * sizeof(T);
     if (off[b + 1] <= p) b = find_bitmap(off, b + 1, b_hi, p);
     x = v[p];
     const bool first = p == off[b];
-    const uint32_t prev = first ? 0u : v[p - 1];
+    const T prev = first ? (T)0 : v[p - 1];
     decreases = !first && x < prev;
-    return first || (x >> 16) != (prev >> 16);
+    return first || (x >> HALF) != (prev >> HALF);
 }
 
-// Container starts per tile (tile_cnt[tile]); *unsorted |= 1 when some bitmap's values decrease,
-// | 2 when that bitmap holds 2^31 values or more (more than one sort call can take).
+// Container (T = uint32_t) or bucket (T = uint64_t) starts per tile (tile_cnt[tile]); *unsorted |= 1
+// when some bitmap's values decrease, | 2 when that bitmap holds 2^31 values or more (more than one
+// sort call can take).
+template <typename T>
 __global__ void __launch_bounds__(BUILD_THREADS)
-k_build_measure(const uint32_t *__restrict__ v, const uint64_t *__restrict__ off, uint32_t n, uint64_t N,
+k_build_measure(const T *__restrict__ v, const uint64_t *__restrict__ off, uint32_t n, uint64_t N,
                 uint64_t *__restrict__ tile_cnt, uint32_t *unsorted) {
     __shared__ uint32_t s_cnt[BUILD_WARPS];
     const uint64_t t0 = (uint64_t)blockIdx.x * BUILD_TILE;
@@ -91,7 +101,7 @@ k_build_measure(const uint32_t *__restrict__ v, const uint64_t *__restrict__ off
     for (int k = 0; k < BUILD_ITEMS; k++) {
         const uint64_t p = t0 + (uint64_t)k * BUILD_THREADS + threadIdx.x;
         if (p >= N) break;
-        uint32_t x;
+        T x;
         bool dec;
         starts += position_starts(v, off, b, b_hi, p, x, dec) ? 1u : 0u;
         if (dec) bad |= (off[b + 1] - off[b] >= (1ull << 31)) ? 3u : 1u;
@@ -124,7 +134,7 @@ k_build_emit(const uint32_t *__restrict__ v, const uint64_t *__restrict__ off, u
         const uint64_t p = t0 + (uint64_t)k * BUILD_THREADS + threadIdx.x;
         uint32_t x = 0;
         bool dec, start = false;
-        if (p < N) start = position_starts(v, off, b, b_hi, p, x, dec);
+        if (p < N) start = position_starts<uint32_t>(v, off, b, b_hi, p, x, dec);
         const unsigned m = __ballot_sync(FULLMASK, start);
         if (lane == 0) s_w[k & 1][warp] = __popc(m);
         __syncthreads();   // s_w[k & 1] is rewritten two chunks later, after the next chunk's barrier
@@ -139,6 +149,47 @@ k_build_emit(const uint32_t *__restrict__ v, const uint64_t *__restrict__ off, u
             const uint64_t c = base + pre + __popc(m & lanemask_lt());
             c_pos[c] = p;
             c_key[c] = (uint16_t)(x >> 16);
+        }
+        base += tot;
+    }
+}
+
+// 64-bit values (tile_base = exclusive scan of k_build_measure<uint64_t>'s bucket starts): the low
+// halves of every position go to lo[p]; the first position and the high 32 bits of every bucket to
+// b_pos / b_high, compacted by ballot in position order.  The buckets of a sorted batch are then
+// sorted 32-bit segments, the input of the 32-bit builder.
+__global__ void __launch_bounds__(BUILD_THREADS)
+k_build64_split(const uint64_t *__restrict__ v, const uint64_t *__restrict__ off, uint32_t n, uint64_t N,
+                const uint64_t *__restrict__ tile_base, uint32_t *__restrict__ lo, uint64_t *__restrict__ b_pos,
+                uint32_t *__restrict__ b_high) {
+    __shared__ uint32_t s_w[2][BUILD_WARPS];
+    const uint64_t t0 = (uint64_t)blockIdx.x * BUILD_TILE;
+    uint32_t b, b_hi;
+    tile_bitmaps(off, n, N, t0, b, b_hi);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint64_t base = tile_base[blockIdx.x];
+    for (int k = 0; k < BUILD_ITEMS; k++) {   // striped as in k_build_emit
+        const uint64_t p = t0 + (uint64_t)k * BUILD_THREADS + threadIdx.x;
+        uint64_t x = 0;
+        bool dec, start = false;
+        if (p < N) {
+            start = position_starts<uint64_t>(v, off, b, b_hi, p, x, dec);
+            lo[p] = (uint32_t)x;
+        }
+        const unsigned m = __ballot_sync(FULLMASK, start);
+        if (lane == 0) s_w[k & 1][warp] = __popc(m);
+        __syncthreads();
+        uint32_t pre = 0, tot = 0;
+#pragma unroll
+        for (int w = 0; w < BUILD_WARPS; w++) {
+            const uint32_t c = s_w[k & 1][w];
+            pre += w < warp ? c : 0u;
+            tot += c;
+        }
+        if (start) {
+            const uint64_t c = base + pre + __popc(m & lanemask_lt());
+            b_pos[c] = p;
+            b_high[c] = (uint32_t)(x >> 32);
         }
         base += tot;
     }
@@ -266,7 +317,21 @@ uint64_t build_tile_count(uint64_t N) { return build_tiles(N); }
 void launch_build_measure(const uint32_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
                           uint32_t *unsorted, cudaStream_t s) {
     if (!N) return;
-    k_build_measure<<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_cnt, unsorted);
+    k_build_measure<uint32_t><<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_cnt, unsorted);
+    g_launches++;
+}
+
+void launch_build64_measure(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
+                            uint32_t *unsorted, cudaStream_t s) {
+    if (!N) return;
+    k_build_measure<uint64_t><<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_cnt, unsorted);
+    g_launches++;
+}
+
+void launch_build64_split(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, const uint64_t *tile_base,
+                          uint32_t *lo, uint64_t *b_pos, uint32_t *b_high, cudaStream_t s) {
+    if (!N) return;
+    k_build64_split<<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_base, lo, b_pos, b_high);
     g_launches++;
 }
 
@@ -310,8 +375,9 @@ bool build_scan(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *ou
 // Sort the values of segments [0, nseg) of a chunk (off: nseg + 1 absolute offsets in device memory,
 // off[nseg] - off[0] < 2^31) from in + off[0] into out + off[0].  rel: nseg + 1 ints of scratch.
 // temp == nullptr: *temp_bytes receives the scratch size (items = off[nseg] - off[0]).
-bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint32_t *in, uint32_t *out, const uint64_t *off,
-                      uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s) {
+template <typename T>
+static bool sort_chunk(void *temp, size_t *temp_bytes, const T *in, T *out, const uint64_t *off, uint64_t first,
+                       uint64_t items, uint32_t nseg, int *rel, cudaStream_t s) {
     if (temp) {
         k_build_rel_offsets<<<(nseg + 256) / 256, 256, 0, s>>>(off, nseg, rel);
         g_launches++;
@@ -320,6 +386,14 @@ bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint32_t *in, uint32
                                                              (int)nseg, rel, rel + 1, s);
     if (temp) g_launches++;
     return e == cudaSuccess;
+}
+bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint32_t *in, uint32_t *out, const uint64_t *off,
+                      uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s) {
+    return sort_chunk(temp, temp_bytes, in, out, off, first, items, nseg, rel, s);
+}
+bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *out, const uint64_t *off,
+                      uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s) {
+    return sort_chunk(temp, temp_bytes, in, out, off, first, items, nseg, rel, s);
 }
 
 }  // namespace rb200

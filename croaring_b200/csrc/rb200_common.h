@@ -329,6 +329,24 @@ void launch_build_write(const uint32_t *v, const uint64_t *c_pos, uint64_t nc, u
 bool build_scan(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *out, uint64_t n, cudaStream_t s);
 bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint32_t *in, uint32_t *out, const uint64_t *off,
                       uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s);
+bool build_sort_chunk(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *out, const uint64_t *off,
+                      uint64_t first, uint64_t items, uint32_t nseg, int *rel, cudaStream_t s);
+// roaring64_bitmap_of_ptr: high-32 bucket starts per tile (+ the unsorted flags of launch_build_measure),
+// then the low halves (lo, N entries) and every bucket's first position and high 32 bits
+void launch_build64_measure(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
+                            uint32_t *unsorted, cudaStream_t s);
+void launch_build64_split(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, const uint64_t *tile_base,
+                          uint32_t *lo, uint64_t *b_pos, uint32_t *b_high, cudaStream_t s);
+// 64-bit portable emission of a set of 64-bit bitmaps whose buckets are the bitmaps of an inner set:
+// per 64-bit bitmap i (buckets [b_beg[i], b_beg[i] + b_cnt[i])) its blob size (exact and 16-byte
+// rounded) from the buckets' exact 32-bit sizes, skipping empty buckets; then, with off = the scan of
+// the rounded sizes, the u64 bucket counts and u32 high words, and boff[j] = where bucket j's 32-bit
+// blob goes (empty or unreferenced buckets: `scratch`, a spare 16 bytes past the blobs)
+void launch_r64_ser_sizes(const uint32_t *b_beg, const uint32_t *b_cnt, uint32_t n, const uint32_t *bm_cnt,
+                          const uint32_t *exact, uint64_t *sizes16, uint64_t *exact64, cudaStream_t s);
+void launch_r64_ser_layout(const uint32_t *b_beg, const uint32_t *b_cnt, const uint32_t *high, uint32_t n,
+                           uint32_t nbuckets, const uint32_t *bm_cnt, const uint32_t *exact, const uint64_t *off,
+                           uint64_t *boff, uint8_t *dst, cudaStream_t s);
 
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
                      uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,

@@ -2818,22 +2818,23 @@ int rb200_set_to_uint32(const rb200_set_t *S, uint32_t **vals, uint64_t **off_ou
 
 void rb200_values_free(uint32_t *vals, uint64_t *off) { rb200_serialized_free((char *)vals, off, nullptr); }
 
-// Arguments of rb200_set_from_uint32*: n < 2^32 bitmaps; n + 1 offsets, off[0] == 0, non-decreasing.
-static bool check_bitmap_count(size_t n) {
+// Arguments of rb200_set_from_uint32* / rb200_set64_from_uint64*: n < 2^32 bitmaps; n + 1 offsets,
+// off[0] == 0, non-decreasing.  `what` names the entry point in the message.
+static bool check_bitmap_count(size_t n, const char *what = "set_from_uint32") {
     if (n <= 0xffffffffull) return true;
-    t_err = "set_from_uint32: " + std::to_string((uint64_t)n) + " bitmaps, at most 2^32 - 1 fit in a set";
+    t_err = std::string(what) + ": " + std::to_string((uint64_t)n) + " bitmaps, at most 2^32 - 1 fit in a set";
     return false;
 }
-static bool check_value_offsets(const uint64_t *off, size_t n) {
-    if (!check_bitmap_count(n)) return false;
-    if (!off) { t_err = "set_from_uint32: offsets are NULL"; return false; }
+static bool check_value_offsets(const uint64_t *off, size_t n, const char *what = "set_from_uint32") {
+    if (!check_bitmap_count(n, what)) return false;
+    if (!off) { t_err = std::string(what) + ": offsets are NULL"; return false; }
     if (off[0] != 0) {
-        t_err = "set_from_uint32: offsets must start at 0 (off[0] = " + std::to_string(off[0]) + ")";
+        t_err = std::string(what) + ": offsets must start at 0 (off[0] = " + std::to_string(off[0]) + ")";
         return false;
     }
     for (size_t i = 0; i < n; i++)
         if (off[i + 1] < off[i]) {
-            t_err = "set_from_uint32: offsets decrease at bitmap " + std::to_string((uint64_t)i) + " (off[" +
+            t_err = std::string(what) + ": offsets decrease at bitmap " + std::to_string((uint64_t)i) + " (off[" +
                     std::to_string((uint64_t)i) + "] = " + std::to_string(off[i]) + ", off[" +
                     std::to_string((uint64_t)i + 1) + "] = " + std::to_string(off[i + 1]) + ")";
             return false;
@@ -2841,25 +2842,84 @@ static bool check_value_offsets(const uint64_t *off, size_t n) {
     return true;
 }
 
+// Segmented sort of src (n segments: h_off on the host, d_off on the device) into *sorted, a new device
+// buffer of h_off[n] values; the input stays as it was.  cub sorts fewer than 2^31 values per call, so
+// the segments go in chunks of that size; a segment too large for one call is sorted already (the
+// measure pass refuses it otherwise) and is copied.  d_temp / temp_bytes: the caller's scratch, grown here.
+extern "C++" {
+template <typename T>
+static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d_off, size_t n, T **sorted,
+                          void *&d_temp, size_t &temp_bytes) {
+    struct Chunk { uint64_t s0, s1; bool copy; };
+    std::vector<Chunk> chunks;
+    const uint64_t LIM = (1ull << 31) - 1, N = h_off[n];
+    for (uint64_t s0 = 0; s0 < n;) {
+        uint64_t s1 = s0;
+        while (s1 < n && h_off[s1 + 1] - h_off[s0] <= LIM && s1 - s0 < LIM - 1) s1++;
+        if (s1 == s0) { chunks.push_back({s0, s0 + 1, true}); s0++; continue; }
+        chunks.push_back({s0, s1, false});
+        s0 = s1;
+    }
+    size_t sort_bytes = 0;
+    uint64_t max_seg = 0;
+    bool ok = true;
+    for (const Chunk &c : chunks) {
+        const uint64_t items = h_off[c.s1] - h_off[c.s0];
+        if (c.copy || !items) continue;
+        size_t b = 0;
+        if (!build_sort_chunk(nullptr, &b, src, (T *)nullptr, nullptr, h_off[c.s0], items, (uint32_t)(c.s1 - c.s0),
+                              nullptr, g.stream)) { ok = false; break; }
+        sort_bytes = std::max(sort_bytes, b);
+        max_seg = std::max(max_seg, c.s1 - c.s0);
+    }
+    if (ok && sort_bytes > temp_bytes) {
+        dev_free(d_temp, temp_bytes);
+        temp_bytes = sort_bytes;
+        ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
+    }
+    const size_t rel_bytes = 4 * (max_seg + 1);
+    int *d_rel = nullptr;
+    ok = ok && (*sorted = (T *)dev_alloc(sizeof(T) * N)) && (d_rel = (int *)dev_alloc(rel_bytes));
+    for (size_t k = 0; k < chunks.size() && ok; k++) {
+        const Chunk &c = chunks[k];
+        const uint64_t first = h_off[c.s0], items = h_off[c.s1] - first;
+        if (!items) continue;
+        if (c.copy) {
+            ok = cudaMemcpyAsync(*sorted + first, src + first, sizeof(T) * items, cudaMemcpyDeviceToDevice,
+                                 g.stream) == cudaSuccess;
+        } else {
+            size_t b = temp_bytes;
+            ok = build_sort_chunk(d_temp, &b, src, *sorted, d_off + c.s0, first, items, (uint32_t)(c.s1 - c.s0), d_rel,
+                                  g.stream);
+        }
+    }
+    dev_free(d_rel, rel_bytes);   // stream-ordered reuse only
+    return ok;
+}
+}  // extern "C++"
+
 // roaring_bitmap_of_ptr of every bitmap (rb200_build.cu).  Values come from the host (h_vals, staged
-// through pinned chunks) or from the device (d_in, read in place); h_off are checked offsets.
-static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in, const uint64_t *h_off, size_t n) {
-    const uint64_t N = h_off[n];
+// through pinned chunks) or from the device (d_in, read in place).  Offsets: h_off, checked host
+// offsets; or d_off_in, device offsets of N values in segments that are sorted already (the buckets of
+// the 64-bit builder), which are never sorted again.
+static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in, const uint64_t *h_off, size_t n,
+                                   const uint64_t *d_off_in = nullptr, uint64_t N_in = 0) {
+    const uint64_t N = h_off ? h_off[n] : N_in;
     const uint64_t ntiles = build_tile_count(N);
     if (ntiles >= (1ull << 31) - 1) { t_err = "set_from_uint32: too many values for one call"; return nullptr; }
-    uint64_t *d_off = (uint64_t *)dev_alloc(8 * (n + 1));
+    uint64_t *d_off = d_off_in ? nullptr : (uint64_t *)dev_alloc(8 * (n + 1));
     uint32_t *d_vals = h_vals ? (uint32_t *)dev_alloc(4 * N) : nullptr, *d_sorted = nullptr;
     uint64_t *d_tcnt = (uint64_t *)dev_alloc(8 * (ntiles + 1)), *d_tbase = (uint64_t *)dev_alloc(8 * (ntiles + 1));
     uint32_t *d_flag = (uint32_t *)dev_alloc(4);
     uint64_t *h_meta = (uint64_t *)pin_alloc(16);
     uint64_t *d_cpos = nullptr, *d_slot = nullptr;
-    int *d_rel = nullptr;
     void *d_temp = nullptr;
-    size_t temp_bytes = 0, scan_bytes = 0, rel_bytes = 0;
+    size_t temp_bytes = 0, scan_bytes = 0;
     uint64_t nc = 0;
     rb200_set *s = nullptr;
-    bool ok = d_off && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
-              cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    bool ok = (d_off || d_off_in) && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
+              (d_off_in || cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess);
+    const uint64_t *offs = d_off_in ? d_off_in : d_off;
     if (ok && h_vals && N) {
         H2DStager stage((uint8_t *)d_vals);
         ok = stage.ok && stage.put(h_vals, 4 * N) && stage.flush();
@@ -2876,7 +2936,7 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
             if (!(d_temp = dev_alloc(temp_bytes))) return false;
         }
         scan_bytes = b;
-        launch_build_measure(src, d_off, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
+        launch_build_measure(src, offs, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
         return build_scan(d_temp, &scan_bytes, d_tcnt, d_tbase, ntiles + 1, g.stream) &&
                cudaMemcpyAsync(h_meta, d_tbase + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
                cudaMemcpyAsync(h_meta + 1, d_flag, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
@@ -2885,59 +2945,21 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
     ok = ok && cudaMemsetAsync(d_flag, 0, 4, g.stream) == cudaSuccess &&
          cudaMemsetAsync(d_tcnt + ntiles, 0, 8, g.stream) == cudaSuccess && measure();
     const uint32_t unsorted = ok ? (uint32_t)h_meta[1] : 0u;
+    if (ok && unsorted && !h_off) {
+        t_err = "internal: presorted segments are not sorted";
+        ok = false;
+    }
     if (ok && (unsorted & 2u)) {
         t_err = "set_from_uint32: a bitmap of 2^31 values or more is not sorted; pass it sorted";
         ok = false;
     }
     if (ok && unsorted) {
-        // segmented sort into scratch (the input stays as it was), in calls of < 2^31 values each;
-        // a bitmap too large for one call is sorted already (else the flag above) and is copied
-        struct Chunk { uint64_t s0, s1; bool copy; };
-        std::vector<Chunk> chunks;
-        const uint64_t LIM = (1ull << 31) - 1;
-        for (uint64_t s0 = 0; s0 < n;) {
-            uint64_t s1 = s0;
-            while (s1 < n && h_off[s1 + 1] - h_off[s0] <= LIM && s1 - s0 < LIM - 1) s1++;
-            if (s1 == s0) { chunks.push_back({s0, s0 + 1, true}); s0++; continue; }
-            chunks.push_back({s0, s1, false});
-            s0 = s1;
-        }
-        size_t sort_bytes = 0;
-        uint64_t max_seg = 0;
-        for (const Chunk &c : chunks) {
-            const uint64_t items = h_off[c.s1] - h_off[c.s0];
-            if (c.copy || !items) continue;
-            size_t b = 0;
-            if (!build_sort_chunk(nullptr, &b, src, nullptr, nullptr, h_off[c.s0], items, (uint32_t)(c.s1 - c.s0),
-                                  nullptr, g.stream)) { ok = false; break; }
-            sort_bytes = std::max(sort_bytes, b);
-            max_seg = std::max(max_seg, c.s1 - c.s0);
-        }
-        if (ok && sort_bytes > temp_bytes) {
-            dev_free(d_temp, temp_bytes);
-            temp_bytes = sort_bytes;
-            ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
-        }
-        rel_bytes = 4 * (max_seg + 1);
-        ok = ok && (d_sorted = (uint32_t *)dev_alloc(4 * N)) && (d_rel = (int *)dev_alloc(rel_bytes));
-        for (size_t k = 0; k < chunks.size() && ok; k++) {
-            const Chunk &c = chunks[k];
-            const uint64_t first = h_off[c.s0], items = h_off[c.s1] - first;
-            if (!items) continue;
-            if (c.copy) {
-                ok = cudaMemcpyAsync(d_sorted + first, src + first, 4 * items, cudaMemcpyDeviceToDevice, g.stream) ==
-                     cudaSuccess;
-            } else {
-                size_t b = temp_bytes;
-                ok = build_sort_chunk(d_temp, &b, src, d_sorted, d_off + c.s0, first, items, (uint32_t)(c.s1 - c.s0),
-                                      d_rel, g.stream);
-            }
-        }
+        ok = sort_segments(src, h_off, d_off, n, &d_sorted, d_temp, temp_bytes);
         if (ok) {
             src = d_sorted;
             ok = measure();
-            if (!ok && t_err.empty()) t_err = "set_from_uint32: segmented sort failed";
         }
+        if (!ok && t_err.empty()) t_err = "set_from_uint32: segmented sort failed";
     }
     if (ok) {
         nc = h_meta[0];
@@ -2956,7 +2978,7 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
             ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
         }
         if (ok) {
-            launch_build_emit(src, d_off, (uint32_t)n, N, d_tbase, s->out().c_key, d_cpos, g.stream);
+            launch_build_emit(src, offs, (uint32_t)n, N, d_tbase, s->out().c_key, d_cpos, g.stream);
             launch_build_slots(d_cpos, nc, N, d_slot, g.stream);
             b = temp_bytes;
             ok = build_scan(d_temp, &b, d_slot, s->out().c_off, nc, g.stream);
@@ -2966,7 +2988,7 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
         ok = stats_reset();
         if (n && !nc) ok = ok && cudaMemsetAsync(s->out().bm_cnt, 0, 4 * n, g.stream) == cudaSuccess &&
                            cudaMemsetAsync(s->out().bm_beg, 0, 4 * n, g.stream) == cudaSuccess;
-        if (nc) launch_build_bitmaps(d_off, (uint32_t)n, d_cpos, nc, s->out().bm_beg, s->out().bm_cnt, g.stream);
+        if (nc) launch_build_bitmaps(offs, (uint32_t)n, d_cpos, nc, s->out().bm_beg, s->out().bm_cnt, g.stream);
         launch_build_write(src, d_cpos, nc, N, s->out(), s->slab_cap, g.d_stats, g.stream);
         launch_bitmap_figures(s->out(), (uint32_t)n, g.d_stats, g.stream);
         ok = ok && stats_fetch();
@@ -2996,7 +3018,6 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
     dev_free(d_cpos, 8 * nc);
     dev_free(d_slot, 8 * nc);
     dev_free(d_temp, temp_bytes);
-    dev_free(d_rel, rel_bytes);
     pin_free(h_meta, 16);
     if (!ok) {
         if (t_err.empty()) t_err = "set_from_uint32 failed";
@@ -3574,13 +3595,29 @@ void roaring_bitmap_flip_inplace(roaring_bitmap_t *r1, uint64_t range_start, uin
     }
 }
 
-// ---- 64-bit bitmaps through their portable format (src/roaring64.c) -------------------------
-// roaring64_bitmap_{and,or,xor,andnot} (roaring64.c:1332, 1541, 1663, 1809) apply the same
-// container cells to equal high-48-bit keys; the 64-bit portable format (roaring64.c:2262-2395)
-// stores one ordinary 32-bit portable bitmap per high-32 "bucket".  Here every bucket of every
-// input becomes one bitmap of ONE resident set, matching buckets of a pair become one pair of the
-// batched kernel (unmatched ones are paired with an empty bitmap = pass-through), and the result
-// buckets are serialized on the device and stitched back into 64-bit blobs.
+// ---- 64-bit bitmaps resident on the device (src/roaring64.c) -------------------------------
+// roaring64_bitmap_{and,or,xor,andnot} (roaring64.c:1332, 1541, 1663, 1809) apply the same container
+// cells to equal high-48-bit keys, and the 64-bit portable format (roaring64.c:2262-2395) stores one
+// ordinary 32-bit portable bitmap per high-32 "bucket".  So a resident set of 64-bit bitmaps is one
+// ordinary set holding every bucket as a 32-bit bitmap (the inner set: every kernel, mirror and
+// deferred counter of 32-bit sets applies to it) plus a bucket directory: per 64-bit bitmap its range
+// of inner bitmaps, per bucket its high 32 bits.  The inner set always ends with one empty bitmap, the
+// sentinel, in no 64-bit bitmap: a bucket without a partner in the other operand is paired with it.
+// A result may hold empty buckets (x XOR x, AND of disjoint keys); they are never planned, counted or
+// serialized, as the reference never keeps an empty container.
+}  // extern "C"
+struct rb200_set64 {
+    rb200_set *inner = nullptr;
+    uint32_t n = 0, nbuckets = 0;   // 64-bit bitmaps; inner bitmaps, the sentinel included
+    uint32_t *h_dir = nullptr;      // pinned host mirror: [b_beg (n) | b_cnt (n) | high (nbuckets)]
+    uint32_t *d_dir = nullptr;      // the same in device memory (copied there when a kernel first needs it)
+    bool dir_on_device = false;
+    size_t dir_bytes = 0;
+    const uint32_t *b_beg() const { return h_dir; }
+    const uint32_t *b_cnt() const { return h_dir + n; }
+    const uint32_t *high() const { return h_dir + 2 * (size_t)n; }
+};
+extern "C" {
 namespace {
 struct R64Bucket { uint32_t high; const char *ptr; size_t len; };
 // length of the 32-bit portable bitmap starting at buf (0 = malformed); header walk only
@@ -3621,77 +3658,463 @@ size_t portable_length(const uint8_t *buf, size_t maxlen) {
     }
     return pos;
 }
-bool parse_r64(const char *buf, size_t len, std::vector<R64Bucket> &out) {
+// The bucket headers of one 64-bit portable blob (roaring64.c:2440-2531); nullptr when they are
+// well formed, else what is wrong.  The buckets' contents are checked by the device parse.
+const char *parse_r64(const char *buf, size_t len, std::vector<R64Bucket> &out) {
     out.clear();
-    if (len < 8) return false;
+    if (len < 8 || !buf) return "shorter than its 8-byte bucket count";
     uint64_t n;
     memcpy(&n, buf, 8);
-    if (n > UINT32_MAX) return false;
+    if (n > UINT32_MAX) return "bucket count above 2^32 - 1";
     size_t pos = 8;
     for (uint64_t i = 0; i < n; i++) {
-        if (pos + 4 > len) return false;
+        if (pos + 4 > len) return "truncated: a bucket header runs past the end";
         R64Bucket b;
         memcpy(&b.high, buf + pos, 4);
         pos += 4;
-        if (i && b.high <= out.back().high) return false;
+        if (i && b.high <= out.back().high) return "the high 32 bits of the buckets are not strictly increasing";
         b.ptr = buf + pos;
         b.len = portable_length((const uint8_t *)buf + pos, len - pos);
-        if (!b.len) return false;
+        if (!b.len) return "a bucket runs past the end of the blob or is not a 32-bit portable bitmap";
         pos += b.len;
         out.push_back(b);
     }
+    return nullptr;
+}
+
+void set64_delete(rb200_set64 *s) {
+    if (!s) return;
+    set_delete(s->inner);
+    pin_free(s->h_dir, s->dir_bytes);
+    dev_free(s->d_dir, s->dir_bytes);
+    delete s;
+}
+// A set of n 64-bit bitmaps over nbuckets inner bitmaps; the caller fills h_dir (or d_dir).
+rb200_set64 *set64_new(uint32_t n, uint32_t nbuckets) {
+    rb200_set64 *s = new rb200_set64();
+    s->n = n;
+    s->nbuckets = nbuckets;
+    s->dir_bytes = 4 * (2 * (size_t)n + nbuckets);
+    s->h_dir = (uint32_t *)pin_alloc(s->dir_bytes);
+    s->d_dir = (uint32_t *)dev_alloc(s->dir_bytes);
+    if (!s->h_dir || !s->d_dir) {
+        set64_delete(s);
+        return nullptr;
+    }
+    return s;
+}
+// The device copy of the directory, for the serialization kernels; a set that is only an operand
+// (the per-call entry points' inputs) never pays this copy.  The caller synchronises the stream
+// before h_dir can be released.
+bool set64_dir_on_device(const rb200_set64 *cs) {
+    rb200_set64 *s = const_cast<rb200_set64 *>(cs);
+    if (s->dir_on_device) return true;
+    if (cudaMemcpyAsync(s->d_dir, s->h_dir, s->dir_bytes, cudaMemcpyHostToDevice, g.stream) != cudaSuccess) {
+        t_err = "set64: directory upload failed";
+        return false;
+    }
+    s->dir_on_device = true;
     return true;
 }
-struct R64Plan {
-    rb200_set *S = nullptr;                 // every bucket of every input + one empty bitmap (last)
-    std::vector<uint32_t> pa, pb, high;     // bucket pairs and their high-32 value
-    std::vector<size_t> first;              // per 64-bit pair: its bucket pairs are [first[p], first[p+1])
-};
-// op < 0: cardinality planning (matched buckets only)
-bool plan_r64(int op, const char *const *a, const size_t *alen, size_t na, const char *const *b,
-              const size_t *blen, size_t nb, const uint32_t *ia, const uint32_t *ib, size_t np, R64Plan &P) {
-    std::vector<std::vector<R64Bucket>> A(na), B(nb);
-    std::vector<size_t> baseA(na), baseB(nb);
+
+// Every bucket of every blob, then the sentinel, as ONE upload_blobs_impl batch (one H2D stream; the
+// device parse checks each bucket fully).  The headers are walked first: malformed input is refused
+// before any CUDA call.
+rb200_set64 *set64_upload_impl(const char *const *bufs, const size_t *lens, size_t n) {
+    if (n > 0xffffffffull) { t_err = "set64: more than 2^32 - 1 bitmaps"; return nullptr; }
+    std::vector<R64Bucket> bk;
     std::vector<const char *> ptrs;
-    std::vector<size_t> lens;
-    for (size_t i = 0; i < na; i++) {
-        if (!parse_r64(a[i], alen[i], A[i])) { t_err = "malformed 64-bit portable bitmap (left) at index " + std::to_string(i); return false; }
-        baseA[i] = ptrs.size();
-        for (auto &x : A[i]) { ptrs.push_back(x.ptr); lens.push_back(x.len); }
-    }
-    for (size_t i = 0; i < nb; i++) {
-        if (!parse_r64(b[i], blen[i], B[i])) { t_err = "malformed 64-bit portable bitmap (right) at index " + std::to_string(i); return false; }
-        baseB[i] = ptrs.size();
-        for (auto &x : B[i]) { ptrs.push_back(x.ptr); lens.push_back(x.len); }
+    std::vector<size_t> blens;
+    std::vector<uint32_t> cnt(n), highs;
+    for (size_t i = 0; i < n; i++) {
+        if (const char *why = parse_r64(bufs[i], lens[i], bk)) {
+            t_err = "malformed 64-bit portable bitmap at index " + std::to_string((uint64_t)i) + ": " + why;
+            return nullptr;
+        }
+        cnt[i] = (uint32_t)bk.size();
+        for (const R64Bucket &b : bk) {
+            ptrs.push_back(b.ptr);
+            blens.push_back(b.len);
+            highs.push_back(b.high);
+        }
+        if (ptrs.size() >= 0xffffffffull) { t_err = "set64: more than 2^32 - 2 buckets"; return nullptr; }
     }
     static const uint32_t empty_blob[2] = {SERIAL_COOKIE_NO_RUN, 0};
-    const uint32_t EMPTY = (uint32_t)ptrs.size();
     ptrs.push_back((const char *)empty_blob);
-    lens.push_back(8);
-    P.first.assign(1, 0);
+    blens.push_back(8);
+    highs.push_back(0);
+    if (!ctx_init()) return nullptr;
+    rb200_set64 *s = set64_new((uint32_t)n, (uint32_t)ptrs.size());
+    if (!s) return nullptr;
+    uint32_t *beg = s->h_dir, *bc = s->h_dir + n;
+    for (size_t i = 0, b = 0; i < n; b += cnt[i], i++) {
+        beg[i] = (uint32_t)b;
+        bc[i] = cnt[i];
+    }
+    memcpy(s->h_dir + 2 * n, highs.data(), 4 * highs.size());
+    s->inner = upload_blobs_impl(ptrs.data(), blens.data(), ptrs.size(), false);
+    if (!s->inner) {
+        set64_delete(s);
+        return nullptr;
+    }
+    return s;
+}
+
+// Bucket pairs of result[p] = A[ia[p]] op B[ib[p]] from the host mirrors: the two high-32 lists
+// merged, empty buckets skipped; a bucket without partner is paired with the other inner set's
+// sentinel (OR, XOR, and ANDNOT's left side) or dropped (AND).  cnt[p]: bucket pairs of result p.
+struct Plan64 { std::vector<uint32_t> pa, pb, high, cnt; };
+bool plan64(int op, const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia, const uint32_t *ib, size_t np,
+            Plan64 &P) {
+    if (!ensure_mirrors(A->inner) || !ensure_mirrors(B->inner)) return false;
+    const uint32_t *ca = A->inner->h_cnt.data(), *cb = B->inner->h_cnt.data();
+    const uint32_t *ha = A->high(), *hb = B->high();
+    const uint32_t EA = A->nbuckets - 1, EB = B->nbuckets - 1;
+    P.cnt.resize(np);
     for (size_t p = 0; p < np; p++) {
-        if (ia[p] >= na || ib[p] >= nb) { t_err = "pair index out of range"; return false; }
-        const auto &x = A[ia[p]], &y = B[ib[p]];
-        size_t i = 0, j = 0;
-        while (i < x.size() || j < y.size()) {
-            const bool only1 = j >= y.size() || (i < x.size() && x[i].high < y[j].high);
-            const bool only2 = !only1 && (i >= x.size() || y[j].high < x[i].high);
+        if (ia[p] >= A->n || ib[p] >= B->n) { t_err = "pair index out of range"; return false; }
+        uint32_t i = A->b_beg()[ia[p]], j = B->b_beg()[ib[p]];
+        const uint32_t ie = i + A->b_cnt()[ia[p]], je = j + B->b_cnt()[ib[p]];
+        const size_t first = P.pa.size();
+        for (;;) {
+            while (i < ie && !ca[i]) i++;
+            while (j < je && !cb[j]) j++;
+            if (i >= ie && j >= je) break;
+            const bool only1 = j >= je || (i < ie && ha[i] < hb[j]);
+            const bool only2 = !only1 && (i >= ie || hb[j] < ha[i]);
             const bool keep = only1 ? (op == OP_OR || op == OP_XOR || op == OP_ANDNOT)
                               : only2 ? (op == OP_OR || op == OP_XOR) : true;
             if (keep) {
-                P.pa.push_back(only2 ? EMPTY : (uint32_t)(baseA[ia[p]] + i));
-                P.pb.push_back(only1 ? EMPTY : (uint32_t)(baseB[ib[p]] + j));
-                P.high.push_back(only2 ? y[j].high : x[i].high);
+                P.pa.push_back(only2 ? EA : i);
+                P.pb.push_back(only1 ? EB : j);
+                P.high.push_back(only2 ? hb[j] : ha[i]);
             }
             if (!only2) i++;
             if (!only1) j++;
         }
-        P.first.push_back(P.pa.size());
+        P.cnt[p] = (uint32_t)(P.pa.size() - first);
+        if (P.pa.size() >= 0xffffffffull) {   // + the result's sentinel must fit a 32-bit bitmap index
+            t_err = "set64 batch: more than 2^32 - 2 bucket pairs, split the pair list";
+            return false;
+        }
     }
-    P.S = upload_blobs_impl(ptrs.data(), lens.data(), ptrs.size(), false);
-    return P.S != nullptr;
+    return true;
+}
+
+rb200_set64 *batch_op64_impl(int op, const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia,
+                             const uint32_t *ib, size_t np) {
+    if (!ctx_init()) return nullptr;
+    if (op < 0 || op > 3) { t_err = "bad op"; return nullptr; }
+    if (np > 0xffffffffull) { t_err = "too many pairs"; return nullptr; }
+    Plan64 P;
+    if (!plan64(op, A, B, ia, ib, np, P)) return nullptr;
+    P.pa.push_back(A->nbuckets - 1);   // (sentinel, sentinel): the result's own sentinel
+    P.pb.push_back(B->nbuckets - 1);
+    P.high.push_back(0);
+    rb200_set64 *R = set64_new((uint32_t)np, (uint32_t)P.pa.size());
+    if (!R) return nullptr;
+    for (size_t p = 0, b = 0; p < np; b += P.cnt[p], p++) {
+        R->h_dir[p] = (uint32_t)b;
+        R->h_dir[np + p] = P.cnt[p];
+    }
+    memcpy(R->h_dir + 2 * np, P.high.data(), 4 * P.high.size());
+    R->inner = batch_op_impl(op, A->inner, B->inner, P.pa.data(), P.pb.data(), P.pa.size());
+    if (!R->inner) {
+        set64_delete(R);
+        return nullptr;
+    }
+    return R;
+}
+
+int and_cardinality64_impl(const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia, const uint32_t *ib,
+                           size_t np, uint64_t *out) {
+    if (!ctx_init()) return -1;
+    if (np == 0) return 0;
+    Plan64 P;
+    if (!plan64(OP_AND, A, B, ia, ib, np, P)) return -1;
+    std::vector<uint64_t> c(P.pa.size());
+    if (!P.pa.empty() && rb200_batch_and_cardinality(A->inner, B->inner, P.pa.data(), P.pb.data(), P.pa.size(), c.data()) != 0)
+        return -1;
+    for (size_t p = 0, q = 0; p < np; p++) {
+        uint64_t sum = 0;
+        for (uint32_t k = 0; k < P.cnt[p]; k++) sum += c[q++];
+        out[p] = sum;
+    }
+    return 0;
+}
+
+// Device-side roaring64_bitmap_portable_serialize of every 64-bit bitmap: the buckets' exact 32-bit
+// sizes (k_ser_measure), the 64-bit blob sizes and their scan (k_r64_ser_sizes, k_pack_scan), one read
+// back of the offsets, then the bucket counts, high words and bucket offsets (k_r64_ser_layout) and
+// the buckets themselves (k_ser_write) into one buffer that leaves in one D2H.  Blob starts are
+// 16-byte aligned; blob i = *buf + (*off)[i], (*len)[i] bytes.
+int serialize64_impl(const rb200_set64 *s, char **buf, uint64_t **off_out, uint64_t **len_out) {
+    if (!ctx_init()) return -1;
+    if (!resolve(s->inner)) return -1;
+    const size_t n = s->n, nb = s->nbuckets;
+    *buf = nullptr;
+    *off_out = (uint64_t *)malloc(8 * (n + 1));
+    *len_out = (uint64_t *)malloc(8 * (n + 1));
+    if (!*off_out || !*len_out) {
+        free(*off_out);
+        free(*len_out);
+        *off_out = *len_out = nullptr;
+        t_err = "set64_serialize: host allocation failed";
+        return -1;
+    }
+    (*off_out)[0] = 0;
+    if (n == 0) return 0;
+    const uint32_t *d_beg = s->d_dir, *d_cnt = s->d_dir + n, *d_high = s->d_dir + 2 * n;
+    uint64_t *d_sz = (uint64_t *)dev_alloc(8 * nb), *d_boff = (uint64_t *)dev_alloc(8 * nb);
+    uint32_t *d_exact = (uint32_t *)dev_alloc(4 * nb), *d_hasrun = (uint32_t *)dev_alloc(4 * nb);
+    uint64_t *d_s16 = (uint64_t *)dev_alloc(8 * n), *d_e64 = (uint64_t *)dev_alloc(8 * n),
+             *d_off = (uint64_t *)dev_alloc(8 * (n + 1)), *d_dummy = (uint64_t *)dev_alloc(8 * (n + 1));
+    uint64_t *h_meta = (uint64_t *)pin_alloc(8 * (2 * n + 1));
+    uint8_t *d_blob = nullptr, *h_blob = nullptr;
+    uint64_t total = 0;
+    const SetView v = s->inner->view();
+    bool ok = d_sz && d_boff && d_exact && d_hasrun && d_s16 && d_e64 && d_off && d_dummy && h_meta &&
+              set64_dir_on_device(s);
+    if (ok) {
+        launch_serialize_measure(v, (uint32_t)nb, d_sz, d_exact, d_hasrun, g.stream);
+        launch_r64_ser_sizes(d_beg, d_cnt, (uint32_t)n, v.bm_cnt, d_exact, d_s16, d_e64, g.stream);
+        launch_pack_scan(d_s16, d_cnt, (uint32_t)n, d_off, d_dummy, g.stream);
+        ok = cudaMemcpyAsync(h_meta, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+             cudaMemcpyAsync(h_meta + n + 1, d_e64, 8 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+             cudaStreamSynchronize(g.stream) == cudaSuccess;
+    }
+    if (ok) {
+        total = h_meta[n];
+        memcpy(*off_out, h_meta, 8 * (n + 1));
+        memcpy(*len_out, h_meta + n + 1, 8 * n);
+        d_blob = (uint8_t *)dev_alloc(total + 16);   // + the scratch empty buckets write to
+        h_blob = (uint8_t *)pin_alloc(total);
+        ok = d_blob && h_blob;
+    }
+    if (ok) {
+        launch_r64_ser_layout(d_beg, d_cnt, d_high, (uint32_t)n, (uint32_t)nb, v.bm_cnt, d_exact, d_off, d_boff,
+                              d_blob, g.stream);
+        launch_serialize_write(v, (uint32_t)nb, d_boff, d_hasrun, d_blob, g.stream);
+        ok = cudaMemcpyAsync(h_blob, d_blob, total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+             cudaStreamSynchronize(g.stream) == cudaSuccess && cudaGetLastError() == cudaSuccess;
+    }
+    g.last_download_bytes = total;
+    dev_free(d_sz, 8 * nb);
+    dev_free(d_boff, 8 * nb);
+    dev_free(d_exact, 4 * nb);
+    dev_free(d_hasrun, 4 * nb);
+    dev_free(d_s16, 8 * n);
+    dev_free(d_e64, 8 * n);
+    dev_free(d_off, 8 * (n + 1));
+    dev_free(d_dummy, 8 * (n + 1));
+    dev_free(d_blob, total + 16);
+    pin_free(h_meta, 8 * (2 * n + 1));
+    if (!ok) {
+        pin_free(h_blob, total);
+        free(*off_out);
+        free(*len_out);
+        *off_out = *len_out = nullptr;
+        if (t_err.empty()) t_err = "set64_serialize failed";
+        return -1;
+    }
+    *buf = (char *)h_blob;
+    g_serialized_sizes[h_blob] = total;
+    return 0;
+}
+
+// roaring64_bitmap_of_ptr of every bitmap (rb200_build.cu): values from the host (staged through
+// pinned chunks) or the device (read in place); h_off: checked host offsets.
+rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, const uint64_t *h_off, size_t n) {
+    const uint64_t N = h_off[n];
+    const uint64_t ntiles = build_tile_count(N);
+    if (ntiles >= (1ull << 31) - 1) { t_err = "set64_from_uint64: too many values for one call"; return nullptr; }
+    uint64_t *d_off = (uint64_t *)dev_alloc(8 * (n + 1));
+    uint64_t *d_vals = h_vals ? (uint64_t *)dev_alloc(8 * N) : nullptr, *d_sorted = nullptr;
+    uint64_t *d_tcnt = (uint64_t *)dev_alloc(8 * (ntiles + 1)), *d_tbase = (uint64_t *)dev_alloc(8 * (ntiles + 1));
+    uint32_t *d_flag = (uint32_t *)dev_alloc(4), *d_lo = nullptr;
+    uint64_t *h_meta = (uint64_t *)pin_alloc(32), *d_bpos = nullptr;
+    void *d_temp = nullptr;
+    size_t temp_bytes = 0;
+    uint64_t nbk = 0;
+    rb200_set64 *R = nullptr;
+    bool ok = d_off && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
+              cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    if (ok && h_vals && N) {
+        H2DStager stage((uint8_t *)d_vals);
+        ok = stage.ok && stage.put(h_vals, 8 * N) && stage.flush();
+        ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
+    }
+    const uint64_t *src = h_vals ? d_vals : d_in;
+    // bucket starts per tile, scanned: the total is the bucket count if the values are sorted
+    auto measure = [&]() -> bool {
+        size_t b = 0;
+        if (!build_scan(nullptr, &b, d_tcnt, d_tbase, ntiles + 1, g.stream)) return false;
+        if (b > temp_bytes) {
+            dev_free(d_temp, temp_bytes);
+            temp_bytes = b;
+            if (!(d_temp = dev_alloc(temp_bytes))) return false;
+        }
+        launch_build64_measure(src, d_off, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
+        return build_scan(d_temp, &b, d_tcnt, d_tbase, ntiles + 1, g.stream) &&
+               cudaMemcpyAsync(h_meta, d_tbase + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+               cudaMemcpyAsync(h_meta + 1, d_flag, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+               cudaStreamSynchronize(g.stream) == cudaSuccess;
+    };
+    if (ok) h_meta[1] = 0;
+    ok = ok && cudaMemsetAsync(d_flag, 0, 4, g.stream) == cudaSuccess &&
+         cudaMemsetAsync(d_tcnt + ntiles, 0, 8, g.stream) == cudaSuccess && measure();
+    const uint32_t unsorted = ok ? (uint32_t)h_meta[1] : 0u;
+    if (ok && (unsorted & 2u)) {
+        t_err = "set64_from_uint64: a bitmap of 2^31 values or more is not sorted; pass it sorted";
+        ok = false;
+    }
+    if (ok && unsorted) {
+        ok = sort_segments(src, h_off, d_off, n, &d_sorted, d_temp, temp_bytes);
+        if (ok) {
+            src = d_sorted;
+            ok = measure();
+        }
+        if (!ok && t_err.empty()) t_err = "set64_from_uint64: segmented sort failed";
+    }
+    if (ok) {
+        nbk = h_meta[0];
+        if (nbk >= 0xffffffffull) { t_err = "set64_from_uint64: more than 2^32 - 2 buckets"; ok = false; }
+    }
+    if (ok) ok = (R = set64_new((uint32_t)n, (uint32_t)(nbk + 1))) != nullptr;
+    if (ok) {
+        // bucket k of the inner set = the sorted low halves lo[b_pos[k] .. b_pos[k + 1]); the sentinel
+        // is the empty segment [N, N)
+        uint32_t *d_high = R->d_dir + 2 * n;
+        h_meta[2] = h_meta[3] = N;
+        ok = (d_lo = (uint32_t *)dev_alloc(4 * (N ? N : 1))) && (d_bpos = (uint64_t *)dev_alloc(8 * (nbk + 2))) &&
+             cudaMemcpyAsync(d_bpos + nbk, h_meta + 2, 16, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+             cudaMemsetAsync(d_high + nbk, 0, 4, g.stream) == cudaSuccess;
+        if (ok) {
+            launch_build64_split(src, d_off, (uint32_t)n, N, d_tbase, d_lo, d_bpos, d_high, g.stream);
+            launch_build_bitmaps(d_off, (uint32_t)n, d_bpos, nbk, R->d_dir, R->d_dir + n, g.stream);
+            dev_free(d_vals, 8 * N);     // stream-ordered reuse: the inner build may take their memory
+            dev_free(d_sorted, 8 * N);
+            d_vals = d_sorted = nullptr;
+            R->inner = from_uint32_impl(nullptr, d_lo, nullptr, nbk + 1, d_bpos, N);
+            ok = R->inner && cudaMemcpyAsync(R->h_dir, R->d_dir, R->dir_bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                 cudaStreamSynchronize(g.stream) == cudaSuccess;
+            R->dir_on_device = true;
+        }
+    } else {
+        cudaStreamSynchronize(g.stream);
+    }
+    dev_free(d_off, 8 * (n + 1));
+    dev_free(d_vals, 8 * N);
+    dev_free(d_sorted, 8 * N);
+    dev_free(d_tcnt, 8 * (ntiles + 1));
+    dev_free(d_tbase, 8 * (ntiles + 1));
+    dev_free(d_flag, 4);
+    dev_free(d_lo, 4 * (N ? N : 1));
+    dev_free(d_bpos, 8 * (nbk + 2));
+    dev_free(d_temp, temp_bytes);
+    pin_free(h_meta, 32);
+    if (!ok) {
+        if (t_err.empty()) t_err = "set64_from_uint64 failed";
+        set64_delete(R);
+        return nullptr;
+    }
+    return R;
+}
+
+// a[] then b[] as ONE resident set (one H2D); ib2 = ib shifted past a[]
+rb200_set64 *r64_operands(const char *const *a, const size_t *alen, size_t na, const char *const *b,
+                          const size_t *blen, size_t nb, const uint32_t *ia, const uint32_t *ib, size_t np,
+                          std::vector<uint32_t> &ib2) {
+    if (na + nb > 0xffffffffull) { t_err = "too many bitmaps"; return nullptr; }
+    ib2.resize(np);
+    for (size_t p = 0; p < np; p++) {
+        if (ia[p] >= na || ib[p] >= nb) { t_err = "pair index out of range"; return nullptr; }
+        ib2[p] = (uint32_t)(ib[p] + na);
+    }
+    std::vector<const char *> ptrs(a, a + na);
+    std::vector<size_t> lens(alen, alen + na);
+    ptrs.insert(ptrs.end(), b, b + nb);
+    lens.insert(lens.end(), blen, blen + nb);
+    return set64_upload_impl(ptrs.data(), lens.data(), ptrs.size());
 }
 }  // namespace
+
+rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size_t *lens, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return set64_upload_impl(bufs, lens, n);
+}
+rb200_set64_t *rb200_set64_from_uint64(const uint64_t *vals, const uint64_t *off, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!check_value_offsets(off, n, "set64_from_uint64")) return nullptr;   // before any CUDA call
+    if (!vals && off[n]) { t_err = "set64_from_uint64: values are NULL"; return nullptr; }
+    if (!ctx_init()) return nullptr;
+    static const uint64_t none = 0;
+    return from_uint64_impl(vals ? vals : &none, nullptr, off, n);
+}
+rb200_set64_t *rb200_set64_from_uint64_device(const uint64_t *d_vals, const uint64_t *d_off, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!check_bitmap_count(n, "set64_from_uint64_device")) return nullptr;
+    if (!d_off) { t_err = "set64_from_uint64_device: offsets are NULL"; return nullptr; }
+    if (!ctx_init()) return nullptr;
+    // the offsets are checked on the host before any kernel reads values through them
+    uint64_t *h_off = (uint64_t *)pin_alloc(8 * (n + 1));
+    if (!h_off) return nullptr;
+    rb200_set64 *s = nullptr;
+    if (cudaMemcpyAsync(h_off, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
+        cudaStreamSynchronize(g.stream) != cudaSuccess) {
+        (void)cudaGetLastError();
+        t_err = "set64_from_uint64_device: offsets are not readable device memory of the library's device";
+    } else if (check_value_offsets(h_off, n, "set64_from_uint64_device")) {
+        if (!d_vals && h_off[n]) t_err = "set64_from_uint64_device: values are NULL";
+        else s = from_uint64_impl(nullptr, d_vals, h_off, n);
+    }
+    pin_free(h_off, 8 * (n + 1));
+    return s;
+}
+void rb200_set64_free(rb200_set64_t *s) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    set64_delete(s);
+}
+size_t rb200_set64_count(const rb200_set64_t *s) { return s->n; }
+int rb200_set64_cardinalities(const rb200_set64_t *s, uint64_t *out) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (s->n == 0) return 0;
+    std::vector<uint64_t> c(s->nbuckets);
+    if (rb200_set_cardinalities(s->inner, c.data()) != 0) return -1;
+    for (uint32_t i = 0; i < s->n; i++) {
+        uint64_t sum = 0;
+        for (uint32_t k = 0; k < s->b_cnt()[i]; k++) sum += c[s->b_beg()[i] + k];
+        out[i] = sum;
+    }
+    return 0;
+}
+rb200_set64_t *rb200_set64_batch_op(int op, const rb200_set64_t *A, const rb200_set64_t *B, const uint32_t *ia,
+                                    const uint32_t *ib, size_t npairs) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return batch_op64_impl(op, A, B, ia, ib, npairs);
+}
+int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_t *B, const uint32_t *ia,
+                                      const uint32_t *ib, size_t npairs, uint64_t *out) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return and_cardinality64_impl(A, B, ia, ib, npairs, out);
+}
+rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!ctx_init()) return nullptr;
+    rb200_set64 *R = set64_new(S->n, S->nbuckets);
+    if (!R) return nullptr;
+    memcpy(R->h_dir, S->h_dir, S->dir_bytes);
+    R->inner = convert_impl(S->inner, mode ? 1 : 0);
+    if (!R->inner) {
+        set64_delete(R);
+        return nullptr;
+    }
+    return R;
+}
+int rb200_set64_serialize(const rb200_set64_t *s, char **buf, uint64_t **off, uint64_t **len) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return serialize64_impl(s, buf, off, len);
+}
 
 // result[k] = roaring64 op of (a[ia[k]], b[ib[k]]), all in the 64-bit portable format.  *out is
 // pinned memory owned by the library (blob k at *out + (*off)[k], (*len)[k] bytes); release with
@@ -3704,63 +4127,14 @@ int rb200_r64_batch_op_serialized(int op, const char *const *a, const size_t *al
     if (op < 0 || op > 3) { t_err = "bad op"; return -1; }
     *out = nullptr;
     *off_out = *len_out = nullptr;
-    R64Plan P;
-    if (!plan_r64(op, a, alen, na, b, blen, nb, ia, ib, np, P)) return -1;
-    rb200_set *R = batch_op_impl(op, P.S, P.S, P.pa.data(), P.pb.data(), P.pa.size());
-    char *sbuf = nullptr;
-    uint64_t *soff = nullptr, *slen = nullptr;
-    int rc = R ? serialize_impl(R, &sbuf, &soff, &slen, false) : -1;
-    set_delete(R);
-    set_delete(P.S);
-    if (rc != 0) return -1;
-    // stitch: u64 bucket count, then per non-empty bucket u32 high32 + 32-bit blob
-    uint64_t *off = (uint64_t *)malloc(8 * (np + 1)), *len = (uint64_t *)malloc(8 * (np + 1));
-    uint64_t total = 0;
-    auto empty_bucket = [&](size_t q) {
-        uint32_t w[2];
-        if (slen[q] != 8) return false;
-        memcpy(w, sbuf + soff[q], 8);
-        return w[0] == SERIAL_COOKIE_NO_RUN && w[1] == 0;
-    };
-    if (off && len) {
-        for (size_t p = 0; p < np; p++) {
-            uint64_t sz = 8;
-            for (size_t q = P.first[p]; q < P.first[p + 1]; q++)
-                if (!empty_bucket(q)) sz += 4 + slen[q];
-            off[p] = total;
-            len[p] = sz;
-            total += (sz + 15) & ~(uint64_t)15;
-        }
-        off[np] = total;
-    }
-    uint8_t *dst = (off && len) ? (uint8_t *)pin_alloc(total ? total : 16) : nullptr;
-    if (dst) {
-        for (size_t p = 0; p < np; p++) {
-            uint8_t *o = dst + off[p];
-            uint64_t kept = 0;
-            size_t pos = 8;
-            for (size_t q = P.first[p]; q < P.first[p + 1]; q++) {
-                if (empty_bucket(q)) continue;
-                memcpy(o + pos, &P.high[q], 4);
-                memcpy(o + pos + 4, sbuf + soff[q], slen[q]);
-                pos += 4 + slen[q];
-                kept++;
-            }
-            memcpy(o, &kept, 8);
-        }
-        g_serialized_sizes[dst] = total ? total : 16;
-    }
-    rb200_serialized_free(sbuf, soff, slen);
-    if (!dst) {
-        free(off);
-        free(len);
-        t_err = "r64 batch op: host allocation failed";
-        return -1;
-    }
-    *out = (char *)dst;
-    *off_out = off;
-    *len_out = len;
-    return 0;
+    std::vector<uint32_t> ib2;
+    rb200_set64 *S = r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2);
+    if (!S) return -1;
+    rb200_set64 *R = batch_op64_impl(op, S, S, ia, ib2.data(), np);
+    const int rc = R ? serialize64_impl(R, out, off_out, len_out) : -1;
+    set64_delete(R);
+    set64_delete(S);
+    return rc;
 }
 
 // out[k] = roaring64_bitmap_and_cardinality(a[ia[k]], b[ib[k]]) (roaring64.c:1375)
@@ -3769,18 +4143,12 @@ int rb200_r64_batch_and_cardinality_serialized(const char *const *a, const size_
                                                const uint32_t *ia, const uint32_t *ib, size_t np, uint64_t *out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
-    R64Plan P;
-    if (!plan_r64(OP_AND, a, alen, na, b, blen, nb, ia, ib, np, P)) return -1;
-    std::vector<uint64_t> c(P.pa.size());
-    const int rc = P.pa.empty() ? 0 : rb200_batch_and_cardinality(P.S, P.S, P.pa.data(), P.pb.data(), P.pa.size(), c.data());
-    set_delete(P.S);
-    if (rc != 0) return -1;
-    for (size_t p = 0; p < np; p++) {
-        uint64_t s = 0;
-        for (size_t q = P.first[p]; q < P.first[p + 1]; q++) s += c[q];
-        out[p] = s;
-    }
-    return 0;
+    std::vector<uint32_t> ib2;
+    rb200_set64 *S = r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2);
+    if (!S) return -1;
+    const int rc = and_cardinality64_impl(S, S, ia, ib2.data(), np, out);
+    set64_delete(S);
+    return rc;
 }
 
 // ---- in-memory roaring64_bitmap_t (include/roaring/roaring64.h:423-522; src/roaring64.c:1332-1895)
@@ -3789,7 +4157,7 @@ int rb200_r64_batch_and_cardinality_serialized(const char *const *a, const size_
 // functions the reference exports for exactly this purpose: the operands are written with the
 // HOST APPLICATION's roaring64_bitmap_portable_serialize (resolved with dlsym in the running
 // process — the reference must be loaded, or nobody could have built a roaring64_bitmap_t), the
-// container grid runs on the device (rb200_r64_batch_op_serialized), and the result bytes become
+// container grid runs on the device (a resident rb200_set64_t), and the result bytes become
 // a roaring64_bitmap_t again through roaring64_bitmap_portable_deserialize_safe.  Results are
 // byte-identical to the reference's (tests/test_gpu_r64.py).
 namespace {
@@ -3823,7 +4191,51 @@ bool r64_serialize_all(const roaring64_bitmap_t *const *bms, size_t n, std::vect
     if (!ok) t_err = "roaring64: serialization of an operand failed";
     return ok;
 }
+
+// out[k] = the host library's deserialization of blob k (in parallel); all or nothing
+bool r64_deserialize_all(const char *blob, const uint64_t *off, const uint64_t *len, size_t n,
+                         roaring64_bitmap_t **out) {
+    std::atomic<bool> ok(true);
+    rb200::parallel_for(n, [&](size_t k) {
+        out[k] = g_r64.deser(blob + off[k], (size_t)len[k]);
+        if (!out[k]) ok = false;
+    });
+    if (ok) return true;
+    // the results that were built go back to the host library
+    auto r64_free = (void (*)(roaring64_bitmap_t *))dlsym(RTLD_DEFAULT, "roaring64_bitmap_free");
+    for (size_t k = 0; k < n; k++) {
+        if (out[k] && r64_free) r64_free(out[k]);
+        out[k] = nullptr;
+    }
+    t_err = "roaring64: the host library refused a result blob";
+    return false;
+}
 }  // namespace
+
+rb200_set64_t *rb200_set64_upload(const roaring64_bitmap_t *const *bitmaps, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!g_r64.ok()) return nullptr;
+    std::vector<std::vector<char>> bufs;
+    if (!r64_serialize_all(bitmaps, n, bufs)) return nullptr;
+    std::vector<const char *> ptrs(n);
+    std::vector<size_t> lens(n);
+    for (size_t i = 0; i < n; i++) {
+        ptrs[i] = bufs[i].data();
+        lens[i] = g_r64.size(bitmaps[i]);
+    }
+    return set64_upload_impl(ptrs.data(), lens.data(), n);
+}
+
+int rb200_set64_download_all(const rb200_set64_t *s, roaring64_bitmap_t **out) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!g_r64.ok()) return -1;
+    char *blob = nullptr;
+    uint64_t *off = nullptr, *len = nullptr;
+    if (serialize64_impl(s, &blob, &off, &len) != 0) return -1;
+    const bool ok = r64_deserialize_all(blob, off, len, s->n, out);
+    rb200_serialized_free(blob, off, len);
+    return ok ? 0 : -1;
+}
 
 // out[k] = roaring64_bitmap_{and,or,xor,andnot}(a[k], b[k]) for npairs in-memory 64-bit bitmaps of the
 // host application's CRoaring; out[k] is a fresh roaring64_bitmap_t the caller frees with
@@ -3848,23 +4260,9 @@ int rb200_r64_batch_op(int op, const roaring64_bitmap_t *const *a, const roaring
     if (rb200_r64_batch_op_serialized(op, pa.data(), la.data(), npairs, pb.data(), lb.data(), npairs, ia.data(),
                                       ib.data(), npairs, &blob, &off, &len) != 0)
         return -1;
-    std::atomic<bool> ok(true);
-    rb200::parallel_for(npairs, [&](size_t k) {
-        out[k] = g_r64.deser(blob + off[k], (size_t)len[k]);
-        if (!out[k]) ok = false;
-    });
+    const bool ok = r64_deserialize_all(blob, off, len, npairs, out);
     rb200_serialized_free(blob, off, len);
-    if (!ok) {
-        // all or nothing: the results that were built go back to the host library
-        auto r64_free = (void (*)(roaring64_bitmap_t *))dlsym(RTLD_DEFAULT, "roaring64_bitmap_free");
-        for (size_t k = 0; k < npairs; k++) {
-            if (out[k] && r64_free) r64_free(out[k]);
-            out[k] = nullptr;
-        }
-        t_err = "roaring64: the host library refused a result blob";
-        return -1;
-    }
-    return 0;
+    return ok ? 0 : -1;
 }
 
 int rb200_r64_batch_and_cardinality(const roaring64_bitmap_t *const *a, const roaring64_bitmap_t *const *b,

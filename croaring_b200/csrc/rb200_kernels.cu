@@ -1066,6 +1066,89 @@ k_ser_write(SetView S, uint32_t n, const uint64_t *__restrict__ off, const uint3
     }
 }
 
+// ---- 64-bit portable format (src/roaring64.c:2262-2395): a u64 bucket count, then per bucket its
+// u32 high 32 bits and the 32-bit portable blob of its low halves.  The buckets are the bitmaps of an
+// inner set (k_ser_measure gives their exact sizes, k_ser_write writes them at boff); empty buckets
+// are not emitted, as the reference never holds one.  Warp per 64-bit bitmap.
+__device__ __forceinline__ unsigned long long warp_incl_scan64(unsigned long long v, int lane) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const unsigned long long t = __shfl_up_sync(FULLMASK, v, d);
+        if (lane >= d) v += t;
+    }
+    return v;
+}
+
+__global__ void __launch_bounds__(128)
+k_r64_ser_sizes(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict__ b_cnt, uint32_t n,
+                const uint32_t *__restrict__ bm_cnt, const uint32_t *__restrict__ exact,
+                uint64_t *__restrict__ sizes16, uint64_t *__restrict__ exact64) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t i = warp; i < n; i += nwarps) {
+        const uint32_t j0 = b_beg[i], c = b_cnt[i];
+        unsigned long long sum = 0;
+        for (uint32_t k = lane; k < c; k += 32)
+            if (bm_cnt[j0 + k]) sum += 4ull + exact[j0 + k];
+        for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(FULLMASK, sum, d);
+        if (lane == 0) {
+            exact64[i] = 8 + sum;
+            sizes16[i] = (8 + sum + 15) & ~15ull;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(128)
+k_r64_ser_layout(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict__ b_cnt,
+                 const uint32_t *__restrict__ high, uint32_t n, uint32_t nbuckets, const uint32_t *__restrict__ bm_cnt,
+                 const uint32_t *__restrict__ exact, const uint64_t *__restrict__ off, uint64_t *__restrict__ boff,
+                 uint8_t *__restrict__ dst) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+    const uint64_t scratch = off[n];
+    // the inner set's last bitmap is its empty sentinel, in no 64-bit bitmap
+    if (blockIdx.x == 0 && threadIdx.x == 0 && nbuckets) boff[nbuckets - 1] = scratch;
+    for (uint32_t i = warp; i < n; i += nwarps) {
+        const uint32_t j0 = b_beg[i], c = b_cnt[i];
+        const uint64_t o = off[i];
+        uint64_t run = o + 8;
+        uint32_t kept = 0;
+        for (uint32_t k0 = 0; k0 < c; k0 += 32) {
+            const uint32_t j = j0 + k0 + lane;
+            const bool in = k0 + lane < c, live = in && bm_cnt[j] != 0;
+            const unsigned long long sz = live ? 4ull + exact[j] : 0ull;
+            const unsigned long long incl = warp_incl_scan64(sz, lane);
+            const uint64_t pos = run + incl - sz;
+            if (live) {
+                store_u32(dst + pos, high[j]);
+                boff[j] = pos + 4;
+            } else if (in) {
+                boff[j] = scratch;
+            }
+            kept += __popc(__ballot_sync(FULLMASK, live));
+            run += __shfl_sync(FULLMASK, incl, 31);
+        }
+        if (lane == 0) *reinterpret_cast<unsigned long long *>(dst + o) = kept;   // blob starts are 16-byte aligned
+    }
+}
+
+void launch_r64_ser_sizes(const uint32_t *b_beg, const uint32_t *b_cnt, uint32_t n, const uint32_t *bm_cnt,
+                          const uint32_t *exact, uint64_t *sizes16, uint64_t *exact64, cudaStream_t s) {
+    if (!n) return;
+    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
+    k_r64_ser_sizes<<<g, 128, 0, s>>>(b_beg, b_cnt, n, bm_cnt, exact, sizes16, exact64);
+    g_launches++;
+}
+void launch_r64_ser_layout(const uint32_t *b_beg, const uint32_t *b_cnt, const uint32_t *high, uint32_t n,
+                           uint32_t nbuckets, const uint32_t *bm_cnt, const uint32_t *exact, const uint64_t *off,
+                           uint64_t *boff, uint8_t *dst, cudaStream_t s) {
+    const uint32_t g = blocks_for_warps(n ? n : 1, 4, sm_count() * 16);
+    k_r64_ser_layout<<<g, 128, 0, s>>>(b_beg, b_cnt, high, n, nbuckets, bm_cnt, exact, off, boff, dst);
+    g_launches++;
+}
+
 void launch_serialize_measure(const SetView &S, uint32_t n, uint64_t *sizes16, uint32_t *exact,
                               uint32_t *hasrun, cudaStream_t s) {
     if (!n) return;

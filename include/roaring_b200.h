@@ -203,8 +203,9 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
 /* 64-bit bitmaps (src/roaring64.c) through their portable format: result[k] =
  * roaring64_bitmap_{and,or,xor,andnot}(a[ia[k]], b[ib[k]]) — the same container grid per
  * high-32 bucket.  *out (pinned, owned by the library; blob k at *out + (*off)[k], (*len)[k]
- * bytes) is released with rb200_serialized_free.  Bytes in, bytes out; the in-memory form is
- * rb200_r64_batch_op below. */
+ * bytes) is released with rb200_serialized_free.  Bytes in, bytes out: one call uploads a[] and b[]
+ * as one rb200_set64_t, runs the op and serializes the result (the resident form is below); the
+ * in-memory form is rb200_r64_batch_op. */
 int rb200_r64_batch_op_serialized(int op, const char *const *a, const size_t *alen, size_t na,
                                   const char *const *b, const size_t *blen, size_t nb,
                                   const uint32_t *ia, const uint32_t *ib, size_t npairs, char **out,
@@ -237,6 +238,48 @@ uint64_t roaring64_bitmap_xor_cardinality(const roaring64_bitmap_t *r1, const ro
 uint64_t roaring64_bitmap_andnot_cardinality(const roaring64_bitmap_t *r1, const roaring64_bitmap_t *r2);
 double roaring64_bitmap_jaccard_index(const roaring64_bitmap_t *r1, const roaring64_bitmap_t *r2);
 bool roaring64_bitmap_intersect(const roaring64_bitmap_t *r1, const roaring64_bitmap_t *r2);
+
+/* ---------------------------------------------------------------------------------------
+ * 64-bit resident sets.  An rb200_set64_t is an ordered collection of 64-bit bitmaps
+ * (roaring64_bitmap_t, src/roaring64.c) in HBM: every high-32 bucket of every bitmap is one 32-bit
+ * bitmap of an inner resident set, plus a bucket directory.  Results stay resident and chain;
+ * they leave as 64-bit portable bytes (roaring64_bitmap_portable_serialize, one D2H for the whole
+ * set) or as the host application's roaring64_bitmap_t objects.  Results are byte-identical to the
+ * reference's roaring64_bitmap_{and,or,xor,andnot}, roaring64_bitmap_of_ptr and
+ * roaring64_bitmap_run_optimize.  Errors: NULL or -1, rb200_last_error() says why.
+ * ------------------------------------------------------------------------------------- */
+typedef struct rb200_set64 rb200_set64_t;
+/* From 64-bit portable blobs: the bucket headers are checked on the host (before any CUDA call),
+ * the buckets are parsed and checked on the device.  Buckets with no container are accepted and
+ * dropped, as the reference's deserialize-then-serialize drops them. */
+rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size_t *lens, size_t n);
+/* From the host application's in-memory bitmaps (through its roaring64_bitmap_portable_serialize). */
+rb200_set64_t *rb200_set64_upload(const roaring64_bitmap_t *const *bitmaps, size_t n);
+/* roaring64_bitmap_of_ptr of every bitmap: bitmap i = of_ptr(off[i+1] - off[i], vals + off[i]), values
+ * in any order, duplicates allowed; per 48-bit key an array of at most 4096 values or a bitset, never
+ * a run (chain rb200_set64_run_optimize).  Offsets: off[0] == 0, non-decreasing, n < 2^32, checked
+ * on the host before any CUDA call.  _device: vals / off in device memory of the library's device,
+ * read on the library stream and not modified. */
+rb200_set64_t *rb200_set64_from_uint64(const uint64_t *vals, const uint64_t *off, size_t n);
+rb200_set64_t *rb200_set64_from_uint64_device(const uint64_t *d_vals, const uint64_t *d_off, size_t n);
+void rb200_set64_free(rb200_set64_t *s);
+size_t rb200_set64_count(const rb200_set64_t *s);
+/* out[i] = roaring64_bitmap_get_cardinality of bitmap i (host array of rb200_set64_count entries). */
+int rb200_set64_cardinalities(const rb200_set64_t *s, uint64_t *out);
+/* result[k] = roaring64_bitmap_<op>(A[ia[k]], B[ib[k]]), a new resident set; A may equal B. */
+rb200_set64_t *rb200_set64_batch_op(int op, const rb200_set64_t *A, const rb200_set64_t *B,
+                                    const uint32_t *ia, const uint32_t *ib, size_t npairs);
+/* out[k] = roaring64_bitmap_and_cardinality(A[ia[k]], B[ib[k]]); 0 on success. */
+int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_t *B, const uint32_t *ia,
+                                      const uint32_t *ib, size_t npairs, uint64_t *out);
+/* mode 1 = roaring64_bitmap_run_optimize, mode 0 = remove the run containers (as rb200_set_run_optimize). */
+rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *s, int mode);
+/* Device-side roaring64_bitmap_portable_serialize of every bitmap + one D2H: blob i = *buf + (*off)[i],
+ * (*len)[i] bytes (blob starts 16-byte aligned); release all three with rb200_serialized_free. */
+int rb200_set64_serialize(const rb200_set64_t *s, char **buf, uint64_t **off, uint64_t **len);
+/* Every bitmap as a roaring64_bitmap_t of the host application (its _portable_deserialize_safe);
+ * out[i] is freed by the caller with roaring64_bitmap_free.  0 on success. */
+int rb200_set64_download_all(const rb200_set64_t *s, roaring64_bitmap_t **out);
 
 /* roaring_bitmap_or_many over S[idx[0..n)] (idx == NULL: all bitmaps in order).
  * Returns a device-resident set holding ONE bitmap. */
