@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libroaring_b200.so")
-SOURCES = ["rb200_kernels.cu", "rb200_many.cu", "rb200_many2.cu", "rb200_convert.cu", "rb200_build.cu", "rb200_host.cu", "rb200_shard.cu",
+SOURCES = ["rb200_kernels.cu", "rb200_compute.cu", "rb200_many.cu", "rb200_many2.cu", "rb200_convert.cu", "rb200_build.cu", "rb200_host.cu", "rb200_shard.cu",
            "rb200_fused.cu"]
 HEADERS = ["rb200_common.h", "rb200_device.cuh", "rb200_cells.cuh", "rb200_internal.h", os.path.join("..", "..", "include", "roaring_b200.h")]
 
@@ -26,6 +26,10 @@ NVCC_FLAGS = [
     "-cudart", "static",
     "-DRB200_BUILDING_LIBRARY",   # include/roaring_b200.h: never pull an installed copy of the reference's headers
 ]
+# The pairwise cell kernel writes results it never reads again: its global stores default to
+# evict-first, so that they do not push the operands, which every cell reads, out of L2
+# (rb200_compute.cu).
+SOURCE_FLAGS = {"rb200_compute.cu": ["-Xptxas", "-dscm=cs"]}
 
 
 def _newest(paths):
@@ -65,7 +69,7 @@ def build(force=False, verbose=False, defines=(), out=None):
     tag = "" if not out else "." + os.path.basename(out).replace(".so", "")
     for s in SOURCES:
         o = os.path.join(CSRC, s.replace(".cu", tag + ".o"))
-        cmd = [nvcc] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + \
+        cmd = [nvcc] + NVCC_FLAGS + SOURCE_FLAGS.get(s, []) + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + \
               ["-c", os.path.join(CSRC, s), "-o", o]
         if verbose:
             print(" ".join(cmd), flush=True)

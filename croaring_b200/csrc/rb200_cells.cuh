@@ -87,6 +87,26 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
         return;
     }
 
+    // ---- bitset | bitset: the result is a bitset (containers.h:1015-1020), so a | b goes from L2 to
+    // the result slot, counted on the way, without the accumulator.  In place, a saturated union
+    // becomes the full run unless the left container was full already (see the rules below).
+    if (OP == OP_OR && !lazy && tA == T_BITSET && tB == T_BITSET && cap >= (uint32_t)BITSET_BYTES) {
+        const int card = acc_bitset_op_bitset<OP_OR>(reinterpret_cast<uint32_t *>(out), pa, pb, lane);
+        otype = T_BITSET;
+        ocard = (uint32_t)card;
+        olen = 1024u;
+        if (card == 0) {
+            otype = 0;
+            olen = 0;
+        } else if (inplace_rules && card == 65536 && cA != 65536u) {
+            // the run {0, 65535} over the first word of the bitset, which this lane stored itself
+            if (lane == 0) reinterpret_cast<uint32_t *>(out)[0] = 0xffff0000u;
+            otype = T_RUN;
+            olen = 1u;
+        }
+        return;
+    }
+
     // ---- general path: acc = A op B --------------------------------------------------------
     int card = -1, nruns = 0;
     if (tA == T_BITSET && tB == T_BITSET) {
@@ -99,16 +119,19 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
         __syncwarp();
     } else if ((tA == T_BITSET && tB == T_ARRAY) || (tA == T_ARRAY && tB == T_BITSET)) {
         // bitset with an array (AND and A x B ANDNOT took the filter above): the bitset is copied into
-        // the accumulator by cp.async and the array applied on top, its first loads issued before the
-        // copy is waited for, so both arrive in the same trip.  A x B unions / xors run as B op A,
-        // the same set.
+        // the accumulator by cp.async and the array applied on top, its first 512 values staged by
+        // cp.async in the same trip.  A x B unions / xors run as B op A, the same set.  The atomics
+        // return the words they change, so the result's cardinality is the bitset's plus what the
+        // array changed, and the accumulator is not counted again (the lazy rules count it anyway).
         const bool arrA = tA == T_ARRAY;
         const uint8_t *parr = arrA ? pa : pb;
         const uint32_t narr = arrA ? cA : cB;
         acc_copy_bitset_async(acc, arrA ? pb : pa, lane);
-        if (op == OP_OR) acc_apply_array<0, APPLY_WAIT, AV>(acc, parr, narr, lane);
-        else if (op == OP_XOR) acc_apply_array<1, APPLY_WAIT, AV>(acc, parr, narr, lane);
-        else if (op == OP_ANDNOT) acc_apply_array<2, APPLY_WAIT, AV>(acc, parr, narr, lane);
+        int delta = 0;
+        if (op == OP_OR) delta = acc_apply_array_staged<0>(acc, parr, narr, lane);
+        else if (op == OP_XOR) delta = acc_apply_array_staged<1>(acc, parr, narr, lane);
+        else if (op == OP_ANDNOT) delta = acc_apply_array_staged<2>(acc, parr, narr, lane);
+        if (!lazy && op != OP_AND) card = (int)(arrA ? cB : cA) + __reduce_add_sync(FULLMASK, delta);
         __syncwarp();
     } else {
         acc_load<AV>(acc, tA, pa, lA, lane);

@@ -302,12 +302,19 @@ __device__ __forceinline__ void acc_store_bitset(const uint32_t *acc, uint8_t *d
     for (int i = 0; i < 16; i++) d[i * 32 + lane] = reinterpret_cast<const uint4 *>(acc)[i * 32 + lane];
 }
 
-// MODE 0 = set (or), 1 = flip (xor), 2 = clear (andnot)
+// MODE 0 = set (or), 1 = flip (xor), 2 = clear (andnot).  Returns the word as it was before.
 template <int MODE>
-__device__ __forceinline__ void acc_atom(uint32_t *p, uint32_t m) {
-    if (MODE == 0) atomicOr(p, m);
-    else if (MODE == 1) atomicXor(p, m);
-    else atomicAnd(p, ~m);
+__device__ __forceinline__ uint32_t acc_atom(uint32_t *p, uint32_t m) {
+    if (MODE == 0) return atomicOr(p, m);
+    else if (MODE == 1) return atomicXor(p, m);
+    else return atomicAnd(p, ~m);
+}
+// how much acc_atom<MODE>(p, m) changed the accumulator's cardinality, given the word it returned
+template <int MODE>
+__device__ __forceinline__ int atom_delta(uint32_t old, uint32_t m) {
+    if (MODE == 0) return __popc(m & ~old);
+    else if (MODE == 1) return __popc(m & ~old) - __popc(m & old);
+    else return -__popc(m & old);
 }
 template <int MODE>
 __device__ __forceinline__ void acc_plain(uint32_t *p) {
@@ -324,9 +331,8 @@ __device__ __forceinline__ void acc_plain(uint32_t *p) {
 #endif
 // Up to VECS vectors per lane (256 values each) are loaded before the first atomic, so an array of up
 // to 256 * VECS values costs one trip to L2.  PRE runs between the first loads and the first atomic:
-// APPLY_ZERO clears the accumulator (rasterising into a fresh one), APPLY_WAIT waits for an
-// acc_copy_bitset_async issued by the caller (the bitset and the array arrive in the same trip).
-constexpr int APPLY_NONE = 0, APPLY_ZERO = 1, APPLY_WAIT = 2;
+// APPLY_ZERO clears the accumulator (rasterising into a fresh one).
+constexpr int APPLY_NONE = 0, APPLY_ZERO = 1;
 #ifndef RB200_APPLY_VECS
 #define RB200_APPLY_VECS 2      // AND / ANDNOT cells, and_cardinality, conversions
 #endif
@@ -386,7 +392,6 @@ __device__ __forceinline__ void acc_apply_array(uint32_t *acc, const uint8_t *__
             if (i < nvec) q[u] = __ldg(v4 + i);
         }
         if (PRE == APPLY_ZERO && i0 == 0) { acc_zero(acc, lane); __syncwarp(); }
-        if (PRE == APPLY_WAIT && i0 == 0) acc_async_wait();
 #pragma unroll 1
         for (uint32_t u = 0; u < VECS; u++) {   // one vector per pass, the next ones moved down
             const uint32_t i = i0 + 32 * u + lane;
@@ -435,6 +440,49 @@ __device__ __forceinline__ void acc_or_vec_sparse(uint32_t *acc, uint4 q, uint32
         const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
         if (k < (int)left) atomicOr(acc + (v >> 5), 1u << (v & 31));
     }
+}
+
+// acc op= {sorted u16 array} on top of a bitset whose acc_copy_bitset_async the caller has issued
+// (the bitset x array cells).  Each trip to L2 stages up to APPLY_STAGE_VECS vectors of the array by
+// cp.async in the 1 KiB that follows the accumulator in the warp's shared block, no registers held:
+// an array of n values takes ceil(n / 512) trips, the first one shared with the bitset (one vector
+// per lane in registers took ceil(n / 256); one more per lane on top of the staging spilled).
+// Returns the lane's share of the change in the accumulator's cardinality, taken from the words the
+// atomics return.
+constexpr uint32_t APPLY_STAGE_VECS = 64;
+template <int MODE>
+__device__ __forceinline__ int acc_apply_array_staged(uint32_t *acc, const uint8_t *__restrict__ src, uint32_t n,
+                                                      int lane) {
+    const uint4 *v4 = reinterpret_cast<const uint4 *>(src);
+    const uint4 *stage = reinterpret_cast<const uint4 *>(acc + ACC_WORDS);
+    const uint32_t nvec = (n + 7) >> 3, d = smem_u32(stage);
+    int delta = 0;
+    uint32_t i0 = 0;
+#pragma unroll 1
+    do {   // (at least once: the bitset copy is waited for here)
+        const uint32_t ns = nvec - i0 < APPLY_STAGE_VECS ? nvec - i0 : APPLY_STAGE_VECS;
+#pragma unroll
+        for (uint32_t s = lane; s < APPLY_STAGE_VECS; s += 32)
+            if (s < ns)
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d + 16u * s), "l"(v4 + i0 + s) : "memory");
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
+        acc_async_wait();
+#pragma unroll 1
+        for (uint32_t s = lane; s < ns; s += 32) {
+            const uint4 q = stage[s];
+            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+            const uint32_t left = n - (i0 + s) * 8;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                const uint32_t v = (k & 1) ? (w[k >> 1] >> 16) : (w[k >> 1] & 0xffffu);
+                const uint32_t bit = 1u << (v & 31);
+                if (k < (int)left) delta += atom_delta<MODE>(acc_atom<MODE>(acc + (v >> 5), bit), bit);
+            }
+        }
+        __syncwarp();   // the next trip's copies overwrite the staging
+        i0 += APPLY_STAGE_VECS;
+    } while (i0 < nvec);
+    return delta;
 }
 
 // Warp-collective: every lane brings one closed range [lo,hi] (valid==false: none).
@@ -570,10 +618,11 @@ __device__ __forceinline__ void acc_op_bitset(uint32_t *acc, const uint8_t *__re
     }
 }
 
-// acc = bitset(a) OP bitset(b) straight from global memory (the B x B cell): 2 x 8 KiB of
-// 128-bit loads per warp, result staged in shared memory, popcount fused.
+// dst = bitset(a) OP bitset(b) straight from global memory (the B x B cell): 2 x 8 KiB of
+// 128-bit loads per warp, popcount fused.  dst is the accumulator (the result is staged there until
+// its type is known) or, when the result is known to be a bitset, the result slot itself.
 template <int OP>
-__device__ __forceinline__ int acc_bitset_op_bitset(uint32_t *acc, const uint8_t *pa,
+__device__ __forceinline__ int acc_bitset_op_bitset(uint32_t *dst, const uint8_t *pa,
                                                     const uint8_t *pb, int lane) {
     const uint4 *a = reinterpret_cast<const uint4 *>(pa);
     const uint4 *b = reinterpret_cast<const uint4 *>(pb);
@@ -593,7 +642,7 @@ __device__ __forceinline__ int acc_bitset_op_bitset(uint32_t *acc, const uint8_t
             else if (OP == OP_OR) { r.x = qa[i].x | qb[i].x; r.y = qa[i].y | qb[i].y; r.z = qa[i].z | qb[i].z; r.w = qa[i].w | qb[i].w; }
             else if (OP == OP_XOR) { r.x = qa[i].x ^ qb[i].x; r.y = qa[i].y ^ qb[i].y; r.z = qa[i].z ^ qb[i].z; r.w = qa[i].w ^ qb[i].w; }
             else { r.x = qa[i].x & ~qb[i].x; r.y = qa[i].y & ~qb[i].y; r.z = qa[i].z & ~qb[i].z; r.w = qa[i].w & ~qb[i].w; }
-            reinterpret_cast<uint4 *>(acc)[(h * 4 + i) * 32 + lane] = r;
+            reinterpret_cast<uint4 *>(dst)[(h * 4 + i) * 32 + lane] = r;
             c += popc4(r);
         }
     }
@@ -870,6 +919,7 @@ constexpr uint32_t MERGE_PER_LANE = 8, MERGE_WIN = 32 * MERGE_PER_LANE;
 constexpr uint32_t MERGE_WBUF = 4104;
 // per-warp shared block: the 8 KiB accumulator, then room for the merge's window buffer (9 KiB)
 constexpr int WARP_SMEM_WORDS = ACC_WORDS + 256;
+static_assert(ACC_WORDS + 4 * APPLY_STAGE_VECS <= WARP_SMEM_WORDS, "array staging of acc_apply_array_staged");
 static_assert(2 * MERGE_WBUF + 2 * (MERGE_WIN + 8) <= 4 * WARP_SMEM_WORDS, "merge window buffer");
 
 // Not inlined: the cell kernel's other paths then keep their register allocation (measured faster
