@@ -721,7 +721,8 @@ class DeviceSet:
 
     def download_all_raw(self):
         """All bitmaps as a ctypes array of roaring_bitmap_t* (no Python wrappers); release with
-        free_raw().  This is the bulk form bench.py's e2e leg times."""
+        free_raw().  bench.py's e2e leg times the visitor form (foreach_async), which shares this
+        download pipeline."""
         n = len(self)
         out = (_P * n)()
         if lib().rb200_set_download_all(self.ptr, out) != 0:

@@ -1901,14 +1901,6 @@ roaring_bitmap_t *build_bitmap(const rb200_set *s, size_t i, const uint8_t *slab
     return r;
 }
 
-}  // namespace
-
-extern "C" {
-
-}  // extern "C" (reopened below)
-
-namespace {
-
 // Persistent host worker pool (materialisation / bulk free).  run(fn, T) executes fn() on T
 // threads (the caller is one of them); fn pulls its own work from a shared atomic counter.
 void bind_to_local_cpus();
@@ -2025,135 +2017,282 @@ unsigned host_workers() {
     return T;
 }
 
+// fn(i) for every i in [0, n) on up to T pool threads, which claim the indices in blocks of blk.
+void pool_for(size_t n, unsigned T, size_t blk, const std::function<void(size_t)> &fn) {
+    if ((size_t)T * blk > n) T = (unsigned)((n + blk - 1) / blk);
+    std::atomic<size_t> next(0);
+    std::function<void()> work = [&]() {
+        for (size_t i0; (i0 = next.fetch_add(blk)) < n;)
+            for (size_t i = i0, i1 = std::min(n, i0 + blk); i < i1; i++) fn(i);
+    };
+    pool().run(work, T);
+}
+
+// Every bulk download takes the same three steps: pack_for_download() lays the set out for the
+// trip (on the library stream), a Ring of pinned slots brings the payload over chunk by chunk, and
+// materialise() builds the bitmaps of each staged chunk on the worker pool while the next chunks
+// are still crossing PCIe.
+
+// A set packed for download: directory in bitmap order, mirrored in pinned memory; payload
+// contiguous in bitmap order with no slot slack (device), cut into chunks of whole bitmaps.
+struct Packed {
+    rb200_set *P = nullptr;
+    size_t nb = 0;
+    uint64_t *h_ob = nullptr;       // [payload offset (nb+1) | first container (nb+1)], pinned
+    std::vector<size_t> chunk_end;  // bitmap index closing each chunk
+    uint64_t max_chunk = 0;         // payload bytes of the largest chunk
+    uint64_t bytes = 0;             // directory + payload: what crosses PCIe
+    Packed() = default;
+    Packed(const Packed &) = delete;
+    ~Packed() {  // every copy out of P must have landed
+        set_delete(P);
+        pin_free(h_ob, 16 * (nb + 1));
+    }
+    size_t begin(size_t k) const { return k ? chunk_end[k - 1] : 0; }
+};
+
+using Clock = std::chrono::steady_clock;
+double ms_since(Clock::time_point t) { return std::chrono::duration<double, std::milli>(Clock::now() - t).count(); }
+
+// What a download moved and where its time went: report() sets rb200_last_download_bytes and
+// prints the RB200_TRACE line.
+struct DlStats {
+    const char *path;
+    size_t sets = 0, bitmaps = 0, chunks = 0;
+    uint64_t bytes = 0;
+    double pack = 0, wait = 0, build = 0;  // ms
+    Clock::time_point t0 = Clock::now();
+    explicit DlStats(const char *p) : path(p) {}
+    void add(const DlStats &o) {
+        if (o.sets && !sets) t0 = o.t0;
+        sets += o.sets, bitmaps += o.bitmaps, chunks += o.chunks, bytes += o.bytes;
+        pack += o.pack, wait += o.wait, build += o.build;
+    }
+    void report() const {
+        g.last_download_bytes = bytes;
+        if (getenv("RB200_TRACE"))
+            fprintf(stderr, "rb200 %s: %zu sets %zu bitmaps %zu chunks %.1f MB | pack %.2f ms, copy-wait %.2f ms, "
+                            "build %.2f ms, total %.2f ms\n",
+                    path, sets, bitmaps, chunks, bytes / 1e6, pack, wait, build, ms_since(t0));
+    }
+};
+
+// Pack s for download on the library stream: chunks of at most chunk_bitmaps bitmaps and ~64 MB of
+// payload.  The directory copy is only enqueued; it lands before any chunk copied after it on the
+// library stream (the background downloader orders its stream after the pack with an event).
+std::unique_ptr<Packed> pack_for_download(const rb200_set *s, size_t chunk_bitmaps, DlStats &stats) {
+    const auto t = Clock::now();
+    if (!resolve(s)) return nullptr;
+    std::unique_ptr<Packed> pk(new Packed());
+    const size_t nb = pk->nb = s->n_bitmaps;
+    bool ok = true;
+    if (nb) {
+        if (chunk_bitmaps == 0) chunk_bitmaps = 1024;
+        uint64_t *d_bytes = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
+                 *d_beg = (uint64_t *)dev_alloc(8 * (nb + 1));
+        uint32_t *d_cnt = (uint32_t *)dev_alloc(4 * nb);
+        pk->h_ob = (uint64_t *)pin_alloc(16 * (nb + 1));
+        ok = d_bytes && d_off && d_beg && d_cnt && pk->h_ob;
+        const int elide = (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0);
+        if (ok) {
+            launch_pack(s->view(), (uint32_t)nb, elide, d_bytes, d_cnt, d_off, d_beg, g.stream);
+            ok = cudaMemcpyAsync(pk->h_ob, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                 cudaMemcpyAsync(pk->h_ob + nb + 1, d_beg, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                 cudaStreamSynchronize(g.stream) == cudaSuccess;
+        }
+        const uint64_t *h_off = pk->h_ob, *h_beg = h_off ? h_off + nb + 1 : nullptr;
+        if (ok) {
+            pk->P = set_new((uint32_t)nb, h_beg[nb], h_off[nb]);
+            ok = pk->P != nullptr;
+        }
+        if (ok) {
+            rb200_set *P = pk->P;
+            P->n_containers = h_beg[nb];
+            P->slab_used = h_off[nb];
+            P->h_flags = s->h_flags;
+            P->parentA = s->parentA;
+            P->parentB = s->parentB;
+            launch_pack_copy(s->view(), (uint32_t)nb, elide, d_off, d_beg, P->out(), g.stream);
+            P->m_dir = (uint8_t *)pin_alloc(P->L.total);
+            ok = P->m_dir != nullptr &&
+                 cudaMemcpyAsync(P->m_dir, P->d_dir, P->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+            const uint64_t CAP = (uint64_t)64 << 20;
+            for (size_t p0 = 0, p1; p0 < nb; p0 = p1) {
+                p1 = p0 + 1;
+                while (p1 < nb && p1 - p0 < chunk_bitmaps && h_off[p1 + 1] - h_off[p0] <= CAP) p1++;
+                pk->chunk_end.push_back(p1);
+                pk->max_chunk = std::max(pk->max_chunk, h_off[p1] - h_off[p0]);
+            }
+            pk->bytes = P->L.total + P->slab_used;
+        }
+        dev_free(d_bytes, 8 * nb);
+        dev_free(d_off, 8 * (nb + 1));
+        dev_free(d_beg, 8 * (nb + 1));
+        dev_free(d_cnt, 4 * nb);
+    }
+    if (!ok) {
+        cudaStreamSynchronize(g.stream);  // before ~Packed recycles what the copies write
+        if (t_err.empty()) t_err = "download: packing failed";
+        return nullptr;
+    }
+    stats.sets++, stats.bitmaps += nb, stats.chunks += pk->chunk_end.size(), stats.bytes += pk->bytes;
+    stats.pack += ms_since(t);
+    return pk;
+}
+
+// Pinned staging slots that D2H copies of chunks fill in turn, so the copy engine can run up to
+// slots-1 chunks ahead of the builders.  Chunks alternate between copy-bound and build-bound, so
+// download_sets() and the background downloader use 4 slots: 2 stall one side or the other.
+class Ring {
+   public:
+    explicit Ring(size_t slots) : buf_(slots, nullptr), ev_(slots, nullptr) {
+        for (auto &e : ev_) e = ev_get();
+    }
+    ~Ring() {  // nothing may be in flight
+        for (size_t k = 0; k < buf_.size(); k++) {
+            pin_free(buf_[k], bytes_);
+            ev_put(ev_[k]);
+        }
+    }
+    uint64_t capacity() const { return bytes_; }
+    bool idle() const { return issued_ == waited_; }
+    bool full() const { return issued_ - waited_ == buf_.size(); }
+    // Slots of at least `bytes`; the ring only grows while idle().
+    bool reserve(uint64_t bytes) {
+        bytes = std::max<uint64_t>(bytes, 1);
+        if (bytes <= bytes_) return true;
+        for (auto &b : buf_) { pin_free(b, bytes_); b = (uint8_t *)pin_alloc(bytes); }
+        bytes_ = bytes;
+        if (std::all_of(buf_.begin(), buf_.end(), [](uint8_t *b) { return b != nullptr; })) return true;
+        for (auto &b : buf_) { pin_free(b, bytes_); b = nullptr; }
+        bytes_ = 0;
+        return false;
+    }
+    // Copy chunk k of pk into the next slot on `stream` (the ring must not be full()).
+    bool enqueue(const Packed &pk, size_t k, cudaStream_t stream) {
+        const size_t slot = issued_++ % buf_.size();
+        const uint64_t b0 = pk.h_ob[pk.begin(k)], b1 = pk.h_ob[pk.chunk_end[k]];
+        const bool ok = b1 == b0 || cudaMemcpyAsync(buf_[slot], pk.P->d_slab + b0, b1 - b0,
+                                                    cudaMemcpyDeviceToHost, stream) == cudaSuccess;
+        return cudaEventRecord(ev_[slot], stream) == cudaSuccess && ok;
+    }
+    // Wait for the oldest copy in flight; its slot, or nullptr if the copy failed.
+    const uint8_t *wait() {
+        const size_t slot = waited_++ % buf_.size();
+        return cudaEventSynchronize(ev_[slot]) == cudaSuccess ? buf_[slot] : nullptr;
+    }
+
+   private:
+    std::vector<uint8_t *> buf_;
+    std::vector<cudaEvent_t> ev_;
+    uint64_t bytes_ = 0;
+    size_t issued_ = 0, waited_ = 0;
+};
+
+// Where materialise() puts each bitmap: out[i] (i counted from the chunk's first bitmap), or
+// fn(base + index in the set, bitmap, ctx), which keeps the bitmap by returning non-zero.
+struct Sink {
+    roaring_bitmap_t **out;
+    rb200_visit_fn fn;
+    void *ctx;
+    size_t base;
+};
+
+// Build the bitmaps of chunk k of pk from its staged payload `buf` on the worker pool; false if
+// one failed (its out[] slot is then null).
+bool materialise(const Packed &pk, size_t k, const uint8_t *buf, const Sink &sink) {
+    const size_t p0 = pk.begin(k), p1 = pk.chunk_end[k], n = p1 - p0;
+    const uint64_t *off = pk.h_ob, *beg = pk.h_ob + pk.nb + 1;
+    // threads scaled to the work of the chunk: waking every worker for a few hundred tiny bitmaps
+    // costs more than it saves
+    const uint64_t want = (off[p1] - off[p0] + 256 * (beg[p1] - beg[p0]) + 512 * n) / (128 << 10) + 1;
+    std::atomic<int> failed(0);
+    pool_for(n, (unsigned)std::min<uint64_t>(want, host_workers()), 8, [&](size_t i) {
+        roaring_bitmap_t *bm = build_bitmap(pk.P, p0 + i, buf, off[p0]);
+        if (!bm) failed = 1;
+        if (sink.out) sink.out[i] = bm;
+        else if (bm && sink.fn(sink.base + p0 + i, bm, sink.ctx) == 0) bitmap_free_host(bm);
+    });
+    return !failed;
+}
+
+// Wait for the ring's oldest copy, chunk k of pk, and materialise it.
+bool drain(Ring &ring, const Packed &pk, size_t k, const Sink &sink, DlStats &stats) {
+    auto t = Clock::now();
+    const uint8_t *buf = ring.wait();
+    stats.wait += ms_since(t);
+    t = Clock::now();
+    const bool ok = buf && materialise(pk, k, buf, sink);
+    stats.build += ms_since(t);
+    return ok;
+}
+
+// Every chunk of the packed sets, in order, through one 4-slot ring on the library stream: into
+// out[] (indexed over all the sets) or to the visitor (index running on across the sets).
+bool download_sets(const std::vector<std::unique_ptr<Packed>> &pks, roaring_bitmap_t **out, rb200_visit_fn fn,
+                   void *ctx, DlStats &stats) {
+    struct Ref { const Packed *pk; size_t k, base; };
+    std::vector<Ref> order;
+    uint64_t slot_bytes = 0;
+    size_t base = 0;
+    for (const auto &pk : pks) {
+        for (size_t k = 0; k < pk->chunk_end.size(); k++) order.push_back(Ref{pk.get(), k, base});
+        base += pk->nb;
+        slot_bytes = std::max(slot_bytes, pk->max_chunk);
+    }
+    Ring ring(4);
+    bool ok = ring.reserve(slot_bytes);
+    size_t copied = 0;
+    for (size_t c = 0; c < order.size() && ok; c++) {
+        for (; ok && copied < order.size() && !ring.full(); copied++)
+            ok = ring.enqueue(*order[copied].pk, order[copied].k, g.stream);
+        const Ref &r = order[c];
+        const Sink sink = out ? Sink{out + r.base + r.pk->begin(r.k), nullptr, nullptr, 0} : Sink{nullptr, fn, ctx, r.base};
+        ok = ok && drain(ring, *r.pk, r.k, sink, stats);
+    }
+    cudaStreamSynchronize(g.stream);
+    return ok;
+}
+
 }  // namespace
 
 // Streaming download: results leave the device chunk by chunk while the caller consumes (and
 // frees) the previous chunk, so host memory stays bounded and D2H overlaps materialisation.
 struct rb200_download_stream {
-    rb200_set *P = nullptr;        // packed copy (device)
-    size_t nb = 0;
-    uint64_t *h_ob = nullptr;      // [off(nb+1) | beg(nb+1)] pinned
-    std::vector<size_t> chunk_end; // bitmap index closing each chunk
-    uint8_t *hbuf[2] = {nullptr, nullptr};
-    size_t hbuf_bytes = 0;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    std::unique_ptr<Packed> pk;
+    Ring ring{2};
+    DlStats stats{"download_stream"};
     size_t next_copy = 0, next_build = 0;
-    uint64_t total_bytes = 0;
 };
 
 namespace {
 
-bool stream_enqueue(rb200_download_stream *st) {
-    if (st->next_copy >= st->chunk_end.size()) return true;
-    const size_t k = st->next_copy;
-    const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-    const uint64_t b0 = st->h_ob[p0], b1 = st->h_ob[p1];
-    if (b1 > b0 && cudaMemcpyAsync(st->hbuf[k & 1], st->P->d_slab + b0, b1 - b0, cudaMemcpyDeviceToHost,
-                                   g.stream) != cudaSuccess)
-        return false;
-    cudaEventRecord(st->ev[k & 1], g.stream);
-    st->next_copy++;
+// Keep every slot of the stream's ring busy.
+bool stream_refill(rb200_download_stream *st) {
+    for (; st->next_copy < st->pk->chunk_end.size() && !st->ring.full(); st->next_copy++)
+        if (!st->ring.enqueue(*st->pk, st->next_copy, g.stream)) return false;
     return true;
-}
-
-void stream_free(rb200_download_stream *st, bool sync = true) {
-    if (!st) return;
-    if (sync) cudaStreamSynchronize(g.stream);
-    for (int k = 0; k < 2; k++) {
-        if (st->ev[k]) cudaEventDestroy(st->ev[k]);
-        pin_free(st->hbuf[k], st->hbuf_bytes);
-    }
-    if (st->P) {
-        pin_free(st->P->m_dir, st->P->L.total);
-        st->P->m_dir = st->P->m_slab = nullptr;
-        set_delete(st->P);
-    }
-    pin_free(st->h_ob, 16 * (st->nb + 1));
-    delete st;
 }
 
 }  // namespace
 
 extern "C" {
 
-static rb200_download_stream *download_begin_impl(const rb200_set *s, size_t chunk_bitmaps, bool defer);
 rb200_download_stream_t *rb200_download_begin(const rb200_set_t *s, size_t chunk_bitmaps) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return download_begin_impl(s, chunk_bitmaps, false);
-}
-// defer: pack only; the caller owns the staging ring and enqueues the copies itself
-static rb200_download_stream *download_begin_impl(const rb200_set *s, size_t chunk_bitmaps, bool defer) {
     if (!ctx_init()) return nullptr;
-    if (!resolve(s)) return nullptr;
-    const size_t nb = s->n_bitmaps;
     rb200_download_stream *st = new rb200_download_stream();
-    st->nb = nb;
-    if (nb == 0) return st;
-    if (chunk_bitmaps == 0) chunk_bitmaps = 1024;
-    uint64_t *d_bytes = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
-             *d_beg = (uint64_t *)dev_alloc(8 * (nb + 1));
-    uint32_t *d_cnt = (uint32_t *)dev_alloc(4 * nb);
-    st->h_ob = (uint64_t *)pin_alloc(16 * (nb + 1));
-    bool ok = d_bytes && d_off && d_beg && d_cnt && st->h_ob;
-    if (ok) {
-        const int elide = (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0);
-        launch_pack(s->view(), (uint32_t)nb, elide, d_bytes, d_cnt, d_off, d_beg, g.stream);
-        ok = cudaMemcpyAsync(st->h_ob, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaMemcpyAsync(st->h_ob + nb + 1, d_beg, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess;
-    }
-    const uint64_t *h_off = st->h_ob, *h_beg = st->h_ob ? st->h_ob + nb + 1 : nullptr;
-    if (ok) {
-        st->P = set_new((uint32_t)nb, h_beg[nb], h_off[nb]);
-        ok = st->P != nullptr;
-    }
-    if (ok) {
-        rb200_set *P = st->P;
-        P->n_containers = h_beg[nb];
-        P->slab_used = h_off[nb];
-        P->h_flags = s->h_flags;
-        P->parentA = s->parentA;
-        P->parentB = s->parentB;
-        launch_pack_copy(s->view(), (uint32_t)nb, (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0), d_off, d_beg,
-                         P->out(), g.stream);
-        P->m_dir = (uint8_t *)pin_alloc(P->L.total);
-        ok = P->m_dir != nullptr &&
-             cudaMemcpyAsync(P->m_dir, P->d_dir, P->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        // chunks: at most chunk_bitmaps bitmaps and ~64 MB of payload each
-        const uint64_t CAP = (uint64_t)64 << 20;
-        uint64_t maxb = 0;
-        size_t p0 = 0;
-        while (p0 < nb) {
-            size_t p1 = p0 + 1;
-            while (p1 < nb && p1 - p0 < chunk_bitmaps && h_off[p1 + 1] - h_off[p0] <= CAP) p1++;
-            st->chunk_end.push_back(p1);
-            maxb = std::max(maxb, h_off[p1] - h_off[p0]);
-            p0 = p1;
-        }
-        st->hbuf_bytes = maxb;
-        for (int k = 0; k < 2 && ok && !defer; k++) {
-            st->hbuf[k] = (uint8_t *)pin_alloc(maxb);
-            ok = st->hbuf[k] != nullptr && cudaEventCreateWithFlags(&st->ev[k], cudaEventDisableTiming) == cudaSuccess;
-        }
-        st->total_bytes = P->L.total + P->slab_used;
-        g.last_download_bytes = st->total_bytes;
-        if (!defer) ok = ok && stream_enqueue(st) && stream_enqueue(st);
-    }
-    dev_free(d_bytes, 8 * nb);
-    dev_free(d_off, 8 * (nb + 1));
-    dev_free(d_beg, 8 * (nb + 1));
-    dev_free(d_cnt, 4 * nb);
-    if (!ok) {
-        if (t_err.empty()) t_err = "download_begin failed";
-        stream_free(st);
-        return nullptr;
-    }
-    return st;
+    st->pk = pack_for_download(s, chunk_bitmaps, st->stats);
+    if (st->pk && st->ring.reserve(st->pk->max_chunk) && stream_refill(st)) return st;
+    if (t_err.empty()) t_err = "download_begin failed";
+    cudaStreamSynchronize(g.stream);
+    delete st;
+    return nullptr;
 }
 
 size_t rb200_download_chunk_capacity(const rb200_download_stream_t *st) {
-    size_t m = 0, p0 = 0;
-    for (size_t e : st->chunk_end) { m = std::max(m, e - p0); p0 = e; }
+    size_t m = 0;
+    for (size_t k = 0; k < st->pk->chunk_end.size(); k++) m = std::max(m, st->pk->chunk_end[k] - st->pk->begin(k));
     return m;
 }
 
@@ -2161,39 +2300,11 @@ size_t rb200_download_chunk_capacity(const rb200_download_stream_t *st) {
 // number of bitmaps produced, 0 at the end of the stream, (size_t)-1 on error.
 size_t rb200_download_next(rb200_download_stream_t *st, roaring_bitmap_t **out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (st->next_build >= st->chunk_end.size()) return 0;
-    const size_t k = st->next_build;
-    const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-    if (cudaEventSynchronize(st->ev[k & 1]) != cudaSuccess) { t_err = "download_next: copy failed"; return (size_t)-1; }
-    const uint8_t *buf = st->hbuf[k & 1];
-    const uint64_t bias = st->h_ob[p0];
-    const size_t n = p1 - p0;
-    std::atomic<size_t> next(0);
-    std::atomic<int> failed(0);
-    const rb200_set *P = st->P;
-    std::function<void()> work = [&]() {
-        for (;;) {
-            const size_t i0 = next.fetch_add(8);
-            if (i0 >= n) break;
-            const size_t i1 = std::min(n, i0 + 8);
-            for (size_t i = i0; i < i1; i++) {
-                out[i] = build_bitmap(P, p0 + i, buf, bias);
-                if (!out[i]) failed = 1;
-            }
-        }
-    };
-    // threads scaled to the work of this chunk: waking 64 workers for a few hundred tiny
-    // bitmaps costs more than it saves
-    const uint64_t chunk_bytes = st->h_ob[p1] - st->h_ob[p0];
-    const uint64_t chunk_conts = st->h_ob[st->nb + 1 + p1] - st->h_ob[st->nb + 1 + p0];
-    uint64_t want = (chunk_bytes + 256 * chunk_conts + 512 * n) / (192 << 10) + 1;
-    unsigned T = host_workers();
-    if (want < T) T = (unsigned)want;
-    if ((size_t)T * 8 > n) T = (unsigned)((n + 7) / 8);
-    pool().run(work, T);
-    st->next_build++;
-    if (!stream_enqueue(st)) failed = 1;  // refill the buffer we just drained
-    if (failed) {
+    if (st->next_build >= st->pk->chunk_end.size()) return 0;
+    const size_t k = st->next_build++;
+    const size_t n = st->pk->chunk_end[k] - st->pk->begin(k);
+    std::fill(out, out + n, nullptr);
+    if (!drain(st->ring, *st->pk, k, Sink{out, nullptr, nullptr, 0}, st->stats) || !stream_refill(st)) {
         for (size_t i = 0; i < n; i++) { bitmap_free_host(out[i]); out[i] = nullptr; }
         t_err = "download_next: host allocation or copy failed";
         return (size_t)-1;
@@ -2203,72 +2314,10 @@ size_t rb200_download_next(rb200_download_stream_t *st, roaring_bitmap_t **out) 
 
 void rb200_download_end(rb200_download_stream_t *st) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    stream_free(st);
-}
-
-// Visitor form of the streaming download: every bitmap of the set is materialised as a host
-// roaring_bitmap_t (reference layout), handed to `fn` ON A WORKER THREAD, and freed right after
-// unless fn returns non-zero (then the callee owns it).  Building, consuming and freeing a result
-// on the same thread is what the reference's own loops do (create, use, roaring_bitmap_free —
-// microbenchmarks/bench.cpp:85-96): the allocator recycles hot blocks instead of touching
-// gigabytes of fresh memory.  Returns 0 on success.
-int rb200_download_foreach(const rb200_set_t *s, rb200_visit_fn fn, void *ctx) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const auto t_enter = std::chrono::steady_clock::now();
-    rb200_download_stream *st = rb200_download_begin(s, 4096);
-    if (!st) return -1;
-    std::atomic<int> failed(0);
-    const bool trace = getenv("RB200_TRACE") != nullptr;
-    double t_wait = 0, t_build = 0;
-    const auto t_begin = std::chrono::steady_clock::now();
-    auto ms_since = [](std::chrono::steady_clock::time_point t) {
-        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-    };
-    const double t_pack = ms_since(t_enter);
-    while (st->next_build < st->chunk_end.size()) {
-        const size_t k = st->next_build;
-        const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-        const auto t0 = std::chrono::steady_clock::now();
-        if (cudaEventSynchronize(st->ev[k & 1]) != cudaSuccess) { failed = 1; break; }
-        t_wait += ms_since(t0);
-        const auto t1 = std::chrono::steady_clock::now();
-        const uint8_t *buf = st->hbuf[k & 1];
-        const uint64_t bias = st->h_ob[p0];
-        const size_t n = p1 - p0;
-        std::atomic<size_t> next(0);
-        const rb200_set *P = st->P;
-        std::function<void()> work = [&]() {
-            for (;;) {
-                const size_t i0 = next.fetch_add(8);
-                if (i0 >= n) break;
-                const size_t i1 = std::min(n, i0 + 8);
-                for (size_t i = i0; i < i1; i++) {
-                    roaring_bitmap_t *bm = build_bitmap(P, p0 + i, buf, bias);
-                    if (!bm) { failed = 1; continue; }
-                    if (fn(p0 + i, bm, ctx) == 0) bitmap_free_host(bm);
-                }
-            }
-        };
-        const uint64_t chunk_bytes = st->h_ob[p1] - st->h_ob[p0];
-        const uint64_t chunk_conts = st->h_ob[st->nb + 1 + p1] - st->h_ob[st->nb + 1 + p0];
-        uint64_t want = (chunk_bytes + 256 * chunk_conts + 512 * n) / (128 << 10) + 1;
-        unsigned T = host_workers();
-        if (want < T) T = (unsigned)want;
-        if ((size_t)T * 8 > n) T = (unsigned)((n + 7) / 8);
-        pool().run(work, T);
-        t_build += ms_since(t1);
-        st->next_build++;
-        if (!stream_enqueue(st)) { failed = 1; break; }
-    }
-    if (trace)
-        fprintf(stderr, "rb200 foreach: %zu bitmaps %zu chunks %.1f MB | pack %.2f ms, copy-wait %.2f ms, build %.2f ms, loop %.2f ms\n",
-                st->nb, st->chunk_end.size(), st->total_bytes / 1e6, t_pack, t_wait, t_build, ms_since(t_begin));
-    stream_free(st);
-    if (failed) {
-        if (t_err.empty()) t_err = "download_foreach: host allocation or copy failed";
-        return -1;
-    }
-    return 0;
+    if (!st) return;
+    cudaStreamSynchronize(g.stream);
+    st->stats.report();
+    delete st;
 }
 
 // Visitor download of SEVERAL result sets as one pipelined stream: every set is packed on the
@@ -2279,101 +2328,30 @@ int rb200_download_foreach(const rb200_set_t *s, rb200_visit_fn fn, void *ctx) {
 int rb200_download_foreach_many(const rb200_set_t *const *sets, size_t nsets, rb200_visit_fn fn, void *ctx) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
-    std::vector<rb200_download_stream *> sts(nsets, nullptr);
-    struct Ref { size_t set; size_t k; };
-    std::vector<Ref> order;
-    std::vector<size_t> first_index(nsets, 0);
-    size_t ring_bytes = 0, running = 0;
-    uint64_t total = 0;
+    DlStats stats("foreach_many");
+    std::vector<std::unique_ptr<Packed>> pks;
     bool ok = true;
     for (size_t i = 0; i < nsets && ok; i++) {
-        sts[i] = download_begin_impl(sets[i], 4096, true);
-        ok = sts[i] != nullptr;
-        if (!ok) break;
-        first_index[i] = running;
-        running += sts[i]->nb;
-        ring_bytes = std::max(ring_bytes, sts[i]->hbuf_bytes);
-        total += sts[i]->total_bytes;
-        for (size_t k = 0; k < sts[i]->chunk_end.size(); k++) order.push_back(Ref{i, k});
+        pks.push_back(pack_for_download(sets[i], 4096, stats));
+        ok = pks.back() != nullptr;
     }
-    // staging ring: RING buffers, so the copy engine can run up to RING-1 chunks ahead of the
-    // builders (chunks alternate between copy-bound and build-bound; 2 buffers stall either side)
-    constexpr int RING = 4;
-    uint8_t *ring[RING] = {nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t rev[RING] = {nullptr, nullptr, nullptr, nullptr};
-    for (int k = 0; k < RING && ok; k++) {
-        ring[k] = (uint8_t *)pin_alloc(ring_bytes ? ring_bytes : 16);
-        ok = ring[k] != nullptr && cudaEventCreateWithFlags(&rev[k], cudaEventDisableTiming) == cudaSuccess;
-    }
-    auto enqueue = [&](size_t gidx) -> bool {
-        if (gidx >= order.size()) return true;
-        const rb200_download_stream *st = sts[order[gidx].set];
-        const size_t k = order[gidx].k;
-        const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-        const uint64_t b0 = st->h_ob[p0], b1 = st->h_ob[p1];
-        if (b1 > b0 && cudaMemcpyAsync(ring[gidx % RING], st->P->d_slab + b0, b1 - b0, cudaMemcpyDeviceToHost,
-                                       g.stream) != cudaSuccess)
-            return false;
-        return cudaEventRecord(rev[gidx % RING], g.stream) == cudaSuccess;
-    };
-    std::atomic<int> failed(0);
-    const bool trace = getenv("RB200_TRACE") != nullptr;
-    double t_wait = 0, t_build = 0;
-    auto ms_since = [](std::chrono::steady_clock::time_point t) {
-        return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-    };
-    const auto t_begin = std::chrono::steady_clock::now();
-    for (int k = 0; k < RING && ok; k++) ok = enqueue((size_t)k);
-    for (size_t gidx = 0; gidx < order.size() && ok; gidx++) {
-        const rb200_download_stream *st = sts[order[gidx].set];
-        const size_t k = order[gidx].k, base_index = first_index[order[gidx].set];
-        const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-        const auto t0 = std::chrono::steady_clock::now();
-        if (cudaEventSynchronize(rev[gidx % RING]) != cudaSuccess) { ok = false; break; }
-        t_wait += ms_since(t0);
-        const auto t1 = std::chrono::steady_clock::now();
-        const uint8_t *buf = ring[gidx % RING];
-        const uint64_t bias = st->h_ob[p0];
-        const size_t n = p1 - p0;
-        std::atomic<size_t> next(0);
-        const rb200_set *P = st->P;
-        std::function<void()> work = [&]() {
-            for (;;) {
-                const size_t i0 = next.fetch_add(8);
-                if (i0 >= n) break;
-                const size_t i1 = std::min(n, i0 + 8);
-                for (size_t i = i0; i < i1; i++) {
-                    roaring_bitmap_t *bm = build_bitmap(P, p0 + i, buf, bias);
-                    if (!bm) { failed = 1; continue; }
-                    if (fn(base_index + p0 + i, bm, ctx) == 0) bitmap_free_host(bm);
-                }
-            }
-        };
-        const uint64_t chunk_bytes = st->h_ob[p1] - st->h_ob[p0];
-        const uint64_t chunk_conts = st->h_ob[st->nb + 1 + p1] - st->h_ob[st->nb + 1 + p0];
-        uint64_t want = (chunk_bytes + 256 * chunk_conts + 512 * n) / (128 << 10) + 1;
-        unsigned T = host_workers();
-        if (want < T) T = (unsigned)want;
-        if ((size_t)T * 8 > n) T = (unsigned)((n + 7) / 8);
-        pool().run(work, T);
-        t_build += ms_since(t1);
-        ok = enqueue(gidx + RING);
-    }
-    if (trace)
-        fprintf(stderr, "rb200 foreach_many: %zu sets %zu chunks %.1f MB | copy-wait %.2f ms, build %.2f ms, loop %.2f ms\n",
-                nsets, order.size(), total / 1e6, t_wait, t_build, ms_since(t_begin));
-    cudaStreamSynchronize(g.stream);
-    for (int k = 0; k < RING; k++) {
-        if (rev[k]) cudaEventDestroy(rev[k]);
-        pin_free(ring[k], ring_bytes ? ring_bytes : 16);
-    }
-    for (auto st : sts) if (st) stream_free(st);
-    g.last_download_bytes = total;
-    if (!ok || failed) {
-        if (t_err.empty()) t_err = "download_foreach_many: host allocation or copy failed";
+    ok = ok && download_sets(pks, nullptr, fn, ctx, stats);
+    stats.report();
+    if (!ok) {
+        if (t_err.empty()) t_err = "download_foreach: host allocation or copy failed";
         return -1;
     }
     return 0;
+}
+
+// Visitor form of the streaming download: every bitmap of the set is materialised as a host
+// roaring_bitmap_t (reference layout), handed to `fn` ON A WORKER THREAD, and freed right after
+// unless fn returns non-zero (then the callee owns it).  Building, consuming and freeing a result
+// on the same thread is what the reference's own loops do (create, use, roaring_bitmap_free —
+// microbenchmarks/bench.cpp:85-96): the allocator recycles hot blocks instead of touching
+// gigabytes of fresh memory.  Returns 0 on success.
+int rb200_download_foreach(const rb200_set_t *s, rb200_visit_fn fn, void *ctx) {
+    return rb200_download_foreach_many(&s, 1, fn, ctx);
 }
 
 }  // extern "C"
@@ -2381,12 +2359,12 @@ int rb200_download_foreach_many(const rb200_set_t *const *sets, size_t nsets, rb
 // ---- asynchronous visitor download ---------------------------------------------------------
 // rb200_download_foreach_async packs the set on the caller's thread (device kernels on the library
 // stream) and hands the packed copy to ONE background downloader thread, which owns a second CUDA
-// stream and a 4-deep pinned staging ring: chunks of all queued sets cross PCIe back to back while
-// the worker pool materialises the previous chunk — and while the caller goes on uploading and
-// launching the next ops.  rb200_download_wait drains the queue.
+// stream and a 4-slot Ring: chunks of all queued sets cross PCIe back to back while the worker
+// pool materialises the previous chunk — and while the caller goes on uploading and launching the
+// next ops.  rb200_download_wait drains the queue.
 namespace {
 struct DlJob {
-    rb200_download_stream *st = nullptr;
+    std::unique_ptr<Packed> pk;
     rb200_visit_fn fn = nullptr;
     void *ctx = nullptr;
     cudaEvent_t ready = nullptr;  // recorded on the library stream after the pack
@@ -2400,7 +2378,7 @@ struct Downloader {
     bool started = false;
     int failed = 0;
     std::string err;
-    uint64_t bytes = 0;
+    DlStats stats{"foreach_async"};  // since the previous rb200_download_wait
     void loop();
 };
 Downloader &dl() {
@@ -2411,17 +2389,11 @@ Downloader &dl() {
 void Downloader::loop() {
     cudaSetDevice(g.device);
     bind_to_local_cpus();
-    constexpr int RING = 4;
     cudaStream_t stream = nullptr;
     cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
-    uint8_t *ring[RING] = {nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t rev[RING];
-    for (int k = 0; k < RING; k++) cudaEventCreateWithFlags(&rev[k], cudaEventDisableTiming);
-    size_t ring_bytes = 0;
-    struct Flight { DlJob *job; size_t k; int slot; };
-    std::deque<Flight> inflight;
-    std::deque<DlJob *> jobs;  // taken from q, not yet fully enqueued
-    uint64_t nslot = 0;
+    Ring ring(4);
+    std::deque<std::pair<DlJob *, size_t>> inflight;  // (job, chunk) in ring order
+    std::deque<DlJob *> jobs;                         // taken from q, not yet fully enqueued
     auto fail = [&](const char *why) {
         std::lock_guard<std::mutex> lk(mu);
         failed = 1;
@@ -2429,7 +2401,6 @@ void Downloader::loop() {
     };
     auto finish = [&](DlJob *j) {
         cudaEventDestroy(j->ready);
-        stream_free(j->st, false);
         delete j;
         std::lock_guard<std::mutex> lk(mu);
         if (--active == 0) idle_cv.notify_all();
@@ -2440,66 +2411,30 @@ void Downloader::loop() {
             if (jobs.empty() && inflight.empty()) cv.wait(lk, [&]() { return !q.empty(); });
             while (!q.empty()) { jobs.push_back(q.front()); q.pop_front(); }
         }
-        // keep the copy engine up to RING chunks ahead
-        while ((int)inflight.size() < RING && !jobs.empty()) {
+        while (!ring.full() && !jobs.empty()) {
             DlJob *j = jobs.front();
-            const rb200_download_stream *st = j->st;
-            if (st->chunk_end.empty()) { jobs.pop_front(); finish(j); continue; }
-            if (st->hbuf_bytes > ring_bytes) {  // grow the ring (only with nothing in flight)
-                if (!inflight.empty()) break;
-                for (int k = 0; k < RING; k++) { pin_free(ring[k], ring_bytes); ring[k] = (uint8_t *)pin_alloc(st->hbuf_bytes); }
-                ring_bytes = st->hbuf_bytes;
-                if (!ring[0] || !ring[1] || !ring[2] || !ring[3]) { fail("downloader: pinned allocation failed"); ring_bytes = 0; }
+            const Packed &pk = *j->pk;
+            if (pk.chunk_end.empty()) { jobs.pop_front(); finish(j); continue; }
+            if (pk.max_chunk > ring.capacity()) {
+                if (!ring.idle()) break;
+                if (!ring.reserve(pk.max_chunk)) fail("downloader: pinned allocation failed");
             }
-            const size_t k = j->next_copy;
-            if (k == 0) cudaStreamWaitEvent(stream, j->ready, 0);
-            const size_t p0 = k ? st->chunk_end[k - 1] : 0, p1 = st->chunk_end[k];
-            const uint64_t b0 = st->h_ob[p0], b1 = st->h_ob[p1];
-            const int slot = (int)(nslot++ % RING);
-            if (ring_bytes && b1 > b0 &&
-                cudaMemcpyAsync(ring[slot], st->P->d_slab + b0, b1 - b0, cudaMemcpyDeviceToHost, stream) != cudaSuccess)
-                fail("downloader: D2H copy failed");
-            cudaEventRecord(rev[slot], stream);
-            inflight.push_back(Flight{j, k, slot});
-            if (++j->next_copy == st->chunk_end.size()) jobs.pop_front();
+            if (j->next_copy == 0) cudaStreamWaitEvent(stream, j->ready, 0);
+            if (!ring.enqueue(pk, j->next_copy, stream)) fail("downloader: D2H copy failed");
+            inflight.emplace_back(j, j->next_copy);
+            if (++j->next_copy == pk.chunk_end.size()) jobs.pop_front();
         }
         if (inflight.empty()) continue;
-        const Flight f = inflight.front();
+        DlJob *j = inflight.front().first;
+        const size_t k = inflight.front().second;
         inflight.pop_front();
-        if (cudaEventSynchronize(rev[f.slot]) != cudaSuccess) fail("downloader: copy failed");
-        const rb200_download_stream *st = f.job->st;
-        const size_t p0 = f.k ? st->chunk_end[f.k - 1] : 0, p1 = st->chunk_end[f.k];
-        if (ring_bytes) {
-            const uint8_t *buf = ring[f.slot];
-            const uint64_t bias = st->h_ob[p0];
-            const size_t n = p1 - p0;
-            std::atomic<size_t> next(0);
-            std::atomic<int> bad(0);
-            const rb200_set *P = st->P;
-            const rb200_visit_fn fn = f.job->fn;
-            void *ctx = f.job->ctx;
-            std::function<void()> work = [&]() {
-                for (;;) {
-                    const size_t i0 = next.fetch_add(8);
-                    if (i0 >= n) break;
-                    const size_t i1 = std::min(n, i0 + 8);
-                    for (size_t i = i0; i < i1; i++) {
-                        roaring_bitmap_t *bm = build_bitmap(P, p0 + i, buf, bias);
-                        if (!bm) { bad = 1; continue; }
-                        if (fn(p0 + i, bm, ctx) == 0) bitmap_free_host(bm);
-                    }
-                }
-            };
-            const uint64_t chunk_bytes = st->h_ob[p1] - st->h_ob[p0];
-            const uint64_t chunk_conts = st->h_ob[st->nb + 1 + p1] - st->h_ob[st->nb + 1 + p0];
-            uint64_t want = (chunk_bytes + 256 * chunk_conts + 512 * n) / (128 << 10) + 1;
-            unsigned T = host_workers();
-            if (want < T) T = (unsigned)want;
-            if ((size_t)T * 8 > n) T = (unsigned)((n + 7) / 8);
-            pool().run(work, T);
-            if (bad) fail("downloader: host allocation failed");
+        DlStats t(nullptr);
+        if (!drain(ring, *j->pk, k, Sink{nullptr, j->fn, j->ctx, 0}, t)) fail("downloader: copy or host allocation failed");
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            stats.add(t);
         }
-        if (++f.job->built == st->chunk_end.size()) finish(f.job);
+        if (++j->built == j->pk->chunk_end.size()) finish(j);
     }
 }
 }  // namespace
@@ -2511,22 +2446,23 @@ extern "C" {
 int rb200_download_foreach_async(const rb200_set_t *s, rb200_visit_fn fn, void *ctx) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
+    DlStats t(nullptr);
     DlJob *j = new DlJob();
-    j->st = download_begin_impl(s, 4096, true);
-    if (!j->st) { delete j; return -1; }
+    j->pk = pack_for_download(s, 4096, t);
+    if (!j->pk) { delete j; return -1; }
     j->fn = fn;
     j->ctx = ctx;
     if (cudaEventCreateWithFlags(&j->ready, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventRecord(j->ready, g.stream) != cudaSuccess) {
         t_err = "download_foreach_async: event failed";
-        stream_free(j->st);
+        cudaStreamSynchronize(g.stream);
         delete j;
         return -1;
     }
     Downloader &d = dl();
     {
         std::lock_guard<std::mutex> dk(d.mu);
-        d.bytes += j->st->total_bytes;
+        d.stats.add(t);
         d.active++;
         d.q.push_back(j);
         if (!d.started) {
@@ -2546,8 +2482,8 @@ int rb200_download_wait(void) {
     d.idle_cv.wait(dk, [&]() { return d.active == 0; });
     const int failed = d.failed;
     const std::string why = d.err;
-    g.last_download_bytes = d.bytes;
-    d.bytes = 0;
+    d.stats.report();
+    d.stats = DlStats("foreach_async");
     d.failed = 0;
     d.err.clear();
     dk.unlock();
@@ -2574,146 +2510,24 @@ roaring_bitmap_t *rb200_set_download(const rb200_set_t *cs, size_t i) {
     return build_bitmap(s, i);
 }
 
-// Download every bitmap of a set as host roaring_bitmap_t (reference layout).
-// Pipeline: (1) device-side pack — directory in bitmap order, payload contiguous in bitmap
-// order, no slot slack; (2) D2H of the payload in ~32 MB chunks of whole bitmaps into pinned
-// memory, one event per chunk; (3) host threads build the bitmaps of a chunk (per-container
-// roaring_malloc + memcpy, the ownership contract of src/containers/containers.c:58-77) as soon
-// as its event fires, while later chunks are still crossing PCIe.
-int rb200_set_download_all(const rb200_set_t *cs, roaring_bitmap_t **out) {
+// Download every bitmap of a set as host roaring_bitmap_t (reference layout): pack, then the
+// chunks of the packed set through a 4-slot ring, each materialised into out[] as it lands.
+int rb200_set_download_all(const rb200_set_t *s, roaring_bitmap_t **out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
-    const rb200_set *s = cs;
-    const size_t nb = s->n_bitmaps;
-    if (nb == 0) return 0;
-    const bool trace = getenv("RB200_TRACE") != nullptr;
-    auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    const double t_start = now();
-    double t_packed = 0, t_copies = 0, t_built = 0;
-    // ---- (1) pack
-    uint64_t *d_bytes = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
-             *d_beg = (uint64_t *)dev_alloc(8 * (nb + 1));
-    uint32_t *d_cnt = (uint32_t *)dev_alloc(4 * nb);
-    uint64_t *h_ob = (uint64_t *)pin_alloc(16 * (nb + 1));
-    rb200_set *P = nullptr;
-    uint8_t *hp = nullptr;
-    size_t hp_bytes = 0;
-    std::vector<cudaEvent_t> evs;
-    bool ok = d_bytes && d_off && d_beg && d_cnt && h_ob;
-    if (ok) {
-        const int elide = (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0);
-        launch_pack(s->view(), (uint32_t)nb, elide, d_bytes, d_cnt, d_off, d_beg, g.stream);
-        ok = cudaMemcpyAsync(h_ob, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaMemcpyAsync(h_ob + nb + 1, d_beg, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess;
+    DlStats stats("download_all");
+    std::vector<std::unique_ptr<Packed>> pks;
+    pks.push_back(pack_for_download(s, 4096, stats));
+    if (!pks[0]) return -1;
+    std::fill(out, out + pks[0]->nb, nullptr);
+    const bool ok = download_sets(pks, out, nullptr, nullptr, stats);
+    stats.report();
+    if (!ok) {
+        for (size_t i = 0; i < pks[0]->nb; i++) { bitmap_free_host(out[i]); out[i] = nullptr; }
+        t_err = "download: host allocation or copy failed";
+        return -1;
     }
-    const uint64_t *h_off = h_ob, *h_beg = h_ob ? h_ob + nb + 1 : nullptr;
-    t_packed = now();
-    if (ok) {
-        P = set_new((uint32_t)nb, h_beg[nb], h_off[nb]);
-        ok = P != nullptr;
-    }
-    if (ok) {
-        P->n_containers = h_beg[nb];
-        P->slab_used = h_off[nb];
-        P->h_flags = s->h_flags;
-        P->parentA = s->parentA;
-        P->parentB = s->parentB;
-        launch_pack_copy(s->view(), (uint32_t)nb, (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0), d_off, d_beg,
-                         P->out(), g.stream);
-        // ---- (2) directory, then payload chunks
-        P->m_dir = (uint8_t *)pin_alloc(P->L.total);
-        hp_bytes = P->slab_used;
-        hp = (uint8_t *)pin_alloc(hp_bytes);
-        ok = P->m_dir && hp;
-    }
-    std::vector<size_t> chunk_end;  // bitmap index (exclusive) closing each chunk
-    if (ok) {
-        P->m_slab = hp;
-        ok = cudaMemcpyAsync(P->m_dir, P->d_dir, P->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        const uint64_t CH = (uint64_t)32 << 20;
-        size_t p0 = 0;
-        while (ok && p0 < nb) {
-            size_t p1 = p0 + 1;
-            while (p1 < nb && h_off[p1 + 1] - h_off[p0] <= CH) p1++;
-            const uint64_t b0 = h_off[p0], b1 = h_off[p1];
-            if (b1 > b0)
-                ok = cudaMemcpyAsync(hp + b0, P->d_slab + b0, b1 - b0, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-            cudaEvent_t ev;
-            ok = ok && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess;
-            if (ok) {
-                cudaEventRecord(ev, g.stream);
-                evs.push_back(ev);
-                chunk_end.push_back(p1);
-            }
-            p0 = p1;
-        }
-    }
-    t_copies = now();
-    // ---- (3) host threads
-    if (ok) {
-        std::atomic<size_t> next(0);
-        std::atomic<int> failed(0);
-        const size_t BLK = 16;
-        unsigned T = std::thread::hardware_concurrency();
-        if (T > 48) T = 48;
-        if (T < 1) T = 1;
-        if ((size_t)T * BLK > nb) T = (unsigned)((nb + BLK - 1) / BLK);
-        const int dev = g.device;
-        auto work = [&]() {
-            cudaSetDevice(dev);
-            size_t cur = 0, done_upto = 0;  // chunks [0, done_upto) are known complete
-            for (;;) {
-                const size_t i0 = next.fetch_add(BLK);
-                if (i0 >= nb) break;
-                const size_t i1 = std::min(nb, i0 + BLK);
-                while (cur + 1 < chunk_end.size() && chunk_end[cur] < i1) cur++;
-                // the chunk holding bitmap i1-1 (and every earlier one: same stream) must be done
-                if (cur >= done_upto) {
-                    if (cudaEventSynchronize(evs[cur]) != cudaSuccess) { failed = 1; break; }
-                    done_upto = cur + 1;
-                }
-                for (size_t i = i0; i < i1; i++) {
-                    out[i] = build_bitmap(P, i);
-                    if (!out[i]) failed = 1;
-                }
-            }
-        };
-        std::vector<std::thread> th;
-        for (unsigned t = 1; t < T; t++) th.emplace_back(work);
-        work();
-        for (auto &t : th) t.join();
-        t_built = now();
-        if (cudaStreamSynchronize(g.stream) != cudaSuccess) failed = 1;
-        if (failed) {
-            for (size_t i = 0; i < nb; i++) { bitmap_free_host(out[i]); out[i] = nullptr; }
-            t_err = "download: host allocation or copy failed";
-            ok = false;
-        }
-        g.last_download_bytes = P->L.total + P->slab_used;
-    } else {
-        cudaStreamSynchronize(g.stream);
-        if (t_err.empty()) t_err = "download: packing failed";
-    }
-    if (trace)
-        fprintf(stderr, "[rb200] download_all nb=%zu bytes=%.1f MB: measure+scan %.2f ms, alloc+enqueue %.2f ms, "
-                        "copy+build %.2f ms, total %.2f ms (chunks %zu)\n",
-                nb, P ? (P->L.total + P->slab_used) / 1e6 : 0.0, t_packed - t_start, t_copies - t_packed,
-                t_built - t_copies, now() - t_start, evs.size());
-    for (auto ev : evs) cudaEventDestroy(ev);
-    if (P) {
-        pin_free(P->m_dir, P->L.total);
-        P->m_dir = nullptr;
-        P->m_slab = nullptr;
-        set_delete(P);
-    }
-    pin_free(hp, hp_bytes);
-    pin_free(h_ob, 16 * (nb + 1));
-    dev_free(d_bytes, 8 * nb);
-    dev_free(d_off, 8 * (nb + 1));
-    dev_free(d_beg, 8 * (nb + 1));
-    dev_free(d_cnt, 4 * nb);
-    return ok ? 0 : -1;
+    return 0;
 }
 
 // roaring_bitmap_run_optimize (mode 1) / roaring_bitmap_remove_run_compression (mode 0) applied
@@ -3156,22 +2970,7 @@ void rb200_serialized_free(char *buf, uint64_t *off, uint64_t *len) {
 
 // Free many host bitmaps (results of rb200_set_download_all) with several threads.
 void rb200_bitmaps_free(roaring_bitmap_t **bms, size_t n) {
-    unsigned T = host_workers();
-    if (n < 64 || T <= 1) {
-        for (size_t i = 0; i < n; i++) bitmap_free_host(bms[i]);
-        return;
-    }
-    std::atomic<size_t> next(0);
-    std::function<void()> work = [&]() {
-        for (;;) {
-            const size_t i0 = next.fetch_add(8);
-            if (i0 >= n) break;
-            const size_t i1 = std::min(n, i0 + 8);
-            for (size_t i = i0; i < i1; i++) bitmap_free_host(bms[i]);
-        }
-    };
-    if ((size_t)T * 8 > n) T = (unsigned)((n + 7) / 8);
-    pool().run(work, T);
+    pool_for(n, n < 64 ? 1 : host_workers(), 8, [&](size_t i) { bitmap_free_host(bms[i]); });
 }
 
 int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_bitmap_t *const *b,
@@ -3202,24 +3001,7 @@ int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_
 }  // extern "C"
 namespace rb200 {
 void set_error(const std::string &msg) { t_err = msg; }
-void parallel_for(size_t n, const std::function<void(size_t)> &fn) {
-    if (n == 0) return;
-    unsigned T = host_workers();
-    if (T <= 1 || n < 2) {
-        for (size_t i = 0; i < n; i++) fn(i);
-        return;
-    }
-    if ((size_t)T > n) T = (unsigned)n;
-    std::atomic<size_t> next(0);
-    std::function<void()> work = [&]() {
-        for (;;) {
-            const size_t i = next.fetch_add(1);
-            if (i >= n) break;
-            fn(i);
-        }
-    };
-    pool().run(work, T);
-}
+void parallel_for(size_t n, const std::function<void(size_t)> &fn) { pool_for(n, host_workers(), 1, fn); }
 }  // namespace rb200
 extern "C" {
 

@@ -424,7 +424,10 @@ uint64_t rb200_last_algorithmic_bytes(void);
 float rb200_last_device_ms(void);
 /* Device time (ms) of the grid-cell kernel (k_compute_items / k_card_items / k_or_many2) alone. */
 float rb200_last_compute_ms(void);
-/* Bytes copied device->host by the last rb200_set_download* call (directory + payload slab). */
+/* Bytes copied device->host by the last download: directory + packed payload of each set, the same
+ * number whichever path downloads it (rb200_set_download_all, rb200_download_begin .. _end,
+ * rb200_download_foreach[_many]; after rb200_download_wait, every set queued since the previous
+ * wait). */
 uint64_t rb200_last_download_bytes(void);
 
 #ifdef __cplusplus
