@@ -71,6 +71,7 @@ def lib():
     sig("rb200_synchronize", None)
     sig("rb200_last_error", C.c_char_p)
     sig("rb200_kernel_launches", C.c_uint64)
+    sig("rb200_device_bytes_in_use", C.c_uint64)
     sig("rb200_last_algorithmic_bytes", C.c_uint64)
     sig("rb200_last_device_ms", C.c_float)
     sig("rb200_last_compute_ms", C.c_float)

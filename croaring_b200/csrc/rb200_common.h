@@ -49,8 +49,12 @@ constexpr uint32_t CARD_UNKNOWN = 0x80000000u, CARD_MASK = 0x7fffffffu;
 //                          negation cells (mixed_negation.c), see decide_type_lazy
 constexpr int RULES_INPLACE = 1, RULES_LAZY = 2, RULES_CONV = 4, RULES_NOFULL = 8, RULES_FLIP = 16;
 
-// Device view of a resident set: SoA container directory + one payload slab.
-// Payload of container c starts at payload + c_off[c] (16-byte aligned, padded to 16 B):
+// Device view of a resident set: SoA container directory + payload.
+// Payload of container c starts at payload + c_off[c] (16-byte aligned, padded to 16 B).  `payload`
+// is the set's payload base: its own slab, or for a batch result whose pass-through containers stay
+// in its operands' slabs (rb200_host.cu, batch_op_impl) the lowest of those slabs, so that every
+// c_off is non-negative and below 2^44 (what CellDesc and m2_entry hold).
+// Layout:
 //   bitset: 1024 x u64;  array: c_len x u16 (sorted);  run: c_len x {u16 start,u16 len-1}.
 // c_card is the true cardinality for every type (runs: sum(len+1), filled at upload).
 struct SetView {
@@ -141,6 +145,16 @@ struct Items {
     uint32_t *olen;      // result length (array values / runs)
 };
 
+// Pass-through containers of a non-lazy batch op are shared with the operand, not copied
+// (k_plan_pairs), on the side(s) where onA / onB is set.  The result's payload base
+// (SetView::payload) is then the lowest of its own slab and the operands' bases; offsets are
+// relative to it: dA / dB = operand base - result base, bias = result slab - result base (added to
+// the offsets of the result's own slots).
+struct PassShare {
+    bool onA, onB;
+    uint64_t dA, dB, bias;
+};
+
 // Counters living in device memory, read back once per op.
 struct OpStats {
     unsigned long long slab_cursor;   // bump allocator over the result slab (bytes)
@@ -155,6 +169,7 @@ struct OpStats {
     unsigned int cls_count[8];        // pairwise ops: live work items per code-path class
     unsigned int cls_cursor[8];       //               fill cursors of k_order_items
     unsigned long long payload_bytes; // set builders: container_size_in_bytes of every container, summed
+    unsigned int shared_used[2];      // pairwise ops: some result container points into A's / B's payload
 };
 
 // Code-path classes of the pairwise work items.  k_compute_items is one large kernel (a code path
@@ -254,7 +269,7 @@ extern unsigned long long g_launches;
 
 void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, const uint32_t *ib,
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
-                       Items it, OpStats *st, cudaStream_t s);
+                       const PassShare &sh, Items it, OpStats *st, cudaStream_t s);
 void launch_order_items(Items it, uint64_t W, OpStats *st, cudaStream_t s);
 void launch_compute_items(const SetView &A, const SetView &B, Items it, uint64_t W, int op,
                           uint8_t *slab, uint64_t slab_cap, OpStats *st, int rules, int copy_ticket,
@@ -262,7 +277,7 @@ void launch_compute_items(const SetView &A, const SetView &B, Items it, uint64_t
 void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W, OpStats *st,
                        cudaStream_t s);
 void launch_finalize_pairs(const SetView &A, const SetView &B, Items it, const uint64_t *item_off,
-                           uint32_t npairs, SetOut out, OpStats *st, cudaStream_t s);
+                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, cudaStream_t s);
 void launch_finalize_cards(Items it, const uint64_t *item_off, uint32_t npairs, uint64_t *out,
                            cudaStream_t s);
 void launch_sum_cardinalities(const uint64_t *bm_card, uint32_t n, uint64_t *d_acc, cudaStream_t s);

@@ -27,6 +27,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <numeric>
 #include <string>
 #include <vector>
 
@@ -118,6 +119,7 @@ struct Ctx {
     int sms = 132;
     std::multimap<size_t, void *> dpool, hpool;
     std::mutex alloc_mu;  // dpool / hpool are also used by the background downloader thread
+    uint64_t dev_in_use = 0;  // bytes of device blocks handed out by dev_alloc and not returned (under alloc_mu)
     uint64_t last_algo_bytes = 0;
     float last_ms = 0.f, last_compute_ms = 0.f;
     uint64_t last_download_bytes = 0;
@@ -195,6 +197,7 @@ void *dev_alloc(size_t n) {
     if (it != g.dpool.end()) {
         void *p = it->second;
         g.dpool.erase(it);
+        g.dev_in_use += b;
         return p;
     }
     void *p = nullptr;
@@ -212,6 +215,7 @@ void *dev_alloc(size_t n) {
             return nullptr;
         }
     }
+    g.dev_in_use += b;
     return p;
 }
 void dev_free(void *p, size_t n) {
@@ -219,6 +223,7 @@ void dev_free(void *p, size_t n) {
     std::lock_guard<std::mutex> alk(g.alloc_mu);
     if (n == 0) n = 1;
     g.dpool.insert({bucket(n), p});
+    g.dev_in_use -= bucket(n);
 }
 bool enter_local_cpus(cpu_set_t *saved);
 void *pin_alloc(size_t n) {
@@ -277,6 +282,17 @@ struct DirLayout {
     }
 };
 
+// A set's payload slab.  Held by the set and by every batch result whose pass-through containers
+// point into it (rb200_set::held): it goes back to the pool when the last holder is freed.
+// Reuse is stream-ordered like every pool block: whatever read it was queued before the release.
+struct Slab {
+    uint8_t *p;
+    size_t cap;
+    Slab(uint8_t *p_, size_t cap_) : p(p_), cap(cap_) {}
+    Slab(const Slab &) = delete;
+    ~Slab() { dev_free(p, cap); }
+};
+
 }  // namespace
 
 struct rb200_set {
@@ -287,7 +303,15 @@ struct rb200_set {
     uint64_t portable_bytes = 0;  // sum of container_size_in_bytes
     DirLayout L;
     uint8_t *d_dir = nullptr;   // one block
-    uint8_t *d_slab = nullptr;
+    uint8_t *d_slab = nullptr;  // own payload slab (owned through `slab`)
+    uint8_t *d_base = nullptr;  // payload base of the view: d_slab, or below it for a batch result that shares
+    std::shared_ptr<Slab> slab;
+    // the slabs of the operands (A, B) this batch result shares pass-through containers with; c_off
+    // is relative to d_base, the lowest of d_slab and the operands' bases.  An operand that shares
+    // itself is copied from instead, so holds never chain: a result keeps at most its two operands'
+    // own slabs alive, and a fold that frees its previous accumulator runs in bounded memory.
+    std::shared_ptr<Slab> held[2];
+    bool sharing() const { return held[0] || held[1]; }
     std::vector<uint32_t> h_cnt;    // host mirror: containers per bitmap
     std::vector<uint64_t> h_card;   // host mirror: cardinality per bitmap (empty = not cached)
     bool mirrors_pending = false;   // batch results: h_cnt / h_bytes / h_card are fetched on first use
@@ -310,8 +334,9 @@ struct rb200_set {
     std::vector<uint64_t> h_bytes;  // host mirror: upper bound of stored payload bytes per bitmap
     std::vector<uint64_t> h_ebytes; // host mirror: upper bound of the "effective bytes" (rb200_device.cuh) per bitmap
     std::vector<uint8_t> h_flags;   // per bitmap: COW flag to propagate
-    // lazily downloaded host mirror (pinned)
+    // host copy of the directory (pinned) and, for a set packed for download, of its payload
     uint8_t *m_dir = nullptr, *m_slab = nullptr;
+    rb200_set *mirror = nullptr;    // rb200_set_download: this set packed, directory and payload on the host
 
     SetView view() const {
         SetView v;
@@ -323,7 +348,7 @@ struct rb200_set {
         v.c_len = (const uint32_t *)(d_dir + L.o_len);
         v.c_off = (const uint64_t *)(d_dir + L.o_off);
         v.c_src = (const uint32_t *)(d_dir + L.o_src);
-        v.payload = d_slab;
+        v.payload = d_base;
         return v;
     }
     SetOut out() {
@@ -360,6 +385,8 @@ rb200_set *set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
         delete s;
         return nullptr;
     }
+    s->slab = std::make_shared<Slab>(s->d_slab, slab_cap);
+    s->d_base = s->d_slab;
     s->h_cnt.assign(nb, 0);
     s->h_bytes.assign(nb, 0);
     s->h_ebytes.assign(nb, 0);
@@ -471,7 +498,9 @@ bool resolve(const rb200_set *cs) {
         s->out_portable = s->pstats->out_portable;
         s->n_containers = s->pstats->dir_cursor;
         s->slab_used = s->pstats->slab_cursor;
-        if (s->n_bitmaps == 1) {  // a single result: its mirrors are the op's counters, no extra D2H
+        for (int k = 0; k < 2; k++)   // an operand none of whose containers was shared is not held
+            if (!s->pstats->shared_used[k]) s->held[k].reset();
+        if (s->n_bitmaps == 1 && !s->sharing()) {  // a single result: its mirrors are the op's counters, no extra D2H
             s->h_cnt[0] = (uint32_t)s->n_containers;
             s->h_bytes[0] = s->slab_used;
             s->h_ebytes[0] = std::max<uint64_t>(s->slab_used, s->n_containers * (uint64_t)BITSET_BYTES);
@@ -502,8 +531,11 @@ void set_delete(rb200_set *s) {
     s->staging = nullptr;
     if (g.last_op == s) g.last_op = nullptr;
     set_drop_mirror(s);
+    set_delete(s->mirror);
     dev_free(s->d_dir, s->L.total);
-    dev_free(s->d_slab, s->slab_cap);
+    s->slab.reset();     // the slabs return to the pool unless a result still points into them
+    s->held[0].reset();
+    s->held[1].reset();
     delete s;
 }
 
@@ -638,6 +670,10 @@ extern "C" {
 
 const char *rb200_last_error(void) { return t_err.c_str(); }
 uint64_t rb200_kernel_launches(void) { return g_launches; }
+uint64_t rb200_device_bytes_in_use(void) {
+    std::lock_guard<std::mutex> alk(g.alloc_mu);
+    return g.dev_in_use;
+}
 static void settle_last_op() {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (g.last_op && g.last_op->pending) resolve(g.last_op);
@@ -1333,11 +1369,14 @@ struct PairBuf {
     size_t bytes = 0;
     uint32_t *d_ia = nullptr, *d_ib = nullptr;
     uint64_t *d_off = nullptr;
-    uint64_t W = 0, slab_bound = 0;
+    uint64_t W = 0;
+    // result slab bound for the sharing mode `share` of build() (bit 0: A's pass-through containers
+    // shared, bit 1: B's), and the bound when everything is copied
+    uint64_t slab_bound = 0, slab_bound_copy = 0;
     // op: OP_* of the batch (OP_AND also for the cardinality-only sweeps, which need no slab)
     // flip: B is the range bitmap of rb200_batch_flip (every container ONE run)
     bool build(const rb200_set *A, const rb200_set *B, const uint32_t *ia, const uint32_t *ib,
-               size_t np, int op, bool lazy = false, bool flip = false) {
+               size_t np, int op, bool lazy = false, bool flip = false, int share = 0) {
         if (!ensure_mirrors(A) || !ensure_mirrors(B)) return false;
         if (np > 0xffffffffull) { t_err = "too many pairs in one batch (2^32 - 1 at most)"; return false; }
         const size_t o_off = 0, o_ia = al256(8 * (np + 1)), o_ib = o_ia + al256(4 * np);
@@ -1347,7 +1386,7 @@ struct PairBuf {
         if (!h || !d) return false;
         uint64_t *off = (uint64_t *)(h + o_off);
         uint32_t *hia = (uint32_t *)(h + o_ia), *hib = (uint32_t *)(h + o_ib);
-        uint64_t w = 0, sb = 0;
+        uint64_t w = 0, sb = 0, sbs = 0;
         for (size_t p = 0; p < np; p++) {
             const uint32_t a = ia[p], b = ib[p];
             if (a >= A->n_bitmaps || b >= B->n_bitmaps) {
@@ -1378,17 +1417,24 @@ struct PairBuf {
                 sb += 3 * (EA + EB) + m * (uint64_t)BITSET_BYTES + 512;
             } else if (op == OP_AND) {
                 sb += (EA < EB ? EA : EB) + 64;
-            } else if (op == OP_ANDNOT) {
-                sb += EA + 64;
             } else {
-                sb += EA + EB + 64;
+                const uint64_t E = op == OP_ANDNOT ? EA : EA + EB;
+                sb += E + 64;
+                // shared pass-through containers take no slot: the result's own containers are the
+                // copied side's and cells of matched keys, at most min(na, nb) of them, each <= 8 KiB
+                if (share) {
+                    const uint64_t own = (share & 1 ? 0 : EA) + (share & 2 || op == OP_ANDNOT ? 0 : EB) +
+                                         (uint64_t)(na < nb ? na : nb) * BITSET_BYTES;
+                    sbs += (own < E ? own : E) + 64;
+                }
             }
         }
         off[np] = w;
         // item ids, directory positions of the result and the order list are 32-bit on the device
         if (w > 0xffffffffull) { t_err = "batch too large: more than 2^32 - 1 container slots, split the pair list"; return false; }
         W = w;
-        slab_bound = sb;
+        slab_bound_copy = sb;
+        slab_bound = share ? sbs : sb;
         d_off = (uint64_t *)(d + o_off);
         d_ia = (uint32_t *)(d + o_ia);
         d_ib = (uint32_t *)(d + o_ib);
@@ -1416,6 +1462,33 @@ bool reject_lazy(const rb200_set *s, const char *what) {
     return true;
 }
 
+// Let R point into A's payload (onA) and / or B's (onB): R holds their slabs and its payload base
+// moves to the lowest of its own slab and their bases.  false (nothing changed) when the span from
+// that base to the end of the highest slab would not fit the 44 bits of a cell descriptor's offsets.
+bool share_operands(rb200_set *R, const rb200_set *A, const rb200_set *B, bool onA, bool onB, PassShare &sh) {
+    uintptr_t lo = (uintptr_t)R->d_slab, hi = lo + R->slab_cap;
+    for (const rb200_set *P : {onA ? A : nullptr, onB ? B : nullptr}) {
+        if (!P) continue;
+        lo = std::min(lo, (uintptr_t)P->d_base);
+        hi = std::max(hi, (uintptr_t)P->slab->p + P->slab->cap);
+    }
+    if (hi - lo >= (1ull << 44)) return false;
+    if (onA) R->held[0] = A->slab;
+    if (onB) R->held[1] = B->slab;
+    R->d_base = (uint8_t *)lo;
+    sh.onA = onA;
+    sh.onB = onB;
+    sh.dA = onA ? (uint64_t)((uintptr_t)A->d_base - lo) : 0;
+    sh.dB = onB ? (uint64_t)((uintptr_t)B->d_base - lo) : 0;
+    sh.bias = (uint64_t)((uintptr_t)R->d_slab - lo);
+    return true;
+}
+
+// Payload bytes a set stores (16-byte rounded slots), wherever they live; its mirrors must be current.
+uint64_t stored_bytes_total(const rb200_set *s) {
+    return s->sharing() ? std::accumulate(s->h_bytes.begin(), s->h_bytes.end(), (uint64_t)0) : s->slab_used;
+}
+
 rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const uint32_t *ia,
                          const uint32_t *ib, size_t np, int rules = 0) {
     if (!ctx_init()) return nullptr;
@@ -1432,15 +1505,29 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     PairBuf pb;
     ItemsBuf ib_;
     rb200_set *R = nullptr;
-    bool ok = pb.build(A, B, ia, ib, np, op, (rules & RULES_LAZY) != 0, (rules & RULES_FLIP) != 0);
+    // Non-lazy ops share the unmatched containers of their operands instead of copying them: the
+    // result points into the operands' slabs (the reference shares them too when copy-on-write is on,
+    // roaring.c:918-922; no batch op ever writes into an operand).  Lazy ops and flips keep copying,
+    // and so does every op from an operand that shares containers itself (see rb200_set::held).
+    // (ensure_mirrors: an operand's holds are settled when its op's counters are read)
+    if (!ensure_mirrors(A) || !ensure_mirrors(B)) return nullptr;
+    const bool can_share = !(rules & RULES_LAZY) && op != OP_AND && np > 0;
+    const bool onA = can_share && !A->sharing(), onB = can_share && op != OP_ANDNOT && !B->sharing();
+    bool ok = pb.build(A, B, ia, ib, np, op, (rules & RULES_LAZY) != 0, (rules & RULES_FLIP) != 0,
+                       (onA ? 1 : 0) | (onB ? 2 : 0));
     // class-ordered tickets pay one more small kernel: only for batches that fill the GPU
     static const uint64_t order_min = []() { const char *e = getenv("RB200_ORDER_MIN"); return e ? (uint64_t)atoll(e) : 16384ull; }();
     // (tried in round 2: ONE launch with a CTA per pair doing plan -> cells -> finalize for small batches —
     //  the 199-pair successive sweep took more device time per call: a pair's cells serialise on
     //  its 8 warps while the three-kernel path spreads them over the GPU)
     if (ok) ok = ib_.alloc(pb.W, true, pb.W >= order_min);
+    PassShare sh = {false, false, 0, 0, 0};
     if (ok) {
         R = set_new((uint32_t)np, pb.W, pb.slab_bound);
+        if (R && (onA || onB) && !share_operands(R, A, B, onA, onB, sh)) {
+            set_delete(R);   // out of the offsets' reach: copy everything into a slab sized for it
+            R = set_new((uint32_t)np, pb.W, pb.slab_bound_copy);
+        }
         ok = R != nullptr;
     }
     if (ok) {
@@ -1452,21 +1539,21 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         cudaEventRecord(R->ev[0], g.stream);
         ok = stats_reset();
         const SetView va = A->view(), vb = B->view();
-        launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, op, false, rules, ib_.it,
+        launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, op, false, rules, sh, ib_.it,
                           g.d_stats, g.stream);
         launch_order_items(ib_.it, pb.W, g.d_stats, g.stream);
         cudaEventRecord(R->ev[1], g.stream);
         // pass-through tickets: one item per lane, fewer lanes when the operands' containers are big
         // (32 x 8 KiB on one warp would be the tail of the launch)
         const uint64_t n_cont = A->n_containers + B->n_containers;
-        const uint64_t avg_b = n_cont ? (A->slab_used + B->slab_used) / n_cont : 4096;
+        const uint64_t avg_b = n_cont ? (stored_bytes_total(A) + stored_bytes_total(B)) / n_cont : 4096;
         // (on the real-data suite 4-32 items per ticket are within noise of each other, 1 item is
         //  clearly slower — RB200_COPY_TICKET overrides)
         static const int ct_env = []() { const char *e = getenv("RB200_COPY_TICKET"); return e ? std::min(32, std::max(1, atoi(e))) : 0; }();
         const int copy_ticket = ct_env ? ct_env : avg_b <= 256 ? 32 : avg_b <= 2048 ? 16 : 8;
         launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_stats, rules, copy_ticket, g.stream);
         cudaEventRecord(R->ev[2], g.stream);
-        launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, R->out(), g.d_stats, g.stream);
+        launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, sh, R->out(), g.d_stats, g.stream);
         ok = ok && cudaMemcpyAsync(R->pstats, g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
         cudaEventRecord(R->ev[3], g.stream);
         // no synchronisation here: the counters are taken over by resolve() on first use
@@ -1524,7 +1611,7 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
         cudaEventRecord(g.ev0, g.stream);
         ok = stats_reset();
         const SetView va = A->view(), vb = B->view();
-        launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, OP_AND, true, 0, ib_.it,
+        launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, OP_AND, true, 0, PassShare{false, false, 0, 0, 0}, ib_.it,
                           g.d_stats, g.stream);
         cudaEventRecord(g.evk0, g.stream);
         launch_card_items(va, vb, ib_.it, pb.W, g.d_stats, g.stream);
@@ -1847,21 +1934,6 @@ int rb200_set_cardinalities(const rb200_set_t *s, uint64_t *out) {
 // =================================================================== download
 namespace {
 
-bool ensure_mirror(rb200_set *s) {
-    if (!resolve(s)) return false;
-    if (s->m_dir) return true;
-    s->m_dir = (uint8_t *)pin_alloc(s->L.total);
-    s->m_slab = (uint8_t *)pin_alloc(s->slab_used);
-    if (!s->m_dir || !s->m_slab) return false;
-    bool ok = cudaMemcpyAsync(s->m_dir, s->d_dir, s->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-    if (s->slab_used)
-        ok = ok && cudaMemcpyAsync(s->m_slab, s->d_slab, s->slab_used, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-    ok = ok && cudaStreamSynchronize(g.stream) == cudaSuccess;
-    if (!ok) t_err = "download: copy failed";
-    g.last_download_bytes = s->L.total + s->slab_used;
-    return ok;
-}
-
 roaring_bitmap_t *build_bitmap(const rb200_set *s, size_t i, const uint8_t *slab = nullptr, uint64_t bias = 0) {
     if (!slab) slab = s->m_slab;
     const uint32_t *c_src = (const uint32_t *)(s->m_dir + s->L.o_src);
@@ -2138,6 +2210,34 @@ std::unique_ptr<Packed> pack_for_download(const rb200_set *s, size_t chunk_bitma
     stats.sets++, stats.bitmaps += nb, stats.chunks += pk->chunk_end.size(), stats.bytes += pk->bytes;
     stats.pack += ms_since(t);
     return pk;
+}
+
+// Host copy of a whole set for rb200_set_download, made on first use: the set packed on the device
+// (a batch result's pass-through containers can live in its operands' slabs), then the packed
+// payload copied to pinned memory.  build_bitmap() reads it.
+const rb200_set *ensure_mirror(rb200_set *s) {
+    if (s->mirror) return s->mirror;
+    DlStats stats("download");
+    std::unique_ptr<Packed> pk = pack_for_download(s, 0, stats);
+    if (!pk) return nullptr;
+    rb200_set *P = pk->P;
+    P->m_slab = (uint8_t *)pin_alloc(P->slab_used);
+    bool ok = P->m_slab != nullptr;
+    if (ok && P->slab_used)
+        ok = cudaMemcpyAsync(P->m_slab, P->d_slab, P->slab_used, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // (also the directory copy of the pack)
+    if (!ok) {
+        t_err = "download: copy failed";
+        return nullptr;
+    }
+    pk->P = nullptr;
+    dev_free(P->d_dir, P->L.total);   // the copies have landed: only the pinned host copies are kept
+    P->d_dir = nullptr;
+    P->slab.reset();
+    P->d_slab = P->d_base = nullptr;
+    s->mirror = P;
+    stats.report();
+    return P;
 }
 
 // Pinned staging slots that D2H copies of chunks fill in turn, so the copy engine can run up to
@@ -2506,8 +2606,8 @@ roaring_bitmap_t *rb200_set_download(const rb200_set_t *cs, size_t i) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     rb200_set *s = const_cast<rb200_set *>(cs);
     if (i >= s->n_bitmaps) { t_err = "download: index out of range"; return nullptr; }
-    if (!ensure_mirror(s)) return nullptr;
-    return build_bitmap(s, i);
+    const rb200_set *m = ensure_mirror(s);
+    return m ? build_bitmap(m, i) : nullptr;
 }
 
 // Download every bitmap of a set as host roaring_bitmap_t (reference layout): pack, then the
@@ -2547,10 +2647,10 @@ rb200_set_t *rb200_set_repair_after_lazy(const rb200_set_t *S) {
 }
 static rb200_set *convert_impl(const rb200_set *S, int mode) {
     if (!ctx_init()) return nullptr;
-    if (!resolve(S)) return nullptr;
+    if (!ensure_mirrors(S)) return nullptr;
     const uint64_t nc = S->n_containers;
     // mode 1 never grows a container by more than its 16-byte padding; mode 0 may expand runs
-    const uint64_t bound = S->slab_used + 16 * nc + (mode == 0 ? nc * (uint64_t)BITSET_BYTES : 0) + 512;
+    const uint64_t bound = stored_bytes_total(S) + 16 * nc + (mode == 0 ? nc * (uint64_t)BITSET_BYTES : 0) + 512;
     rb200_set *R = set_new(S->n_bitmaps, nc, bound);
     if (!R) return nullptr;
     bool ok = stats_reset();
@@ -2565,7 +2665,6 @@ static rb200_set *convert_impl(const rb200_set *S, int mode) {
     R->n_containers = nc;
     R->slab_used = g.h_stats->slab_cursor;
     R->h_flags = S->h_flags;
-    if (!ensure_mirrors(S)) { set_delete(R); return nullptr; }
     R->h_cnt = S->h_cnt;
     for (size_t b = 0; b < R->n_bitmaps; b++) {
         R->h_bytes[b] = (uint64_t)R->h_cnt[b] * BITSET_BYTES;

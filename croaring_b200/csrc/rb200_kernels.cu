@@ -62,17 +62,23 @@ __device__ __forceinline__ int cell_class(int op, int rules, int tA, int tB, uin
 }
 
 // ------------------------------------------------------------------------------ planner
+// sh.onA / sh.onB: an unmatched container of that operand is not copied but shared — no slot, no
+// cell, its directory entry (type, card, len as in the parent; c_off = sh.dA / sh.dB + the parent's
+// c_off) goes straight into the item records for k_finalize_pairs, and st->shared_used[side] is set.
+// Own slots are offset by sh.bias (see PassShare).
 __global__ void __launch_bounds__(128)
 k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
              const uint32_t *__restrict__ ib, const uint64_t *__restrict__ item_off,
-             uint32_t npairs, int op, bool card_only, int rules, Items it, OpStats *st) {
+             uint32_t npairs, int op, bool card_only, int rules, PassShare sh, Items it, OpStats *st) {
     __shared__ unsigned int s_cls[N_CLS];   // live items per class of this block (one global atomic per class at the end)
     // the four pairs of a block reserve their result slots with ONE atomic per round (the slab cursor
     // is a single address: a returning atomic per pair serialised 19 900 of them per launch)
     __shared__ uint32_t s_tot[4];
     __shared__ unsigned long long s_base;
+    __shared__ unsigned int s_used[2];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     if (threadIdx.x < N_CLS) s_cls[threadIdx.x] = 0;
+    if (threadIdx.x < 2) s_used[threadIdx.x] = 0;
     __syncthreads();
     for (uint32_t p0 = blockIdx.x * 4; p0 < npairs; p0 += gridDim.x * 4) {
         const uint32_t p = p0 + wid;
@@ -117,12 +123,12 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
                         }
                     } else if (op != OP_AND && !card_only) {
                         kind = K_COPY_A;
-                        cls = CLS_COPY;
+                        cls = sh.onA ? CLS_NONE : CLS_COPY;
                         d.tA = A.c_type[ca];
                         d.cA = A.c_card[ca];
                         d.lA = A.c_len[ca];
                         d.offA = A.c_off[ca];
-                        cap = round16(stored_bytes(d.tA, d.lA));
+                        cap = sh.onA ? 0u : round16(stored_bytes(d.tA, d.lA));
                     }
                 } else {
                     const uint32_t j = t - na;
@@ -133,12 +139,12 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
                     pos = j + ub;
                     if (!matched && (op == OP_OR || op == OP_XOR) && !card_only) {
                         kind = K_COPY_B;
-                        cls = CLS_COPY;
+                        cls = sh.onB ? CLS_NONE : CLS_COPY;
                         d.tA = B.c_type[cb];
                         d.cA = B.c_card[cb];
                         d.lA = B.c_len[cb];
                         d.offA = B.c_off[cb];
-                        cap = round16(stored_bytes(d.tA, d.lA));
+                        cap = sh.onB ? 0u : round16(stored_bytes(d.tA, d.lA));
                     }
                 }
             }
@@ -154,25 +160,28 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
             __syncthreads();
             unsigned long long slab_base = s_base;
             for (int w = 0; w < wid; w++) slab_base += s_tot[w];
+            const bool shared = (kind == K_COPY_A && sh.onA) || (kind == K_COPY_B && sh.onB);
+            if (shared) s_used[kind == K_COPY_B] = 1u;
             if (t < tot) {
                 const uint64_t idx = base_item + pos;
+                const int dkind = shared ? K_HOLE : kind;   // nothing for k_compute_items to do
                 it.kind[idx] = (uint8_t)kind;
                 it.key[idx] = (uint16_t)key;
                 it.ca[idx] = ca;
                 it.cb[idx] = cb;
-                it.slot_off[idx] = slab_base + incl - cap;
+                it.slot_off[idx] = shared ? (kind == K_COPY_A ? sh.dA : sh.dB) + d.offA : slab_base + incl - cap + sh.bias;
                 // the class-ordered list copies only live descriptors; without it the holes are read too
-                if (it.desc && (kind != K_HOLE || !it.desc_cls)) {
+                if (it.desc && (dkind != K_HOLE || !it.desc_cls)) {
                     d.off = slab_base + incl - cap;
                     d.cap = cap;
-                    d.kind = kind;
+                    d.kind = dkind;
                     d.item = (uint32_t)idx;
                     cd_pack(d, it.desc[2 * idx], it.desc[2 * idx + 1]);
                 }
                 if (it.cls) it.cls[idx] = (uint8_t)cls;
-                it.otype[idx] = 0;
-                it.ocard[idx] = 0;
-                it.olen[idx] = 0;
+                it.otype[idx] = shared ? (uint8_t)d.tA : 0;
+                it.ocard[idx] = shared ? d.cA : 0;
+                it.olen[idx] = shared ? d.lA : 0;
             }
             if (it.cls) {   // live items per class
 #pragma unroll
@@ -185,6 +194,7 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
     }
     __syncthreads();
     if (it.cls && threadIdx.x < N_CLS && s_cls[threadIdx.x]) atomicAdd(&st->cls_count[threadIdx.x], s_cls[threadIdx.x]);
+    if (threadIdx.x < 2 && s_used[threadIdx.x]) st->shared_used[threadIdx.x] = 1u;
 }
 
 // descriptors of the live items grouped by class: desc_cls[prefix(class) + k].  A block takes chunks of 2048 item slots
@@ -326,7 +336,7 @@ __device__ __forceinline__ uint32_t portable_header_bytes(uint32_t n, bool hasru
 #endif
 __global__ void __launch_bounds__(128)
 k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ item_off,
-                 uint32_t npairs, SetOut out, OpStats *st) {
+                 uint32_t npairs, uint32_t rw_a, uint32_t rw_b, SetOut out, OpStats *st) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     // the four pairs of a block reserve their directory range with ONE atomic (the cursor is a single
     // address: one returning atomic per pair serialised 19 900 of them per launch)
@@ -355,8 +365,8 @@ k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ it
                 const uint32_t ca = it.ca[i], cb = it.cb[i];
                 bytes += portable_bytes(A.c_type[ca], A.c_len[ca]) +
                          portable_bytes(B.c_type[cb], B.c_len[cb]) + osz;
-            } else {
-                bytes += 2ull * osz;
+            } else {   // a copied pass-through container is read and written, a shared one moves nothing
+                bytes += (unsigned long long)(kind == K_COPY_A ? rw_a : rw_b) * osz;
             }
             if (ot) {
                 cnt++;
@@ -619,10 +629,10 @@ static inline uint32_t blocks_for_warps(uint64_t warps, int warps_per_block, int
 
 void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, const uint32_t *ib,
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
-                       Items it, OpStats *st, cudaStream_t s) {
+                       const PassShare &sh, Items it, OpStats *st, cudaStream_t s) {
     if (!npairs) return;
     const uint32_t g = blocks_for_warps(npairs, 4, sm_count() * 16);
-    k_plan_pairs<<<g, 128, 0, s>>>(A, B, ia, ib, item_off, npairs, op, card_only, rules, it, st);
+    k_plan_pairs<<<g, 128, 0, s>>>(A, B, ia, ib, item_off, npairs, op, card_only, rules, sh, it, st);
     g_launches++;
 }
 
@@ -643,11 +653,11 @@ void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W,
 }
 
 void launch_finalize_pairs(const SetView &A, const SetView &B, Items it, const uint64_t *item_off,
-                           uint32_t npairs, SetOut out, OpStats *st, cudaStream_t s) {
+                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, cudaStream_t s) {
     if (!npairs) return;
     // a warp per pair, full residency (16 CTAs of 4 warps per SM); counters: one atomic per block
     const uint32_t g = blocks_for_warps(npairs, 4, sm_count() * RB200_FIN_BLOCKS);
-    k_finalize_pairs<<<g, 128, 0, s>>>(A, B, it, item_off, npairs, out, st);
+    k_finalize_pairs<<<g, 128, 0, s>>>(A, B, it, item_off, npairs, sh.onA ? 0u : 2u, sh.onB ? 0u : 2u, out, st);
     g_launches++;
 }
 

@@ -147,11 +147,16 @@ void rb200_synchronize(void);
 const char *rb200_last_error(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 uint64_t rb200_kernel_launches(void);
+/* device bytes the library's sets and scratch hold right now (pool blocks handed out and not yet
+ * returned).  A freed set's slab is returned only once no result still points into it. */
+uint64_t rb200_device_bytes_in_use(void);
 
 /* Upload (H2D): pack n host bitmaps into one device-resident set (one contiguous copy). */
 rb200_set_t *rb200_set_upload(const roaring_bitmap_t *const *bitmaps, size_t n);
 /* Same from portable-serialized bytes ("identical serialized inputs"). */
 rb200_set_t *rb200_set_upload_serialized(const char *const *bufs, const size_t *lens, size_t n);
+/* Free a set.  Sets may be freed in any order: a batch result keeps the device memory of the
+ * operands it shares containers with until it is freed itself. */
 void rb200_set_free(rb200_set_t *s);
 /* Opt-in for sets made by rb200_set_upload: promise that the host bitmaps stay alive and unmodified
  * while results derived from the set are downloaded.  Pass-through containers of batch results
@@ -163,7 +168,8 @@ uint64_t rb200_set_container_count(const rb200_set_t *s);   /* total containers 
 uint64_t rb200_set_payload_bytes(const rb200_set_t *s);     /* container_size_in_bytes summed */
 
 /* Pairwise batch: result bitmap k = A[ia[k]] op B[ib[k]], k < npairs (ia/ib host arrays).
- * Returns a new device-resident set of npairs bitmaps (NULL on error).  A may equal B. */
+ * Returns a new device-resident set of npairs bitmaps (NULL on error).  A may equal B.  Containers
+ * whose key is in one operand only are shared with that operand, not copied (non-lazy ops). */
 rb200_set_t *rb200_batch_op(int op, const rb200_set_t *A, const rb200_set_t *B,
                             const uint32_t *ia, const uint32_t *ib, size_t npairs);
 
@@ -418,7 +424,8 @@ int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_
                         size_t npairs, roaring_bitmap_t **out);
 
 /* Algorithmic bytes of the last batch / many op as defined in SURVEY.md §8(d)
- * (container_size_in_bytes of matched inputs + outputs + 2x pass-through). */
+ * (container_size_in_bytes of matched inputs + outputs + 2x copied pass-through; the pass-through
+ * containers a non-lazy op shares with its operands move no bytes and count none). */
 uint64_t rb200_last_algorithmic_bytes(void);
 /* Device time (ms) of the last batch / many op, measured with CUDA events on its stream. */
 float rb200_last_device_ms(void);

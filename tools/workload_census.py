@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """Census of the headline workload (realdata all-pairs): work items of k_compute_items by kind,
-type pair and size class, per dataset — what the kernel's time has to be spent on."""
+type pair and size class, per dataset — what the kernel's time has to be spent on — and the
+pass-through containers of each op (keys in one operand only: OR / XOR keep both sides', ANDNOT
+the left side's) with their stored bytes, 16-byte rounded as in the slab.  Non-lazy batch ops
+share these with their operands instead of copying them."""
 import collections
 import os
 import sys
@@ -48,6 +51,12 @@ def index(blob):
     return keys, types, cards, lens
 
 
+def stored16(types, cards, lens):
+    """slab bytes of each container: bitset 8192, array 2 x card, run 4 x runs, rounded up to 16"""
+    b = np.where(types == 1, 8192, np.where(types == 2, 2 * cards, 4 * lens))
+    return (b + 15) // 16 * 16
+
+
 def main():
     T = {1: "B", 2: "A", 3: "R"}
     for ds in ["census1881", "weather_sept_85", "wikileaks-noquotes"]:
@@ -67,6 +76,9 @@ def main():
         cells = collections.Counter()
         sizes = collections.defaultdict(list)
         copies = collections.Counter()
+        sb = [stored16(t, c, l) for k, t, c, l in ix]
+        pt_n = {"left": 0, "right": 0}
+        pt_b = {"left": 0, "right": 0}
         n = len(ix)
         for i in range(n):
             ki, ti, ci, li = ix[i]
@@ -87,8 +99,17 @@ def main():
                     copies[T[int(t)]] += 1
                 for t in tj[mj]:
                     copies[T[int(t)]] += 1
+                pt_n["left"] += int(mi.sum())
+                pt_n["right"] += int(mj.sum())
+                pt_b["left"] += int(sb[i][mi].sum())
+                pt_b["right"] += int(sb[j][mj].sum())
         tot = sum(cells.values())
         print(f"   matched cells {tot} ({tot / 19900:.1f}/pair), pass-through {sum(copies.values())} ({sum(copies.values()) / 19900:.1f}/pair) {dict(copies)}")
+        for op, sides in (("or / xor", ("left", "right")), ("andnot", ("left",))):
+            cnt_op = sum(pt_n[x] for x in sides)
+            b_op = sum(pt_b[x] for x in sides)
+            print(f"   pass-through per {op} call: {cnt_op} containers, {b_op} stored bytes ({b_op / 1e9:.3f} GB); "
+                  f"a copy reads and writes them: {2 * b_op / 1e9:.3f} GB")
         for tp, cnt in cells.most_common():
             s = np.array(sizes[tp])
             print(f"     {tp}: {cnt:8d} ({100 * cnt / tot:5.1f}%)  cardA mean {s[:, 0].mean():7.0f} cardB mean {s[:, 1].mean():7.0f} "
