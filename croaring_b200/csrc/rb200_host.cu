@@ -129,7 +129,6 @@ struct Ctx {
 } g;
 // rb200_last_error() is per calling thread: concurrent callers do not read each other's failures
 thread_local std::string t_err;
-std::map<uint8_t *, size_t> g_serialized_sizes;  // pinned blobs handed out by rb200_set_serialize
 
 #define CK(call)                                                                    \
     do {                                                                            \
@@ -259,6 +258,85 @@ void pin_free(void *p, size_t n) {
     g.hpool.insert({bucket(n), p});
 }
 
+// Owner of one block of the device pool (Dev) or of the pinned pool: it keeps the byte size it
+// asked for, so the block goes back under the size class it came from.  A device block may be
+// released as soon as the work using it is enqueued (stream-ordered reuse on the library stream); a
+// pinned block only once no copy from or into it can still be in flight.
+template <typename T, bool Dev>
+class PoolBlock {
+   public:
+    PoolBlock() = default;
+    explicit PoolBlock(size_t count) { reset(count); }
+    PoolBlock(PoolBlock &&o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr, o.bytes_ = 0; }
+    PoolBlock &operator=(PoolBlock &&o) noexcept {
+        if (this != &o) {
+            reset();
+            std::swap(p_, o.p_);
+            std::swap(bytes_, o.bytes_);
+        }
+        return *this;
+    }
+    ~PoolBlock() { reset(); }
+    // A block of `count` elements (at least one byte) in place of the current one; false: out of
+    // memory (t_err says so) and the owner is empty.
+    bool reset(size_t count) {
+        reset();
+        const size_t b = count ? sizeof(T) * count : 1;
+        p_ = (T *)(Dev ? dev_alloc(b) : pin_alloc(b));
+        bytes_ = p_ ? b : 0;
+        return p_ != nullptr;
+    }
+    void reset() {
+        if (p_) Dev ? dev_free(p_, bytes_) : pin_free(p_, bytes_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+    T *get() const { return p_; }
+    size_t bytes() const { return bytes_; }
+    explicit operator bool() const { return p_ != nullptr; }
+
+   private:
+    T *p_ = nullptr;
+    size_t bytes_ = 0;
+};
+template <typename T> using DevBlock = PoolBlock<T, true>;
+template <typename T> using PinBlock = PoolBlock<T, false>;
+
+std::map<uint8_t *, PinBlock<uint8_t>> g_serialized;  // pinned blobs handed out, until rb200_serialized_free
+
+// What a serialization hands out: off (n + 1 entries) and len (optional) from malloc, and the
+// pinned blob.  They belong to this object until hand_out(), so a failed call leaves nothing behind.
+struct HostArrays {
+    uint64_t *off = nullptr, *len = nullptr;
+    PinBlock<uint8_t> blob;
+    HostArrays() = default;
+    HostArrays(const HostArrays &) = delete;
+    ~HostArrays() {
+        free(off);
+        free(len);
+    }
+    bool alloc(size_t n, bool with_len) {
+        off = (uint64_t *)malloc(8 * (n + 1));
+        if (with_len) len = (uint64_t *)malloc(8 * (n + 1));
+        if (!off || (with_len && !len)) return false;
+        off[0] = 0;
+        return true;
+    }
+    // Everything to the caller (*buf = NULL without a blob); the blob is released by
+    // rb200_serialized_free.  Returns 0, the status of a successful call.
+    template <typename T>
+    int hand_out(T **buf, uint64_t **off_out, uint64_t **len_out) {
+        uint8_t *p = blob.get();
+        if (p) g_serialized.emplace(p, std::move(blob));
+        *buf = (T *)p;
+        *off_out = off;
+        off = nullptr;
+        if (len_out) *len_out = len;
+        len = nullptr;
+        return 0;
+    }
+};
+
 // ------------------------------------------------------------------ set object
 inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
@@ -286,12 +364,18 @@ struct DirLayout {
 // point into it (rb200_set::held): it goes back to the pool when the last holder is freed.
 // Reuse is stream-ordered like every pool block: whatever read it was queued before the release.
 struct Slab {
+    DevBlock<uint8_t> block;
     uint8_t *p;
     size_t cap;
-    Slab(uint8_t *p_, size_t cap_) : p(p_), cap(cap_) {}
-    Slab(const Slab &) = delete;
-    ~Slab() { dev_free(p, cap); }
+    explicit Slab(size_t cap_) : block(cap_), p(block.get()), cap(cap_) {}
 };
+
+// Owning handles of sets: a temporary set goes back when its handle leaves scope, and release()
+// hands a set to the caller.
+struct SetFree { void operator()(rb200_set *s) const; };
+struct Set64Free { void operator()(rb200_set64 *s) const; };
+using SetPtr = std::unique_ptr<rb200_set, SetFree>;
+using Set64Ptr = std::unique_ptr<rb200_set64, Set64Free>;
 
 }  // namespace
 
@@ -302,7 +386,7 @@ struct rb200_set {
     uint64_t slab_cap = 0, slab_used = 0;
     uint64_t portable_bytes = 0;  // sum of container_size_in_bytes
     DirLayout L;
-    uint8_t *d_dir = nullptr;   // one block
+    DevBlock<uint8_t> d_dir;    // one block
     uint8_t *d_slab = nullptr;  // own payload slab (owned through `slab`)
     uint8_t *d_base = nullptr;  // payload base of the view: d_slab, or below it for a batch result that shares
     std::shared_ptr<Slab> slab;
@@ -320,9 +404,8 @@ struct rb200_set {
     // kernels and the D2H copy of its counters are queued; resolve() waits for them on first use,
     // so consecutive batch calls pipeline on the stream without a host round trip.
     bool pending = false, failed = false;
-    OpStats *pstats = nullptr;                  // pinned
-    uint8_t *staging = nullptr;                 // pinned pair list of the op (alive until it ran)
-    size_t staging_bytes = 0;
+    PinBlock<OpStats> pstats;
+    PinBlock<uint8_t> staging;                  // pair list of the op (alive until it ran)
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // op start, kernel start, kernel end, op end
     float ms = 0.f, compute_ms = 0.f;
     uint64_t algo_bytes = 0, out_portable = 0;
@@ -335,35 +418,37 @@ struct rb200_set {
     std::vector<uint64_t> h_ebytes; // host mirror: upper bound of the "effective bytes" (rb200_device.cuh) per bitmap
     std::vector<uint8_t> h_flags;   // per bitmap: COW flag to propagate
     // host copy of the directory (pinned) and, for a set packed for download, of its payload
-    uint8_t *m_dir = nullptr, *m_slab = nullptr;
-    rb200_set *mirror = nullptr;    // rb200_set_download: this set packed, directory and payload on the host
+    PinBlock<uint8_t> m_dir, m_slab;
+    SetPtr mirror;                  // rb200_set_download: this set packed, directory and payload on the host
 
     SetView view() const {
+        const uint8_t *d = d_dir.get();
         SetView v;
-        v.bm_beg = (const uint32_t *)(d_dir + L.o_beg);
-        v.bm_cnt = (const uint32_t *)(d_dir + L.o_cnt);
-        v.c_key = (const uint16_t *)(d_dir + L.o_key);
-        v.c_type = (const uint8_t *)(d_dir + L.o_type);
-        v.c_card = (const uint32_t *)(d_dir + L.o_card);
-        v.c_len = (const uint32_t *)(d_dir + L.o_len);
-        v.c_off = (const uint64_t *)(d_dir + L.o_off);
-        v.c_src = (const uint32_t *)(d_dir + L.o_src);
+        v.bm_beg = (const uint32_t *)(d + L.o_beg);
+        v.bm_cnt = (const uint32_t *)(d + L.o_cnt);
+        v.c_key = (const uint16_t *)(d + L.o_key);
+        v.c_type = (const uint8_t *)(d + L.o_type);
+        v.c_card = (const uint32_t *)(d + L.o_card);
+        v.c_len = (const uint32_t *)(d + L.o_len);
+        v.c_off = (const uint64_t *)(d + L.o_off);
+        v.c_src = (const uint32_t *)(d + L.o_src);
         v.payload = d_base;
         return v;
     }
     SetOut out() {
+        uint8_t *d = d_dir.get();
         SetOut v;
-        v.bm_beg = (uint32_t *)(d_dir + L.o_beg);
-        v.bm_cnt = (uint32_t *)(d_dir + L.o_cnt);
-        v.bm_card = (uint64_t *)(d_dir + L.o_bcard);
-        v.bm_bytes = (uint64_t *)(d_dir + L.o_bbytes);
-        v.bm_ebytes = (uint64_t *)(d_dir + L.o_bebytes);
-        v.c_key = (uint16_t *)(d_dir + L.o_key);
-        v.c_type = (uint8_t *)(d_dir + L.o_type);
-        v.c_card = (uint32_t *)(d_dir + L.o_card);
-        v.c_len = (uint32_t *)(d_dir + L.o_len);
-        v.c_off = (uint64_t *)(d_dir + L.o_off);
-        v.c_src = (uint32_t *)(d_dir + L.o_src);
+        v.bm_beg = (uint32_t *)(d + L.o_beg);
+        v.bm_cnt = (uint32_t *)(d + L.o_cnt);
+        v.bm_card = (uint64_t *)(d + L.o_bcard);
+        v.bm_bytes = (uint64_t *)(d + L.o_bbytes);
+        v.bm_ebytes = (uint64_t *)(d + L.o_bebytes);
+        v.c_key = (uint16_t *)(d + L.o_key);
+        v.c_type = (uint8_t *)(d + L.o_type);
+        v.c_card = (uint32_t *)(d + L.o_card);
+        v.c_len = (uint32_t *)(d + L.o_len);
+        v.c_off = (uint64_t *)(d + L.o_off);
+        v.c_src = (uint32_t *)(d + L.o_src);
         v.payload = d_slab;
         return v;
     }
@@ -371,33 +456,21 @@ struct rb200_set {
 
 namespace {
 
-rb200_set *set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
-    rb200_set *s = new rb200_set();
+SetPtr set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
+    SetPtr s(new rb200_set());
     s->n_bitmaps = nb;
     s->dir_cap = dir_cap;
     s->slab_cap = slab_cap;
     s->L.compute(nb, dir_cap);
-    s->d_dir = (uint8_t *)dev_alloc(s->L.total);
-    s->d_slab = (uint8_t *)dev_alloc(slab_cap);
-    if (!s->d_dir || !s->d_slab) {
-        dev_free(s->d_dir, s->L.total);
-        dev_free(s->d_slab, slab_cap);
-        delete s;
-        return nullptr;
-    }
-    s->slab = std::make_shared<Slab>(s->d_slab, slab_cap);
-    s->d_base = s->d_slab;
+    if (!s->d_dir.reset(s->L.total)) return nullptr;
+    s->slab = std::make_shared<Slab>(slab_cap);
+    if (!s->slab->p) return nullptr;
+    s->d_slab = s->d_base = s->slab->p;
     s->h_cnt.assign(nb, 0);
     s->h_bytes.assign(nb, 0);
     s->h_ebytes.assign(nb, 0);
     s->h_flags.assign(nb, 0);
     return s;
-}
-
-void set_drop_mirror(rb200_set *s) {
-    pin_free(s->m_dir, s->L.total);
-    pin_free(s->m_slab, s->slab_used);
-    s->m_dir = s->m_slab = nullptr;
 }
 
 cudaEvent_t ev_get() {
@@ -425,27 +498,24 @@ void ev_put(cudaEvent_t e) {
 // outlive a synchronisation of the stream after the last flush.
 struct H2DStager {
     static constexpr size_t CH = (size_t)32 << 20;
-    uint8_t *dst, *chunk[2];
+    uint8_t *dst;
+    PinBlock<uint8_t> chunk[2];
     cudaEvent_t cev[2] = {nullptr, nullptr};
     bool cev_used[2] = {false, false};
     bool ok;
     int cur = 0;
     size_t used = 0;
     uint64_t base = 0;
-    explicit H2DStager(uint8_t *d) : dst(d) {
-        chunk[0] = (uint8_t *)pin_alloc(CH);
-        chunk[1] = (uint8_t *)pin_alloc(CH);
+    explicit H2DStager(uint8_t *d) : dst(d), chunk{PinBlock<uint8_t>(CH), PinBlock<uint8_t>(CH)} {
         ok = chunk[0] && chunk[1];
         for (int k = 0; k < 2 && ok; k++) ok = cudaEventCreateWithFlags(&cev[k], cudaEventDisableTiming) == cudaSuccess;
     }
     ~H2DStager() {
         for (int k = 0; k < 2; k++) if (cev[k]) cudaEventDestroy(cev[k]);
-        pin_free(chunk[0], CH);
-        pin_free(chunk[1], CH);
     }
     bool flush() {
         if (used) {
-            if (cudaMemcpyAsync(dst + base, chunk[cur], used, cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
+            if (cudaMemcpyAsync(dst + base, chunk[cur].get(), used, cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
                 return false;
             cudaEventRecord(cev[cur], g.stream);
             cev_used[cur] = true;
@@ -462,10 +532,10 @@ struct H2DStager {
             if (used == CH && !flush()) return false;
             const size_t take = std::min(CH - used, n);
             if (p) {
-                memcpy(chunk[cur] + used, p, take);
+                memcpy(chunk[cur].get() + used, p, take);
                 p += take;
             } else {
-                memset(chunk[cur] + used, 0, take);
+                memset(chunk[cur].get() + used, 0, take);
             }
             used += take;
             n -= take;
@@ -473,6 +543,57 @@ struct H2DStager {
         return true;
     }
 };
+
+// The ending of a call that waits for its device work before it returns.  begin() records the op's
+// start event (a timed call) and resets the stats; kernels_begin() / kernels_end() / end() mark the
+// timed brackets; finish(ok) fetches the stats, waits for the stream and checks for a launch error,
+// and a timed call then becomes what the rb200_last_* getters describe.  A call that returns before
+// finish() still waits for the stream, here in the destructor: declared after the pinned blocks the
+// stream may still be copying, the helper is destroyed, and the stream drained, before they go back
+// to the pool.  `what` / `launch_what` head t_err for a failed wait / launch (no message if null).
+class SyncCall {
+   public:
+    explicit SyncCall(const char *what = nullptr, const char *launch_what = nullptr, bool timed = false)
+        : what_(what), launch_what_(launch_what ? launch_what : what), timed_(timed) {}
+    SyncCall(const SyncCall &) = delete;
+    ~SyncCall() { if (!finished_) cudaStreamSynchronize(g.stream); }
+    bool begin() {
+        if (timed_) cudaEventRecord(g.ev0, g.stream);
+        return stats_reset();
+    }
+    void kernels_begin() { cudaEventRecord(g.evk0, g.stream); }
+    void kernels_end() { cudaEventRecord(g.evk1, g.stream); }
+    void end() { cudaEventRecord(g.ev1, g.stream); }
+    bool finish(bool ok, bool fetch_stats = true) {
+        finished_ = true;
+        if (fetch_stats) ok = ok && stats_fetch();
+        cudaError_t e = cudaStreamSynchronize(g.stream);
+        const bool waited = e == cudaSuccess;
+        if (waited) e = cudaGetLastError();
+        if (e != cudaSuccess) {
+            if (what_ && (!waited || ok)) t_err = std::string(waited ? launch_what_ : what_) + ": " + cudaGetErrorString(e);
+            ok = false;
+        }
+        if (ok && timed_) {
+            g.last_op = nullptr;  // the rb200_last_* getters now describe this (synchronous) op
+            cudaEventElapsedTime(&g.last_ms, g.ev0, g.ev1);
+            cudaEventElapsedTime(&g.last_compute_ms, g.evk0, g.evk1);
+        }
+        return ok;
+    }
+
+   private:
+    const char *what_, *launch_what_;
+    bool timed_, finished_ = false;
+};
+
+// The batch op that produced s has run (or was never enqueued): its events, counters and pair list
+// go back to the pools.
+void retire_op(rb200_set *s) {
+    for (int k = 0; k < 4; k++) { ev_put(s->ev[k]); s->ev[k] = nullptr; }
+    s->pstats.reset();
+    s->staging.reset();
+}
 
 // Wait for the op that produced `cs` (if it is still in flight) and take over its counters.
 // false: the op failed (t_err says why); the set must not be used.
@@ -483,23 +604,24 @@ bool resolve(const rb200_set *cs) {
         return !s->failed;
     }
     s->pending = false;
+    const OpStats &st = *s->pstats.get();
     cudaError_t e = cudaEventSynchronize(s->ev[3]);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) {
         t_err = std::string("batch op: ") + cudaGetErrorString(e);
         s->failed = true;
-    } else if (s->pstats->error) {
-        t_err = s->pstats->error == 2 ? "internal: result slab bound exceeded" : "internal: result slot bound exceeded";
+    } else if (st.error) {
+        t_err = st.error == 2 ? "internal: result slab bound exceeded" : "internal: result slot bound exceeded";
         s->failed = true;
     } else {
         cudaEventElapsedTime(&s->ms, s->ev[0], s->ev[3]);
         cudaEventElapsedTime(&s->compute_ms, s->ev[1], s->ev[2]);
-        s->algo_bytes = s->pstats->algo_bytes;
-        s->out_portable = s->pstats->out_portable;
-        s->n_containers = s->pstats->dir_cursor;
-        s->slab_used = s->pstats->slab_cursor;
+        s->algo_bytes = st.algo_bytes;
+        s->out_portable = st.out_portable;
+        s->n_containers = st.dir_cursor;
+        s->slab_used = st.slab_cursor;
         for (int k = 0; k < 2; k++)   // an operand none of whose containers was shared is not held
-            if (!s->pstats->shared_used[k]) s->held[k].reset();
+            if (!st.shared_used[k]) s->held[k].reset();
         if (s->n_bitmaps == 1 && !s->sharing()) {  // a single result: its mirrors are the op's counters, no extra D2H
             s->h_cnt[0] = (uint32_t)s->n_containers;
             s->h_bytes[0] = s->slab_used;
@@ -507,11 +629,7 @@ bool resolve(const rb200_set *cs) {
             s->mirrors_pending = false;
         }
     }
-    for (int k = 0; k < 4; k++) { ev_put(s->ev[k]); s->ev[k] = nullptr; }
-    pin_free(s->pstats, sizeof(OpStats));
-    pin_free(s->staging, s->staging_bytes);
-    s->pstats = nullptr;
-    s->staging = nullptr;
+    retire_op(s);
     if (g.last_op == s) {
         g.last_ms = s->ms;
         g.last_compute_ms = s->compute_ms;
@@ -524,20 +642,11 @@ bool resolve(const rb200_set *cs) {
 void set_delete(rb200_set *s) {
     if (!s) return;
     if (s->pending) resolve(s);  // pinned staging / counters must not be recycled under a pending DMA
-    for (int k = 0; k < 4; k++) { ev_put(s->ev[k]); s->ev[k] = nullptr; }  // (only set if the enqueue failed half way)
-    pin_free(s->pstats, sizeof(OpStats));
-    pin_free(s->staging, s->staging_bytes);
-    s->pstats = nullptr;
-    s->staging = nullptr;
+    retire_op(s);                // (only needed if the enqueue failed half way)
     if (g.last_op == s) g.last_op = nullptr;
-    set_drop_mirror(s);
-    set_delete(s->mirror);
-    dev_free(s->d_dir, s->L.total);
-    s->slab.reset();     // the slabs return to the pool unless a result still points into them
-    s->held[0].reset();
-    s->held[1].reset();
-    delete s;
+    delete s;  // the slabs return to the pool unless a result still points into them
 }
+void SetFree::operator()(rb200_set *s) const { set_delete(s); }
 
 // ------------------------------------------------------------------ host containers
 inline const void *unwrap_shared(const void *c, uint8_t &type) {  // containers.h:105-114
@@ -995,19 +1104,16 @@ rb200_set *upload_impl(const PackSrc &src) {
             for (int32_t i = 0; i < v.size; i++) slab += round16(stored_bytes(v.type[i], v.len[i]));
         }
     }
-    rb200_set *s = set_new((uint32_t)nb, nc, slab);
+    SetPtr s = set_new((uint32_t)nb, nc, slab);
     if (!s) return nullptr;
     s->n_containers = nc;
     s->slab_used = slab;
     // pass 2: directory into one pinned block, payload streamed through two pinned chunks
-    uint8_t *hd = (uint8_t *)pin_alloc(s->L.total);
-    const size_t CH = (size_t)32 << 20;
-    uint8_t *chunk[2] = {(uint8_t *)pin_alloc(CH), (uint8_t *)pin_alloc(CH)};
-    cudaEvent_t cev[2];
-    bool ok = hd && chunk[0] && chunk[1];
-    for (int k = 0; k < 2; k++) cudaEventCreateWithFlags(&cev[k], cudaEventDisableTiming);
-    bool cev_used[2] = {false, false};
+    PinBlock<uint8_t> dir(s->L.total);
+    H2DStager stage(s->d_slab);
+    bool ok = dir && stage.ok;
     if (ok) {
+        uint8_t *hd = dir.get();
         uint32_t *bm_beg = (uint32_t *)(hd + s->L.o_beg), *bm_cnt = (uint32_t *)(hd + s->L.o_cnt);
         uint64_t *bm_card = (uint64_t *)(hd + s->L.o_bcard);
         uint16_t *c_key = (uint16_t *)(hd + s->L.o_key);
@@ -1016,22 +1122,7 @@ rb200_set *upload_impl(const PackSrc &src) {
         uint64_t *c_off = (uint64_t *)(hd + s->L.o_off);
         uint32_t *c_src = (uint32_t *)(hd + s->L.o_src);
         if (src.bms) s->h_ptr_all = std::make_shared<std::vector<const void *>>(nc);
-        uint64_t ci = 0, off = 0, chunk_base = 0;
-        int cur = 0;
-        size_t used = 0;
-        auto flush = [&]() -> bool {
-            if (used) {
-                if (cudaMemcpyAsync(s->d_slab + chunk_base, chunk[cur], used, cudaMemcpyHostToDevice,
-                                    g.stream) != cudaSuccess) return false;
-                cudaEventRecord(cev[cur], g.stream);
-                cev_used[cur] = true;
-            }
-            chunk_base += used;
-            used = 0;
-            cur ^= 1;
-            if (cev_used[cur]) cudaEventSynchronize(cev[cur]);
-            return true;
-        };
+        uint64_t ci = 0, off = 0;
         for (size_t b = 0; b < nb && ok; b++) {
             const roaring_array_t *ra = src.bms ? &src.bms[b]->high_low_container : nullptr;
             const PView *pv = src.views ? &(*src.views)[b] : nullptr;
@@ -1084,10 +1175,7 @@ rb200_set *upload_impl(const PackSrc &src) {
                     }
                 }
                 const uint32_t sb = stored_bytes(t, len), sb16 = round16(sb);
-                if (used + sb16 > CH) ok = flush();
-                memcpy(chunk[cur] + used, p, sb);
-                if (sb16 > sb) memset(chunk[cur] + used + sb, 0, sb16 - sb);
-                used += sb16;
+                ok = ok && stage.put(p, sb) && stage.put(nullptr, sb16 - sb);
                 c_key[ci] = key;
                 c_type[ci] = t;
                 c_card[ci] = card;
@@ -1105,21 +1193,15 @@ rb200_set *upload_impl(const PackSrc &src) {
             s->h_bytes[b] = bbytes;
             s->h_ebytes[b] = bebytes;
         }
-        if (ok) ok = flush();
-        if (ok && cudaMemcpyAsync(s->d_dir, hd, s->L.total, cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
-            ok = false;
+        ok = ok && stage.flush() &&
+             cudaMemcpyAsync(s->d_dir.get(), hd, s->L.total, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
         if (cudaStreamSynchronize(g.stream) != cudaSuccess) ok = false;
     }
-    for (int k = 0; k < 2; k++) cudaEventDestroy(cev[k]);
-    pin_free(hd, s->L.total);
-    pin_free(chunk[0], CH);
-    pin_free(chunk[1], CH);
     if (!ok) {
         if (t_err.empty()) t_err = "upload failed";
-        set_delete(s);
         return nullptr;
     }
-    return s;
+    return s.release();
 }
 
 }  // namespace
@@ -1176,19 +1258,21 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
         raw_total += (lens[i] + 15) & ~(uint64_t)15;
         slab_total += ((lens[i] + 15) & ~(uint64_t)15) + 16ull * size;   // payload <= blob bytes, + 16-byte padding per container
     }
-    rb200_set *s = set_new((uint32_t)n, nc, slab_total + 16);
+    SetPtr s = set_new((uint32_t)n, nc, slab_total + 16);
     if (!s) return nullptr;
     s->n_containers = nc;
     s->slab_used = slab_total;
     // per-bitmap tables: [roff | rlen | slab_base] for the kernels, bm_beg / bm_cnt into the directory
-    const size_t tb = 24 * (n ? n : 1);
-    uint64_t *h_tab = (uint64_t *)pin_alloc(tb), *d_tab = (uint64_t *)dev_alloc(tb);
-    uint32_t *h_bc = (uint32_t *)pin_alloc(8 * (n ? n : 1));
-    uint8_t *d_raw = (uint8_t *)dev_alloc(raw_total ? raw_total : 16);
-    uint64_t *d_src = (uint64_t *)dev_alloc(8 * (nc ? nc : 1));
-    H2DStager stage(d_raw);
-    bool ok = h_tab && d_tab && h_bc && d_raw && d_src && stage.ok;
+    PinBlock<uint64_t> tab(3 * n);
+    PinBlock<uint32_t> bc(2 * n);
+    DevBlock<uint64_t> d_tab(3 * n), d_src(nc);
+    DevBlock<uint8_t> d_raw(raw_total);
+    H2DStager stage(d_raw.get());
+    SyncCall call("deserialize");
+    bool ok = tab && d_tab && bc && d_raw && d_src && stage.ok;
     if (ok) {
+        uint64_t *h_tab = tab.get();
+        uint32_t *h_bc = bc.get();
         uint64_t ro = 0, so = 0, cb = 0;
         for (size_t i = 0; i < n; i++) {
             h_tab[i] = ro;
@@ -1207,29 +1291,25 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
             so += ((lens[i] + 15) & ~(uint64_t)15) + 16ull * cnt[i];
             cb += cnt[i];
         }
-        ok = cudaMemcpyAsync(d_tab, h_tab, tb, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+        ok = cudaMemcpyAsync(d_tab.get(), h_tab, d_tab.bytes(), cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
              (n == 0 ||
-              (cudaMemcpyAsync(s->d_dir + s->L.o_beg, h_bc, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
-               cudaMemcpyAsync(s->d_dir + s->L.o_cnt, h_bc + n, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess));
+              (cudaMemcpyAsync(s->d_dir.get() + s->L.o_beg, h_bc, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+               cudaMemcpyAsync(s->d_dir.get() + s->L.o_cnt, h_bc + n, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess));
         // raw bytes as one stream through the two pinned chunks
         for (size_t i = 0; i < n && ok; i++)
             ok = stage.put(bufs[i], lens[i]) && stage.put(nullptr, ((lens[i] + 15) & ~(size_t)15) - lens[i]);
         if (ok) ok = stage.flush();
     }
     if (ok) {
-        ok = stats_reset();
+        ok = call.begin();
+        const uint64_t *t = d_tab.get();
         if (frozen)
-            launch_deserialize_frozen(d_raw, d_tab, d_tab + n, d_tab + 2 * n, (uint32_t)n, nc, s->out(), d_src,
+            launch_deserialize_frozen(d_raw.get(), t, t + n, t + 2 * n, (uint32_t)n, nc, s->out(), d_src.get(),
                                       g.d_stats, g.stream);
         else
-            launch_deserialize(d_raw, d_tab, d_tab + n, d_tab + 2 * n, (uint32_t)n, nc, s->out(), d_src, g.d_stats,
+            launch_deserialize(d_raw.get(), t, t + n, t + 2 * n, (uint32_t)n, nc, s->out(), d_src.get(), g.d_stats,
                                g.stream);
-        ok = ok && stats_fetch();
-        cudaError_t e = cudaStreamSynchronize(g.stream);
-        if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
-            t_err = std::string("deserialize: ") + cudaGetErrorString(e);
-            ok = false;
-        }
+        ok = call.finish(ok);
         if (ok && g.h_stats->error == 4u) {
             t_err = "malformed serialized bitmap: invalid container contents (a run ends past 65535, runs "
                     "overlap or are out of order, or array values are not strictly increasing)";
@@ -1239,21 +1319,13 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
                     std::to_string((uint64_t)n - g.h_stats->nk);
             ok = false;
         }
-    } else {
-        cudaStreamSynchronize(g.stream);
     }
-    if (ok) s->mirrors_pending = n > 0;   // exact per-bitmap bytes / effective bytes: k_deser_bitmap_cards wrote them
-    pin_free(h_tab, tb);
-    pin_free(h_bc, 8 * (n ? n : 1));
-    dev_free(d_tab, tb);
-    dev_free(d_raw, raw_total ? raw_total : 16);
-    dev_free(d_src, 8 * (nc ? nc : 1));
     if (!ok) {
         if (t_err.empty()) t_err = "upload_serialized failed";
-        set_delete(s);
         return nullptr;
     }
-    return s;
+    s->mirrors_pending = n > 0;   // exact per-bitmap bytes / effective bytes: k_deser_bitmap_cards wrote them
+    return s.release();
 }
 
 // Declare that the host bitmaps this set was uploaded from stay alive (and unmodified) for as long
@@ -1302,10 +1374,11 @@ bool ensure_mirrors(const rb200_set *cs) {
     const size_t nb = s->n_bitmaps;
     // one copy: [cnt | bcard | bbytes | bebytes], all written by the kernel that produced the set
     const size_t bytes = (s->L.o_bebytes - s->L.o_cnt) + 8 * nb;
-    uint8_t *h = (uint8_t *)pin_alloc(bytes);
-    if (!h) return false;
-    bool ok = cudaMemcpyAsync(h, s->d_dir + s->L.o_cnt, bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-              cudaStreamSynchronize(g.stream) == cudaSuccess;
+    PinBlock<uint8_t> hb(bytes);
+    if (!hb) return false;
+    const uint8_t *h = hb.get();
+    const bool ok = cudaMemcpyAsync(hb.get(), s->d_dir.get() + s->L.o_cnt, bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                    cudaStreamSynchronize(g.stream) == cudaSuccess;
     if (ok) {
         const uint32_t *cnt = (const uint32_t *)h;
         const uint64_t *card = (const uint64_t *)(h + (s->L.o_bcard - s->L.o_cnt));
@@ -1321,13 +1394,11 @@ bool ensure_mirrors(const rb200_set *cs) {
     } else {
         t_err = "fetching result directory failed";
     }
-    pin_free(h, bytes);
     return ok;
 }
 
 struct ItemsBuf {
-    uint8_t *block = nullptr;
-    size_t bytes = 0;
+    DevBlock<uint8_t> mem;
     Items it;
     // with_desc: cell descriptors (k_compute_items); with_order: batches with at least order_min item
     // slots also get them sorted by class
@@ -1344,9 +1415,8 @@ struct ItemsBuf {
         const size_t o_key = o; o += al256(2 * W);
         const size_t o_kind = o; o += al256(W);
         const size_t o_otype = o; o += al256(W);
-        bytes = o ? o : 256;
-        block = (uint8_t *)dev_alloc(bytes);
-        if (!block) return false;
+        if (!mem.reset(o ? o : 256)) return false;
+        uint8_t *block = mem.get();
         it.slot_off = (uint64_t *)(block + o_off);
         it.desc = with_desc ? (uint4 *)(block + o_desc) : nullptr;
         it.desc_cls = with_order ? (uint4 *)(block + o_dcls) : nullptr;
@@ -1360,13 +1430,12 @@ struct ItemsBuf {
         it.otype = block + o_otype;
         return true;
     }
-    void release() { dev_free(block, bytes); block = nullptr; }
 };
 
 // pair lists + item offsets: one pinned staging block, one H2D copy
 struct PairBuf {
-    uint8_t *h = nullptr, *d = nullptr;
-    size_t bytes = 0;
+    PinBlock<uint8_t> h;
+    DevBlock<uint8_t> d;
     uint32_t *d_ia = nullptr, *d_ib = nullptr;
     uint64_t *d_off = nullptr;
     uint64_t W = 0;
@@ -1380,12 +1449,10 @@ struct PairBuf {
         if (!ensure_mirrors(A) || !ensure_mirrors(B)) return false;
         if (np > 0xffffffffull) { t_err = "too many pairs in one batch (2^32 - 1 at most)"; return false; }
         const size_t o_off = 0, o_ia = al256(8 * (np + 1)), o_ib = o_ia + al256(4 * np);
-        bytes = o_ib + al256(4 * np);
-        h = (uint8_t *)pin_alloc(bytes);
-        d = (uint8_t *)dev_alloc(bytes);
-        if (!h || !d) return false;
-        uint64_t *off = (uint64_t *)(h + o_off);
-        uint32_t *hia = (uint32_t *)(h + o_ia), *hib = (uint32_t *)(h + o_ib);
+        const size_t bytes = o_ib + al256(4 * np);
+        if (!h.reset(bytes) || !d.reset(bytes)) return false;
+        uint64_t *off = (uint64_t *)(h.get() + o_off);
+        uint32_t *hia = (uint32_t *)(h.get() + o_ia), *hib = (uint32_t *)(h.get() + o_ib);
         uint64_t w = 0, sb = 0, sbs = 0;
         for (size_t p = 0; p < np; p++) {
             const uint32_t a = ia[p], b = ib[p];
@@ -1435,15 +1502,10 @@ struct PairBuf {
         W = w;
         slab_bound_copy = sb;
         slab_bound = share ? sbs : sb;
-        d_off = (uint64_t *)(d + o_off);
-        d_ia = (uint32_t *)(d + o_ia);
-        d_ib = (uint32_t *)(d + o_ib);
-        return cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
-    }
-    void release() {
-        pin_free(h, bytes);
-        dev_free(d, bytes);
-        h = d = nullptr;
+        d_off = (uint64_t *)(d.get() + o_off);
+        d_ia = (uint32_t *)(d.get() + o_ia);
+        d_ib = (uint32_t *)(d.get() + o_ib);
+        return cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
     }
 };
 
@@ -1504,7 +1566,7 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     if (np > 0xffffffffull) { t_err = "too many pairs"; return nullptr; }
     PairBuf pb;
     ItemsBuf ib_;
-    rb200_set *R = nullptr;
+    SetPtr R;
     // Non-lazy ops share the unmatched containers of their operands instead of copying them: the
     // result points into the operands' slabs (the reference shares them too when copy-on-write is on,
     // roaring.c:918-922; no batch op ever writes into an operand).  Lazy ops and flips keep copying,
@@ -1524,16 +1586,15 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     PassShare sh = {false, false, 0, 0, 0};
     if (ok) {
         R = set_new((uint32_t)np, pb.W, pb.slab_bound);
-        if (R && (onA || onB) && !share_operands(R, A, B, onA, onB, sh)) {
-            set_delete(R);   // out of the offsets' reach: copy everything into a slab sized for it
+        if (R && (onA || onB) && !share_operands(R.get(), A, B, onA, onB, sh)) {
+            R.reset();   // out of the offsets' reach: copy everything into a slab sized for it
             R = set_new((uint32_t)np, pb.W, pb.slab_bound_copy);
         }
         ok = R != nullptr;
     }
     if (ok) {
         for (int k = 0; k < 4; k++) R->ev[k] = ev_get();
-        R->pstats = (OpStats *)pin_alloc(sizeof(OpStats));
-        ok = R->pstats && R->ev[0] && R->ev[1] && R->ev[2] && R->ev[3];
+        ok = R->pstats.reset(1) && R->ev[0] && R->ev[1] && R->ev[2] && R->ev[3];
     }
     if (ok) {
         cudaEventRecord(R->ev[0], g.stream);
@@ -1554,29 +1615,26 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_stats, rules, copy_ticket, g.stream);
         cudaEventRecord(R->ev[2], g.stream);
         launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, sh, R->out(), g.d_stats, g.stream);
-        ok = ok && cudaMemcpyAsync(R->pstats, g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = ok && cudaMemcpyAsync(R->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
         cudaEventRecord(R->ev[3], g.stream);
         // no synchronisation here: the counters are taken over by resolve() on first use
         R->pending = true;
-        R->staging = pb.h;            // the pinned pair list must outlive its H2D copy
-        R->staging_bytes = pb.bytes;
-        pb.h = nullptr;
+        R->staging = std::move(pb.h);   // the pinned pair list must outlive its H2D copy
         R->parentA = A->h_ptr;
         R->parentB = B->h_ptr;
         R->portable_bytes = 0;
         R->mirrors_pending = np > 0;  // h_cnt / h_bytes / h_card: see ensure_mirrors()
         R->lazy = (rules & RULES_LAZY) != 0 && !(rules & RULES_FLIP);
         for (size_t p = 0; p < np; p++) R->h_flags[p] = (A->h_flags[ia[p]] | B->h_flags[ib[p]]) & FLAG_COW;
-        g.last_op = R;
+        g.last_op = R.get();
     }
-    pb.release();     // device buffers: stream-ordered reuse
-    ib_.release();
+    // the device buffers go back when pb / ib_ leave scope: stream-ordered reuse
     if (!ok) {
         if (t_err.empty()) t_err = "batch op: enqueue failed";
-        set_delete(R);
+        if (pb.h) cudaStreamSynchronize(g.stream);   // the pair list's H2D copy may still read it
         return nullptr;
     }
-    return R;
+    return R.release();
 }
 
 }  // namespace
@@ -1603,36 +1661,24 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
     if (reject_lazy(A, "and_cardinality") || reject_lazy(B, "and_cardinality")) return -1;
     PairBuf pb;
     ItemsBuf ib_;
-    uint64_t *d_out = nullptr, *h_out = nullptr;
-    bool ok = pb.build(A, B, ia, ib, np, OP_AND);
-    if (ok) ok = ib_.alloc(pb.W, false, false);
-    if (ok) { d_out = (uint64_t *)dev_alloc(8 * np); h_out = (uint64_t *)pin_alloc(8 * np); ok = d_out && h_out; }
+    DevBlock<uint64_t> d_out;
+    PinBlock<uint64_t> h_out;
+    SyncCall call("and_cardinality", "and_cardinality launch", true);
+    bool ok = pb.build(A, B, ia, ib, np, OP_AND) && ib_.alloc(pb.W, false, false) && d_out.reset(np) && h_out.reset(np);
     if (ok) {
-        cudaEventRecord(g.ev0, g.stream);
-        ok = stats_reset();
+        ok = call.begin();
         const SetView va = A->view(), vb = B->view();
         launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, OP_AND, true, 0, PassShare{false, false, 0, 0, 0}, ib_.it,
                           g.d_stats, g.stream);
-        cudaEventRecord(g.evk0, g.stream);
+        call.kernels_begin();
         launch_card_items(va, vb, ib_.it, pb.W, g.d_stats, g.stream);
-        cudaEventRecord(g.evk1, g.stream);
-        launch_finalize_cards(ib_.it, pb.d_off, (uint32_t)np, d_out, g.stream);
-        cudaEventRecord(g.ev1, g.stream);
-        ok = ok && cudaMemcpyAsync(h_out, d_out, 8 * np, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        cudaError_t e = cudaStreamSynchronize(g.stream);
-        if (e != cudaSuccess) { t_err = std::string("and_cardinality: ") + cudaGetErrorString(e); ok = false; }
-        if (ok && (e = cudaGetLastError()) != cudaSuccess) { t_err = std::string("and_cardinality launch: ") + cudaGetErrorString(e); ok = false; }
+        call.kernels_end();
+        launch_finalize_cards(ib_.it, pb.d_off, (uint32_t)np, d_out.get(), g.stream);
+        call.end();
+        ok = ok && cudaMemcpyAsync(h_out.get(), d_out.get(), 8 * np, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok, false);
     }
-    if (ok) {
-        memcpy(out, h_out, 8 * np);
-        g.last_op = nullptr;  // the rb200_last_* getters now describe this (synchronous) op
-        cudaEventElapsedTime(&g.last_ms, g.ev0, g.ev1);
-        cudaEventElapsedTime(&g.last_compute_ms, g.evk0, g.evk1);
-    }
-    dev_free(d_out, 8 * np);
-    pin_free(h_out, 8 * np);
-    pb.release();
-    ib_.release();
+    if (ok) memcpy(out, h_out.get(), 8 * np);
     return ok ? 0 : -1;
 }
 
@@ -1674,22 +1720,22 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     if (tot > 0xffffffffu) { t_err = "or_many: the inputs carry more than 2^32 - 1 containers (every key counts, whatever the key range)"; return nullptr; }
     uint64_t maxk = key_lo <= key_hi ? (uint64_t)key_hi - key_lo + 1 : 0;
     if (tot < maxk) maxk = tot;
-    rb200_set *R = set_new(1, maxk, maxk * BITSET_BYTES);
+    SetPtr R = set_new(1, maxk, maxk * BITSET_BYTES);
     if (!R) return nullptr;
-    uint32_t *d_idx = nullptr, *h_idx = nullptr;
+    DevBlock<uint32_t> d_idx;
+    PinBlock<uint32_t> h_idx, ck;
+    DevBlock<uint8_t> d_index;
+    SyncCall call("or_many", "or_many launch", true);
     bool ok = true;
     if (idx && n) {
-        d_idx = (uint32_t *)dev_alloc(4 * n);
-        h_idx = (uint32_t *)pin_alloc(4 * n);
-        ok = d_idx && h_idx;
+        ok = d_idx.reset(n) && h_idx.reset(n);
         if (ok) {
-            memcpy(h_idx, idx, 4 * n);
-            ok = cudaMemcpyAsync(d_idx, h_idx, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+            memcpy(h_idx.get(), idx, 4 * n);
+            ok = cudaMemcpyAsync(d_idx.get(), h_idx.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
         }
     }
-    uint32_t *h_ck = nullptr;
     cudaEvent_t evc0 = nullptr, evc1 = nullptr;
-    if (ok && want_ck) { h_ck = (uint32_t *)pin_alloc(65536 * 4); ok = h_ck != nullptr; }
+    if (ok && want_ck) ok = ck.reset(65536);
     if (ok && sh) { evc0 = ev_get(); evc1 = ev_get(); ok = evc0 && evc1; }
     // index: entries + work-unit table from the device pool
     uint64_t tot_kib = 0;
@@ -1698,12 +1744,9 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     // key-window index build: per-(window, chunk of 256 bitmaps) key counts when there are several chunks
     const uint64_t m2_chunks = (n + 255) / 256;
     const size_t tab_bytes = m2_chunks > 1 && m2_chunks <= M2W_MAX_CHUNKS ? (size_t)2048 * m2_chunks * 32 * 4 : 0;
-    const size_t e_bytes = al256(16 * tot) + al256(4 * max_units) + al256(tab_bytes);
-    uint8_t *d_index = nullptr;
-    if (ok) { d_index = (uint8_t *)dev_alloc(e_bytes); ok = d_index != nullptr; }
+    if (ok) ok = d_index.reset(al256(16 * tot) + al256(4 * max_units) + al256(tab_bytes));
     if (ok) {
-        cudaEventRecord(g.ev0, g.stream);
-        ok = stats_reset();
+        ok = call.begin();
         const SetView vs = S->view();
         Many2Index ix;
         ix.key_cu = (unsigned long long *)g.d_m2_tables;          // [0, 2): zeroed per call
@@ -1719,8 +1762,8 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         ix.fold_F = g.d_m2_tables + 12 * 65536;
         ix.fold_L = g.d_m2_tables + 13 * 65536;
         ix.keys = g.d_keys;
-        ix.ent = (uint4 *)d_index;
-        ix.unit_ki = (uint32_t *)(d_index + al256(16 * tot));
+        ix.ent = (uint4 *)d_index.get();
+        ix.unit_ki = (uint32_t *)(d_index.get() + al256(16 * tot));
         // operand staging by TMA bulk copies pays off when the containers are mostly bitsets
         // (RB200_OR_MANY_TMA=0/1 forces the choice)
         static const int tma_env = []() { const char *e = getenv("RB200_OR_MANY_TMA"); return e ? atoi(e) : -1; }();
@@ -1732,32 +1775,27 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         const bool window_index = m2_chunks <= M2W_MAX_CHUNKS && n > 0 && (win_env >= 0 ? win_env != 0 : (tot >= 64 * (uint64_t)n));
         cudaMemsetAsync(g.d_m2_tables, 0, 3 * 65536 * sizeof(uint32_t), g.stream);
         if (want_ck) cudaMemsetAsync(g.d_cardkey, 0, 65536 * 4, g.stream);
-        launch_or_many2(vs, d_idx, (uint32_t)n, key_lo, key_hi, ix, (uint32_t)max_units,
+        launch_or_many2(vs, d_idx.get(), (uint32_t)n, key_lo, key_hi, ix, (uint32_t)max_units,
                         g.d_m2_scratch, g.d_m2_tickets, M2_SCRATCH_SLOTS, R->out(), want_ck ? g.d_cardkey : nullptr,
                         g.d_stats, g.sms, g.stream, g.evk0, use_tma, window_index,
-                        (uint32_t *)(d_index + al256(16 * tot) + al256(4 * max_units)));
+                        (uint32_t *)(d_index.get() + al256(16 * tot) + al256(4 * max_units)));
     }
     if (ok) {
-        cudaEventRecord(g.evk1, g.stream);
+        call.kernels_end();
         if (sh) {  // the ONE collective of the path: per-key cardinalities, summed over the ranks, on the device
             cudaEventRecord(evc0, g.stream);
             ok = ok && comm_allreduce_sum(sh->comm, g.d_cardkey + sh->span_lo, span_n, false, g.stream, t_err);
             cudaEventRecord(evc1, g.stream);
         }
-        cudaEventRecord(g.ev1, g.stream);
-        ok = ok && stats_fetch();
+        call.end();
         if (card_per_key)
-            ok = ok && cudaMemcpyAsync(h_ck, g.d_cardkey, 65536 * 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+            ok = ok && cudaMemcpyAsync(ck.get(), g.d_cardkey, 65536 * 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
         else if (sh)
-            ok = ok && cudaMemcpyAsync(h_ck, g.d_cardkey + sh->span_lo, 4ull * span_n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        cudaError_t e = cudaStreamSynchronize(g.stream);
-        if (e != cudaSuccess) { t_err = std::string("or_many: ") + cudaGetErrorString(e); ok = false; }
-        if (ok && (e = cudaGetLastError()) != cudaSuccess) { t_err = std::string("or_many launch: ") + cudaGetErrorString(e); ok = false; }
+            ok = ok && cudaMemcpyAsync(ck.get(), g.d_cardkey + sh->span_lo, 4ull * span_n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok);
     }
     if (ok) {
-        g.last_op = nullptr;  // the rb200_last_* getters now describe this (synchronous) op
-        cudaEventElapsedTime(&g.last_ms, g.ev0, g.ev1);
-        cudaEventElapsedTime(&g.last_compute_ms, g.evk0, g.evk1);
+        const uint32_t *h_ck = ck.get();
         const uint32_t nk = g.h_stats->nk;
         R->n_containers = nk;
         R->slab_used = (uint64_t)nk * BITSET_BYTES;
@@ -1785,18 +1823,13 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         if (key_lo == 0 && key_hi == 65535 && idx == nullptr) inb = S->portable_bytes;
         g.last_algo_bytes = inb;
     }
-    dev_free(d_idx, 4 * n);
-    dev_free(d_index, e_bytes);
-    pin_free(h_idx, 4 * n);
-    pin_free(h_ck, 65536 * 4);
     ev_put(evc0);
     ev_put(evc1);
     if (!ok) {
         if (t_err.empty()) t_err = "or_many failed";
-        set_delete(R);
         return nullptr;
     }
-    return R;
+    return R.release();
 }
 
 rb200_set_t *rb200_or_many_keyrange(const rb200_set_t *S, const uint32_t *idx, size_t n,
@@ -1826,7 +1859,7 @@ int rb200_set_add_cardinality_device(const rb200_set_t *s, uint64_t *d_acc) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
     if (s->failed) { t_err = "the operation that produced this set failed"; return -1; }
-    launch_sum_cardinalities((const uint64_t *)(s->d_dir + s->L.o_bcard), s->n_bitmaps, d_acc, g.stream);
+    launch_sum_cardinalities((const uint64_t *)(s->d_dir.get() + s->L.o_bcard), s->n_bitmaps, d_acc, g.stream);
     return 0;
 }
 // in-place all-reduce(sum) of `count` u64 words in device memory on the library stream
@@ -1850,41 +1883,34 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
         tot += S->h_cnt[b];
     }
     const uint64_t maxk = std::min<uint64_t>(65536, tot);
-    rb200_set *R = set_new(1, maxk, maxk * BITSET_BYTES);
+    SetPtr R = set_new(1, maxk, maxk * BITSET_BYTES);
     if (!R) return nullptr;
-    uint32_t *d_idx = nullptr, *h_idx = nullptr;
-    uint8_t *t_type = (uint8_t *)dev_alloc(maxk);
-    uint32_t *t_card = (uint32_t *)dev_alloc(4 * maxk), *t_len = (uint32_t *)dev_alloc(4 * maxk);
+    DevBlock<uint32_t> d_idx;
+    PinBlock<uint32_t> h_idx;
+    DevBlock<uint8_t> t_type(maxk);
+    DevBlock<uint32_t> t_card(maxk), t_len(maxk);
+    SyncCall call("xor_many", "xor_many launch", true);
     bool ok = t_type && t_card && t_len;
     if (ok && idx && n) {
-        d_idx = (uint32_t *)dev_alloc(4 * n);
-        h_idx = (uint32_t *)pin_alloc(4 * n);
-        ok = d_idx && h_idx;
+        ok = d_idx.reset(n) && h_idx.reset(n);
         if (ok) {
-            memcpy(h_idx, idx, 4 * n);
-            ok = cudaMemcpyAsync(d_idx, h_idx, 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+            memcpy(h_idx.get(), idx, 4 * n);
+            ok = cudaMemcpyAsync(d_idx.get(), h_idx.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
         }
     }
     if (ok) {
-        cudaEventRecord(g.ev0, g.stream);
-        ok = stats_reset();
+        ok = call.begin();
         const SetView vs = S->view();
-        launch_many_mark(vs, d_idx, (uint32_t)n, 0, 65535, g.d_flags, g.stream);
+        launch_many_mark(vs, d_idx.get(), (uint32_t)n, 0, 65535, g.d_flags, g.stream);
         launch_many_compact(g.d_flags, g.d_keys, g.d_stats, g.stream);
-        cudaEventRecord(g.evk0, g.stream);
-        launch_xor_many(vs, d_idx, (uint32_t)n, g.d_keys, t_type, t_card, t_len, R->out(), g.d_stats,
-                        g.sms, g.stream);
-        cudaEventRecord(g.evk1, g.stream);
-        cudaEventRecord(g.ev1, g.stream);
-        ok = ok && stats_fetch();
-        cudaError_t e = cudaStreamSynchronize(g.stream);
-        if (e != cudaSuccess) { t_err = std::string("xor_many: ") + cudaGetErrorString(e); ok = false; }
-        if (ok && (e = cudaGetLastError()) != cudaSuccess) { t_err = std::string("xor_many launch: ") + cudaGetErrorString(e); ok = false; }
+        call.kernels_begin();
+        launch_xor_many(vs, d_idx.get(), (uint32_t)n, g.d_keys, t_type.get(), t_card.get(), t_len.get(), R->out(),
+                        g.d_stats, g.sms, g.stream);
+        call.kernels_end();
+        call.end();
+        ok = call.finish(ok);
     }
     if (ok) {
-        g.last_op = nullptr;  // the rb200_last_* getters now describe this (synchronous) op
-        cudaEventElapsedTime(&g.last_ms, g.ev0, g.ev1);
-        cudaEventElapsedTime(&g.last_compute_ms, g.evk0, g.evk1);
         const uint32_t live = (uint32_t)g.h_stats->dir_cursor;
         R->n_containers = live;
         R->slab_used = (uint64_t)g.h_stats->nk * BITSET_BYTES;
@@ -1896,16 +1922,7 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
         R->h_flags[0] = fl & FLAG_COW;
         g.last_algo_bytes = (idx == nullptr) ? S->portable_bytes : 0;
     }
-    dev_free(d_idx, 4 * n);
-    pin_free(h_idx, 4 * n);
-    dev_free(t_type, maxk);
-    dev_free(t_card, 4 * maxk);
-    dev_free(t_len, 4 * maxk);
-    if (!ok) {
-        set_delete(R);
-        return nullptr;
-    }
-    return R;
+    return ok ? R.release() : nullptr;
 }
 
 int rb200_set_cardinalities(const rb200_set_t *s, uint64_t *out) {
@@ -1918,14 +1935,13 @@ int rb200_set_cardinalities(const rb200_set_t *s, uint64_t *out) {
         memcpy(out, s->h_card.data(), 8 * nb);
         return 0;
     }
-    uint64_t *h = (uint64_t *)pin_alloc(8 * nb);
+    PinBlock<uint64_t> h(nb);
     if (!h) return -1;
     // bm_card is maintained by upload / finalize / or_many
-    bool ok = cudaMemcpyAsync(h, s->d_dir + s->L.o_bcard, 8 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    bool ok = cudaMemcpyAsync(h.get(), s->d_dir.get() + s->L.o_bcard, 8 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
     ok = ok && cudaStreamSynchronize(g.stream) == cudaSuccess;
-    if (ok) memcpy(out, h, 8 * nb);
+    if (ok) memcpy(out, h.get(), 8 * nb);
     else t_err = "set_cardinalities: copy failed";
-    pin_free(h, 8 * nb);
     return ok ? 0 : -1;
 }
 
@@ -1935,16 +1951,17 @@ int rb200_set_cardinalities(const rb200_set_t *s, uint64_t *out) {
 namespace {
 
 roaring_bitmap_t *build_bitmap(const rb200_set *s, size_t i, const uint8_t *slab = nullptr, uint64_t bias = 0) {
-    if (!slab) slab = s->m_slab;
-    const uint32_t *c_src = (const uint32_t *)(s->m_dir + s->L.o_src);
+    if (!slab) slab = s->m_slab.get();
+    const uint8_t *m_dir = s->m_dir.get();
+    const uint32_t *c_src = (const uint32_t *)(m_dir + s->L.o_src);
     const std::vector<const void *> *tabA = s->parentA.get(), *tabB = s->parentB.get();
-    const uint32_t *bm_beg = (const uint32_t *)(s->m_dir + s->L.o_beg);
-    const uint32_t *bm_cnt = (const uint32_t *)(s->m_dir + s->L.o_cnt);
-    const uint16_t *c_key = (const uint16_t *)(s->m_dir + s->L.o_key);
-    const uint8_t *c_type = s->m_dir + s->L.o_type;
-    const uint32_t *c_card = (const uint32_t *)(s->m_dir + s->L.o_card);
-    const uint32_t *c_len = (const uint32_t *)(s->m_dir + s->L.o_len);
-    const uint64_t *c_off = (const uint64_t *)(s->m_dir + s->L.o_off);
+    const uint32_t *bm_beg = (const uint32_t *)(m_dir + s->L.o_beg);
+    const uint32_t *bm_cnt = (const uint32_t *)(m_dir + s->L.o_cnt);
+    const uint16_t *c_key = (const uint16_t *)(m_dir + s->L.o_key);
+    const uint8_t *c_type = m_dir + s->L.o_type;
+    const uint32_t *c_card = (const uint32_t *)(m_dir + s->L.o_card);
+    const uint32_t *c_len = (const uint32_t *)(m_dir + s->L.o_len);
+    const uint64_t *c_off = (const uint64_t *)(m_dir + s->L.o_off);
     const uint32_t beg = bm_beg[i], cnt = bm_cnt[i];
     roaring_bitmap_t *r = bitmap_alloc((int32_t)cnt);
     if (!r) return nullptr;
@@ -2107,19 +2124,15 @@ void pool_for(size_t n, unsigned T, size_t blk, const std::function<void(size_t)
 
 // A set packed for download: directory in bitmap order, mirrored in pinned memory; payload
 // contiguous in bitmap order with no slot slack (device), cut into chunks of whole bitmaps.
+// Every copy out of P must have landed before a Packed is destroyed.
 struct Packed {
-    rb200_set *P = nullptr;
+    SetPtr P;
     size_t nb = 0;
-    uint64_t *h_ob = nullptr;       // [payload offset (nb+1) | first container (nb+1)], pinned
+    PinBlock<uint64_t> ob;          // [payload offset (nb+1) | first container (nb+1)]
     std::vector<size_t> chunk_end;  // bitmap index closing each chunk
     uint64_t max_chunk = 0;         // payload bytes of the largest chunk
     uint64_t bytes = 0;             // directory + payload: what crosses PCIe
-    Packed() = default;
-    Packed(const Packed &) = delete;
-    ~Packed() {  // every copy out of P must have landed
-        set_delete(P);
-        pin_free(h_ob, 16 * (nb + 1));
-    }
+    const uint64_t *h_ob() const { return ob.get(); }
     size_t begin(size_t k) const { return k ? chunk_end[k - 1] : 0; }
 };
 
@@ -2160,34 +2173,31 @@ std::unique_ptr<Packed> pack_for_download(const rb200_set *s, size_t chunk_bitma
     bool ok = true;
     if (nb) {
         if (chunk_bitmaps == 0) chunk_bitmaps = 1024;
-        uint64_t *d_bytes = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
-                 *d_beg = (uint64_t *)dev_alloc(8 * (nb + 1));
-        uint32_t *d_cnt = (uint32_t *)dev_alloc(4 * nb);
-        pk->h_ob = (uint64_t *)pin_alloc(16 * (nb + 1));
-        ok = d_bytes && d_off && d_beg && d_cnt && pk->h_ob;
+        DevBlock<uint64_t> d_bytes(nb), d_off(nb + 1), d_beg(nb + 1);
+        DevBlock<uint32_t> d_cnt(nb);
+        ok = d_bytes && d_off && d_beg && d_cnt && pk->ob.reset(2 * (nb + 1));
         const int elide = (s->parentA ? 1 : 0) | (s->parentB ? 2 : 0);
+        uint64_t *h_off = pk->ob.get(), *h_beg = ok ? h_off + nb + 1 : nullptr;
         if (ok) {
-            launch_pack(s->view(), (uint32_t)nb, elide, d_bytes, d_cnt, d_off, d_beg, g.stream);
-            ok = cudaMemcpyAsync(pk->h_ob, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-                 cudaMemcpyAsync(pk->h_ob + nb + 1, d_beg, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+            launch_pack(s->view(), (uint32_t)nb, elide, d_bytes.get(), d_cnt.get(), d_off.get(), d_beg.get(), g.stream);
+            ok = cudaMemcpyAsync(h_off, d_off.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                 cudaMemcpyAsync(h_beg, d_beg.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
                  cudaStreamSynchronize(g.stream) == cudaSuccess;
         }
-        const uint64_t *h_off = pk->h_ob, *h_beg = h_off ? h_off + nb + 1 : nullptr;
         if (ok) {
             pk->P = set_new((uint32_t)nb, h_beg[nb], h_off[nb]);
             ok = pk->P != nullptr;
         }
         if (ok) {
-            rb200_set *P = pk->P;
+            rb200_set *P = pk->P.get();
             P->n_containers = h_beg[nb];
             P->slab_used = h_off[nb];
             P->h_flags = s->h_flags;
             P->parentA = s->parentA;
             P->parentB = s->parentB;
-            launch_pack_copy(s->view(), (uint32_t)nb, elide, d_off, d_beg, P->out(), g.stream);
-            P->m_dir = (uint8_t *)pin_alloc(P->L.total);
-            ok = P->m_dir != nullptr &&
-                 cudaMemcpyAsync(P->m_dir, P->d_dir, P->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+            launch_pack_copy(s->view(), (uint32_t)nb, elide, d_off.get(), d_beg.get(), P->out(), g.stream);
+            ok = P->m_dir.reset(P->L.total) &&
+                 cudaMemcpyAsync(P->m_dir.get(), P->d_dir.get(), P->L.total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
             const uint64_t CAP = (uint64_t)64 << 20;
             for (size_t p0 = 0, p1; p0 < nb; p0 = p1) {
                 p1 = p0 + 1;
@@ -2197,10 +2207,6 @@ std::unique_ptr<Packed> pack_for_download(const rb200_set *s, size_t chunk_bitma
             }
             pk->bytes = P->L.total + P->slab_used;
         }
-        dev_free(d_bytes, 8 * nb);
-        dev_free(d_off, 8 * (nb + 1));
-        dev_free(d_beg, 8 * (nb + 1));
-        dev_free(d_cnt, 4 * nb);
     }
     if (!ok) {
         cudaStreamSynchronize(g.stream);  // before ~Packed recycles what the copies write
@@ -2216,26 +2222,23 @@ std::unique_ptr<Packed> pack_for_download(const rb200_set *s, size_t chunk_bitma
 // (a batch result's pass-through containers can live in its operands' slabs), then the packed
 // payload copied to pinned memory.  build_bitmap() reads it.
 const rb200_set *ensure_mirror(rb200_set *s) {
-    if (s->mirror) return s->mirror;
+    if (s->mirror) return s->mirror.get();
     DlStats stats("download");
     std::unique_ptr<Packed> pk = pack_for_download(s, 0, stats);
     if (!pk) return nullptr;
-    rb200_set *P = pk->P;
-    P->m_slab = (uint8_t *)pin_alloc(P->slab_used);
-    bool ok = P->m_slab != nullptr;
+    rb200_set *P = pk->P.get();
+    bool ok = P->m_slab.reset(P->slab_used);
     if (ok && P->slab_used)
-        ok = cudaMemcpyAsync(P->m_slab, P->d_slab, P->slab_used, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = cudaMemcpyAsync(P->m_slab.get(), P->d_slab, P->slab_used, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
     ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // (also the directory copy of the pack)
     if (!ok) {
         t_err = "download: copy failed";
         return nullptr;
     }
-    pk->P = nullptr;
-    dev_free(P->d_dir, P->L.total);   // the copies have landed: only the pinned host copies are kept
-    P->d_dir = nullptr;
+    P->d_dir.reset();   // the copies have landed: only the pinned host copies are kept
     P->slab.reset();
     P->d_slab = P->d_base = nullptr;
-    s->mirror = P;
+    s->mirror = std::move(pk->P);
     stats.report();
     return P;
 }
@@ -2245,14 +2248,11 @@ const rb200_set *ensure_mirror(rb200_set *s) {
 // download_sets() and the background downloader use 4 slots: 2 stall one side or the other.
 class Ring {
    public:
-    explicit Ring(size_t slots) : buf_(slots, nullptr), ev_(slots, nullptr) {
+    explicit Ring(size_t slots) : buf_(slots), ev_(slots, nullptr) {
         for (auto &e : ev_) e = ev_get();
     }
     ~Ring() {  // nothing may be in flight
-        for (size_t k = 0; k < buf_.size(); k++) {
-            pin_free(buf_[k], bytes_);
-            ev_put(ev_[k]);
-        }
+        for (cudaEvent_t e : ev_) ev_put(e);
     }
     uint64_t capacity() const { return bytes_; }
     bool idle() const { return issued_ == waited_; }
@@ -2261,29 +2261,32 @@ class Ring {
     bool reserve(uint64_t bytes) {
         bytes = std::max<uint64_t>(bytes, 1);
         if (bytes <= bytes_) return true;
-        for (auto &b : buf_) { pin_free(b, bytes_); b = (uint8_t *)pin_alloc(bytes); }
-        bytes_ = bytes;
-        if (std::all_of(buf_.begin(), buf_.end(), [](uint8_t *b) { return b != nullptr; })) return true;
-        for (auto &b : buf_) { pin_free(b, bytes_); b = nullptr; }
+        for (auto &b : buf_) b.reset();
         bytes_ = 0;
-        return false;
+        for (auto &b : buf_)
+            if (!b.reset(bytes)) {
+                for (auto &c : buf_) c.reset();
+                return false;
+            }
+        bytes_ = bytes;
+        return true;
     }
     // Copy chunk k of pk into the next slot on `stream` (the ring must not be full()).
     bool enqueue(const Packed &pk, size_t k, cudaStream_t stream) {
         const size_t slot = issued_++ % buf_.size();
-        const uint64_t b0 = pk.h_ob[pk.begin(k)], b1 = pk.h_ob[pk.chunk_end[k]];
-        const bool ok = b1 == b0 || cudaMemcpyAsync(buf_[slot], pk.P->d_slab + b0, b1 - b0,
+        const uint64_t b0 = pk.h_ob()[pk.begin(k)], b1 = pk.h_ob()[pk.chunk_end[k]];
+        const bool ok = b1 == b0 || cudaMemcpyAsync(buf_[slot].get(), pk.P->d_slab + b0, b1 - b0,
                                                     cudaMemcpyDeviceToHost, stream) == cudaSuccess;
         return cudaEventRecord(ev_[slot], stream) == cudaSuccess && ok;
     }
     // Wait for the oldest copy in flight; its slot, or nullptr if the copy failed.
     const uint8_t *wait() {
         const size_t slot = waited_++ % buf_.size();
-        return cudaEventSynchronize(ev_[slot]) == cudaSuccess ? buf_[slot] : nullptr;
+        return cudaEventSynchronize(ev_[slot]) == cudaSuccess ? buf_[slot].get() : nullptr;
     }
 
    private:
-    std::vector<uint8_t *> buf_;
+    std::vector<PinBlock<uint8_t>> buf_;
     std::vector<cudaEvent_t> ev_;
     uint64_t bytes_ = 0;
     size_t issued_ = 0, waited_ = 0;
@@ -2302,13 +2305,13 @@ struct Sink {
 // one failed (its out[] slot is then null).
 bool materialise(const Packed &pk, size_t k, const uint8_t *buf, const Sink &sink) {
     const size_t p0 = pk.begin(k), p1 = pk.chunk_end[k], n = p1 - p0;
-    const uint64_t *off = pk.h_ob, *beg = pk.h_ob + pk.nb + 1;
+    const uint64_t *off = pk.h_ob(), *beg = off + pk.nb + 1;
     // threads scaled to the work of the chunk: waking every worker for a few hundred tiny bitmaps
     // costs more than it saves
     const uint64_t want = (off[p1] - off[p0] + 256 * (beg[p1] - beg[p0]) + 512 * n) / (128 << 10) + 1;
     std::atomic<int> failed(0);
     pool_for(n, (unsigned)std::min<uint64_t>(want, host_workers()), 8, [&](size_t i) {
-        roaring_bitmap_t *bm = build_bitmap(pk.P, p0 + i, buf, off[p0]);
+        roaring_bitmap_t *bm = build_bitmap(pk.P.get(), p0 + i, buf, off[p0]);
         if (!bm) failed = 1;
         if (sink.out) sink.out[i] = bm;
         else if (bm && sink.fn(sink.base + p0 + i, bm, sink.ctx) == 0) bitmap_free_host(bm);
@@ -2651,17 +2654,12 @@ static rb200_set *convert_impl(const rb200_set *S, int mode) {
     const uint64_t nc = S->n_containers;
     // mode 1 never grows a container by more than its 16-byte padding; mode 0 may expand runs
     const uint64_t bound = stored_bytes_total(S) + 16 * nc + (mode == 0 ? nc * (uint64_t)BITSET_BYTES : 0) + 512;
-    rb200_set *R = set_new(S->n_bitmaps, nc, bound);
+    SetPtr R = set_new(S->n_bitmaps, nc, bound);
     if (!R) return nullptr;
-    bool ok = stats_reset();
+    SyncCall call("run_optimize");
+    const bool ok = call.begin();
     launch_run_optimize(S->view(), S->n_bitmaps, nc, mode, R->out(), g.d_stats, g.stream);
-    ok = ok && stats_fetch();
-    cudaError_t e = cudaStreamSynchronize(g.stream);
-    if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
-        t_err = std::string("run_optimize: ") + cudaGetErrorString(e);
-        ok = false;
-    }
-    if (!ok) { set_delete(R); return nullptr; }
+    if (!call.finish(ok)) return nullptr;
     R->n_containers = nc;
     R->slab_used = g.h_stats->slab_cursor;
     R->h_flags = S->h_flags;
@@ -2670,63 +2668,49 @@ static rb200_set *convert_impl(const rb200_set *S, int mode) {
         R->h_bytes[b] = (uint64_t)R->h_cnt[b] * BITSET_BYTES;
         R->h_ebytes[b] = std::max<uint64_t>(R->h_bytes[b], S->h_ebytes[b]);
     }
-    return R;
+    return R.release();
 }
 
 // roaring_bitmap_to_uint32_array for every bitmap of a set: *vals (pinned host memory owned by the
 // library) holds all values; bitmap i = vals[off[i] .. off[i+1]).  Release with rb200_values_free.
 int rb200_set_to_uint32(const rb200_set_t *S, uint32_t **vals, uint64_t **off_out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
+    *vals = nullptr;
+    *off_out = nullptr;
     if (!ctx_init()) return -1;
     if (!resolve(S)) return -1;
     const size_t nb = S->n_bitmaps;
     const uint64_t nc = S->n_containers;
-    *vals = nullptr;
-    *off_out = (uint64_t *)malloc(8 * (nb + 1));
-    if (!*off_out) return -1;
-    (*off_out)[0] = 0;
-    if (nb == 0) return 0;
-    uint64_t *d_bv = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
-             *d_dummy = (uint64_t *)dev_alloc(8 * (nb + 1)), *d_cstart = (uint64_t *)dev_alloc(8 * nc);
-    uint32_t *d_zero = (uint32_t *)dev_alloc(4 * nb), *d_cbm = (uint32_t *)dev_alloc(4 * nc);
-    uint64_t *h_off = (uint64_t *)pin_alloc(8 * (nb + 1));
-    uint32_t *d_vals = nullptr, *h_vals = nullptr;
+    HostArrays out;
+    if (!out.alloc(nb, false)) return -1;
+    if (nb == 0) return out.hand_out(vals, off_out, nullptr);
+    DevBlock<uint64_t> d_bv(nb), d_off(nb + 1), d_dummy(nb + 1), d_cstart(nc);
+    DevBlock<uint32_t> d_zero(nb), d_cbm(nc), d_vals;
+    PinBlock<uint64_t> h_off(nb + 1);
+    SyncCall call;
     uint64_t total = 0;
     bool ok = d_bv && d_off && d_dummy && d_cstart && d_zero && d_cbm && h_off;
     if (ok) {
-        launch_values_measure(S->view(), (uint32_t)nb, d_bv, d_zero, d_cstart, d_cbm, g.stream);
-        launch_pack_scan(d_bv, d_zero, (uint32_t)nb, d_off, d_dummy, g.stream);
-        ok = cudaMemcpyAsync(h_off, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+        launch_values_measure(S->view(), (uint32_t)nb, d_bv.get(), d_zero.get(), d_cstart.get(), d_cbm.get(), g.stream);
+        launch_pack_scan(d_bv.get(), d_zero.get(), (uint32_t)nb, d_off.get(), d_dummy.get(), g.stream);
+        ok = cudaMemcpyAsync(h_off.get(), d_off.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;
     }
     if (ok) {
-        total = h_off[nb];
-        memcpy(*off_out, h_off, 8 * (nb + 1));
-        d_vals = (uint32_t *)dev_alloc(4 * total);
-        h_vals = (uint32_t *)pin_alloc(4 * total);
-        ok = d_vals && h_vals;
+        total = h_off.get()[nb];
+        memcpy(out.off, h_off.get(), 8 * (nb + 1));
+        ok = d_vals.reset(total) && out.blob.reset(4 * total);
     }
     if (ok) {
-        launch_values_write(S->view(), (uint32_t)nb, d_off, d_cstart, d_cbm, nc, d_vals, g.stream);
-        ok = cudaMemcpyAsync(h_vals, d_vals, 4 * total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess && cudaGetLastError() == cudaSuccess;
+        launch_values_write(S->view(), (uint32_t)nb, d_off.get(), d_cstart.get(), d_cbm.get(), nc, d_vals.get(), g.stream);
+        ok = cudaMemcpyAsync(out.blob.get(), d_vals.get(), 4 * total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok, false);
     }
-    dev_free(d_bv, 8 * nb);
-    dev_free(d_off, 8 * (nb + 1));
-    dev_free(d_dummy, 8 * (nb + 1));
-    dev_free(d_cstart, 8 * nc);
-    dev_free(d_zero, 4 * nb);
-    dev_free(d_cbm, 4 * nc);
-    dev_free(d_vals, 4 * total);
-    pin_free(h_off, 8 * (nb + 1));
     if (!ok) {
-        pin_free(h_vals, 4 * total);
         if (t_err.empty()) t_err = "set_to_uint32 failed";
         return -1;
     }
-    *vals = h_vals;
-    g_serialized_sizes[(uint8_t *)h_vals] = 4 * total;
-    return 0;
+    return out.hand_out(vals, off_out, nullptr);
 }
 
 void rb200_values_free(uint32_t *vals, uint64_t *off) { rb200_serialized_free((char *)vals, off, nullptr); }
@@ -2755,14 +2739,14 @@ static bool check_value_offsets(const uint64_t *off, size_t n, const char *what 
     return true;
 }
 
-// Segmented sort of src (n segments: h_off on the host, d_off on the device) into *sorted, a new device
+// Segmented sort of src (n segments: h_off on the host, d_off on the device) into `sorted`, a new device
 // buffer of h_off[n] values; the input stays as it was.  cub sorts fewer than 2^31 values per call, so
 // the segments go in chunks of that size; a segment too large for one call is sorted already (the
-// measure pass refuses it otherwise) and is copied.  d_temp / temp_bytes: the caller's scratch, grown here.
+// measure pass refuses it otherwise) and is copied.  temp: the caller's scratch, grown here.
 extern "C++" {
 template <typename T>
-static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d_off, size_t n, T **sorted,
-                          void *&d_temp, size_t &temp_bytes) {
+static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d_off, size_t n, DevBlock<T> &sorted,
+                          DevBlock<uint8_t> &temp) {
     struct Chunk { uint64_t s0, s1; bool copy; };
     std::vector<Chunk> chunks;
     const uint64_t LIM = (1ull << 31) - 1, N = h_off[n];
@@ -2785,30 +2769,107 @@ static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d
         sort_bytes = std::max(sort_bytes, b);
         max_seg = std::max(max_seg, c.s1 - c.s0);
     }
-    if (ok && sort_bytes > temp_bytes) {
-        dev_free(d_temp, temp_bytes);
-        temp_bytes = sort_bytes;
-        ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
-    }
-    const size_t rel_bytes = 4 * (max_seg + 1);
-    int *d_rel = nullptr;
-    ok = ok && (*sorted = (T *)dev_alloc(sizeof(T) * N)) && (d_rel = (int *)dev_alloc(rel_bytes));
+    if (ok && sort_bytes > temp.bytes()) ok = temp.reset(sort_bytes);
+    DevBlock<int> rel;   // stream-ordered reuse only
+    ok = ok && sorted.reset(N) && rel.reset(max_seg + 1);
     for (size_t k = 0; k < chunks.size() && ok; k++) {
         const Chunk &c = chunks[k];
         const uint64_t first = h_off[c.s0], items = h_off[c.s1] - first;
         if (!items) continue;
         if (c.copy) {
-            ok = cudaMemcpyAsync(*sorted + first, src + first, sizeof(T) * items, cudaMemcpyDeviceToDevice,
+            ok = cudaMemcpyAsync(sorted.get() + first, src + first, sizeof(T) * items, cudaMemcpyDeviceToDevice,
                                  g.stream) == cudaSuccess;
         } else {
-            size_t b = temp_bytes;
-            ok = build_sort_chunk(d_temp, &b, src, *sorted, d_off + c.s0, first, items, (uint32_t)(c.s1 - c.s0), d_rel,
-                                  g.stream);
+            size_t b = temp.bytes();
+            ok = build_sort_chunk(temp.get(), &b, src, sorted.get(), d_off + c.s0, first, items, (uint32_t)(c.s1 - c.s0),
+                                  rel.get(), g.stream);
         }
     }
-    dev_free(d_rel, rel_bytes);   // stream-ordered reuse only
     return ok;
 }
+
+// The first passes of the set builders (rb200_build.cu), the same for 32- and 64-bit values: the
+// offsets and host values go to the device, then the measure pass counts per tile the starts of the
+// containers (32-bit) or buckets (64-bit) and scans them, so the total is their count if every
+// bitmap's values are sorted.  Unsorted bitmaps are sorted by segment and measured again.
+template <typename V>
+struct BuildInput {
+    const char *what;         // the builder, in messages
+    size_t n;
+    uint64_t N, ntiles;
+    const uint64_t *h_off;    // checked host offsets; null: presorted device segments
+    const uint64_t *offs = nullptr;   // the offsets on the device
+    const V *src = nullptr;   // the values on the device, sorted once measure_sorted() returned true
+    DevBlock<uint64_t> d_off, tcnt, tbase;
+    DevBlock<V> vals, sorted;
+    DevBlock<uint32_t> flag;
+    DevBlock<uint8_t> temp;   // cub scratch, grown by grow_temp()
+    PinBlock<uint64_t> meta;  // [count | unsorted flags | two words of the caller's]
+
+    BuildInput(const char *what_, const uint64_t *h_off_, size_t n_, uint64_t N_)
+        : what(what_), n(n_), N(N_), ntiles(build_tile_count(N_)), h_off(h_off_) {}
+    bool grow_temp(size_t b) { return b <= temp.bytes() || temp.reset(b); }
+
+    // Offsets (h_off, or d_off_in already on the device) and values (h_vals from the host, or d_in
+    // on the device) in place; false: t_err says why.
+    bool load(const V *h_vals, const V *d_in, const uint64_t *d_off_in) {
+        if (ntiles >= (1ull << 31) - 1) { t_err = std::string(what) + ": too many values for one call"; return false; }
+        if (!d_off_in && !d_off.reset(n + 1)) return false;
+        if (h_vals && !vals.reset(N)) return false;
+        if (!tcnt.reset(ntiles + 1) || !tbase.reset(ntiles + 1) || !flag.reset(1) || !meta.reset(4)) return false;
+        offs = d_off_in ? d_off_in : d_off.get();
+        src = h_vals ? vals.get() : d_in;
+        if (!d_off_in && cudaMemcpyAsync(d_off.get(), h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
+            return false;
+        if (h_vals && N) {
+            H2DStager stage((uint8_t *)vals.get());
+            const bool ok = stage.ok && stage.put(h_vals, sizeof(V) * N) && stage.flush();
+            return cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
+        }
+        return true;
+    }
+
+    // launch(src) enqueues the measure kernel over the values; *count: containers (buckets).
+    template <typename Launch>
+    bool measure_sorted(Launch launch, uint64_t &count) {
+        uint64_t *h = meta.get();
+        auto measure = [&]() -> bool {
+            size_t b = 0;
+            if (!build_scan(nullptr, &b, tcnt.get(), tbase.get(), ntiles + 1, g.stream) || !grow_temp(b)) return false;
+            launch(src);
+            return build_scan(temp.get(), &b, tcnt.get(), tbase.get(), ntiles + 1, g.stream) &&
+                   cudaMemcpyAsync(h, tbase.get() + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                   cudaMemcpyAsync(h + 1, flag.get(), 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                   cudaStreamSynchronize(g.stream) == cudaSuccess;
+        };
+        h[1] = 0;
+        if (cudaMemsetAsync(flag.get(), 0, 4, g.stream) != cudaSuccess ||
+            cudaMemsetAsync(tcnt.get() + ntiles, 0, 8, g.stream) != cudaSuccess || !measure())
+            return false;
+        const uint32_t unsorted = (uint32_t)h[1];
+        if (unsorted && !h_off) {
+            t_err = "internal: presorted segments are not sorted";
+            return false;
+        }
+        if (unsorted & 2u) {
+            t_err = std::string(what) + ": a bitmap of 2^31 values or more is not sorted; pass it sorted";
+            return false;
+        }
+        if (unsorted) {
+            bool ok = sort_segments(src, h_off, d_off.get(), n, sorted, temp);
+            if (ok) {
+                src = sorted.get();
+                ok = measure();
+            }
+            if (!ok) {
+                if (t_err.empty()) t_err = std::string(what) + ": segmented sort failed";
+                return false;
+            }
+        }
+        count = h[0];
+        return true;
+    }
+};
 }  // extern "C++"
 
 // roaring_bitmap_of_ptr of every bitmap (rb200_build.cu).  Values come from the host (h_vals, staged
@@ -2817,127 +2878,52 @@ static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d
 // the 64-bit builder), which are never sorted again.
 static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in, const uint64_t *h_off, size_t n,
                                    const uint64_t *d_off_in = nullptr, uint64_t N_in = 0) {
-    const uint64_t N = h_off ? h_off[n] : N_in;
-    const uint64_t ntiles = build_tile_count(N);
-    if (ntiles >= (1ull << 31) - 1) { t_err = "set_from_uint32: too many values for one call"; return nullptr; }
-    uint64_t *d_off = d_off_in ? nullptr : (uint64_t *)dev_alloc(8 * (n + 1));
-    uint32_t *d_vals = h_vals ? (uint32_t *)dev_alloc(4 * N) : nullptr, *d_sorted = nullptr;
-    uint64_t *d_tcnt = (uint64_t *)dev_alloc(8 * (ntiles + 1)), *d_tbase = (uint64_t *)dev_alloc(8 * (ntiles + 1));
-    uint32_t *d_flag = (uint32_t *)dev_alloc(4);
-    uint64_t *h_meta = (uint64_t *)pin_alloc(16);
-    uint64_t *d_cpos = nullptr, *d_slot = nullptr;
-    void *d_temp = nullptr;
-    size_t temp_bytes = 0, scan_bytes = 0;
+    BuildInput<uint32_t> in("set_from_uint32", h_off, n, h_off ? h_off[n] : N_in);
+    const uint64_t N = in.N;
+    SetPtr s;
+    DevBlock<uint64_t> d_cpos, d_slot;
+    SyncCall call("set_from_uint32");
     uint64_t nc = 0;
-    rb200_set *s = nullptr;
-    bool ok = (d_off || d_off_in) && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
-              (d_off_in || cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess);
-    const uint64_t *offs = d_off_in ? d_off_in : d_off;
-    if (ok && h_vals && N) {
-        H2DStager stage((uint8_t *)d_vals);
-        ok = stage.ok && stage.put(h_vals, 4 * N) && stage.flush();
-        ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
-    }
-    const uint32_t *src = h_vals ? d_vals : d_in;
-    // container starts per tile, scanned; the total is the container count if the values are sorted
-    auto measure = [&]() -> bool {
-        size_t b = 0;
-        if (!build_scan(nullptr, &b, d_tcnt, d_tbase, ntiles + 1, g.stream)) return false;
-        if (b > temp_bytes) {
-            dev_free(d_temp, temp_bytes);
-            temp_bytes = b;
-            if (!(d_temp = dev_alloc(temp_bytes))) return false;
-        }
-        scan_bytes = b;
-        launch_build_measure(src, offs, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
-        return build_scan(d_temp, &scan_bytes, d_tcnt, d_tbase, ntiles + 1, g.stream) &&
-               cudaMemcpyAsync(h_meta, d_tbase + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-               cudaMemcpyAsync(h_meta + 1, d_flag, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-               cudaStreamSynchronize(g.stream) == cudaSuccess;
-    };
-    ok = ok && cudaMemsetAsync(d_flag, 0, 4, g.stream) == cudaSuccess &&
-         cudaMemsetAsync(d_tcnt + ntiles, 0, 8, g.stream) == cudaSuccess && measure();
-    const uint32_t unsorted = ok ? (uint32_t)h_meta[1] : 0u;
-    if (ok && unsorted && !h_off) {
-        t_err = "internal: presorted segments are not sorted";
-        ok = false;
-    }
-    if (ok && (unsorted & 2u)) {
-        t_err = "set_from_uint32: a bitmap of 2^31 values or more is not sorted; pass it sorted";
-        ok = false;
-    }
-    if (ok && unsorted) {
-        ok = sort_segments(src, h_off, d_off, n, &d_sorted, d_temp, temp_bytes);
-        if (ok) {
-            src = d_sorted;
-            ok = measure();
-        }
-        if (!ok && t_err.empty()) t_err = "set_from_uint32: segmented sort failed";
-    }
-    if (ok) {
-        nc = h_meta[0];
-        if (nc > 0xffffffffull) { t_err = "set_from_uint32: more than 2^32 - 1 containers"; ok = false; }
-    }
+    bool ok = in.load(h_vals, d_in, d_off_in) && in.measure_sorted([&](const uint32_t *src) {
+        launch_build_measure(src, in.offs, (uint32_t)n, N, in.tcnt.get(), in.flag.get(), g.stream);
+    }, nc);
+    if (ok && nc > 0xffffffffull) { t_err = "set_from_uint32: more than 2^32 - 1 containers"; ok = false; }
     // every container stores at most 2 bytes per input value (an array 2 d <= 2 count, a bitset needs
     // d > 4096, so 8192 < 2 count) plus its 16-byte padding
     if (ok) ok = (s = set_new((uint32_t)n, nc, 2 * N + 16 * nc + 16)) != nullptr;
     if (ok && nc) {
         size_t b = 0;
-        ok = (d_cpos = (uint64_t *)dev_alloc(8 * nc)) && (d_slot = (uint64_t *)dev_alloc(8 * nc)) &&
-             build_scan(nullptr, &b, d_slot, s->out().c_off, nc, g.stream);
-        if (ok && b > temp_bytes) {
-            dev_free(d_temp, temp_bytes);
-            temp_bytes = b;
-            ok = (d_temp = dev_alloc(temp_bytes)) != nullptr;
-        }
+        ok = d_cpos.reset(nc) && d_slot.reset(nc) && build_scan(nullptr, &b, d_slot.get(), s->out().c_off, nc, g.stream) &&
+             in.grow_temp(b);
         if (ok) {
-            launch_build_emit(src, offs, (uint32_t)n, N, d_tbase, s->out().c_key, d_cpos, g.stream);
-            launch_build_slots(d_cpos, nc, N, d_slot, g.stream);
-            b = temp_bytes;
-            ok = build_scan(d_temp, &b, d_slot, s->out().c_off, nc, g.stream);
+            launch_build_emit(in.src, in.offs, (uint32_t)n, N, in.tbase.get(), s->out().c_key, d_cpos.get(), g.stream);
+            launch_build_slots(d_cpos.get(), nc, N, d_slot.get(), g.stream);
+            b = in.temp.bytes();
+            ok = build_scan(in.temp.get(), &b, d_slot.get(), s->out().c_off, nc, g.stream);
         }
     }
     if (ok) {
-        ok = stats_reset();
+        ok = call.begin();
         if (n && !nc) ok = ok && cudaMemsetAsync(s->out().bm_cnt, 0, 4 * n, g.stream) == cudaSuccess &&
                            cudaMemsetAsync(s->out().bm_beg, 0, 4 * n, g.stream) == cudaSuccess;
-        if (nc) launch_build_bitmaps(offs, (uint32_t)n, d_cpos, nc, s->out().bm_beg, s->out().bm_cnt, g.stream);
-        launch_build_write(src, d_cpos, nc, N, s->out(), s->slab_cap, g.d_stats, g.stream);
+        if (nc) launch_build_bitmaps(in.offs, (uint32_t)n, d_cpos.get(), nc, s->out().bm_beg, s->out().bm_cnt, g.stream);
+        launch_build_write(in.src, d_cpos.get(), nc, N, s->out(), s->slab_cap, g.d_stats, g.stream);
         launch_bitmap_figures(s->out(), (uint32_t)n, g.d_stats, g.stream);
-        ok = ok && stats_fetch();
-        cudaError_t e = cudaStreamSynchronize(g.stream);
-        if (e != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
-            t_err = std::string("set_from_uint32: ") + cudaGetErrorString(e);
-            ok = false;
-        } else if (ok && g.h_stats->error) {
+        ok = call.finish(ok);
+        if (ok && g.h_stats->error) {
             t_err = "internal: result slab bound exceeded";
             ok = false;
         }
-    } else {
-        cudaStreamSynchronize(g.stream);
     }
-    if (ok) {
-        s->n_containers = nc;
-        s->slab_used = g.h_stats->slab_cursor;
-        s->portable_bytes = g.h_stats->payload_bytes;
-        s->mirrors_pending = n > 0;   // containers / bytes / effective bytes per bitmap: k_deser_bitmap_cards wrote them
-    }
-    dev_free(d_off, 8 * (n + 1));
-    dev_free(d_vals, 4 * N);
-    dev_free(d_sorted, 4 * N);
-    dev_free(d_tcnt, 8 * (ntiles + 1));
-    dev_free(d_tbase, 8 * (ntiles + 1));
-    dev_free(d_flag, 4);
-    dev_free(d_cpos, 8 * nc);
-    dev_free(d_slot, 8 * nc);
-    dev_free(d_temp, temp_bytes);
-    pin_free(h_meta, 16);
     if (!ok) {
         if (t_err.empty()) t_err = "set_from_uint32 failed";
-        set_delete(s);
         return nullptr;
     }
-    return s;
+    s->n_containers = nc;
+    s->slab_used = g.h_stats->slab_cursor;
+    s->portable_bytes = g.h_stats->payload_bytes;
+    s->mirrors_pending = n > 0;   // containers / bytes / effective bytes per bitmap: k_deser_bitmap_cards wrote them
+    return s.release();
 }
 
 rb200_set_t *rb200_set_from_uint32(const uint32_t *vals, const uint64_t *off, size_t n) {
@@ -2949,25 +2935,30 @@ rb200_set_t *rb200_set_from_uint32(const uint32_t *vals, const uint64_t *off, si
     return from_uint32_impl(vals ? vals : &none, nullptr, off, n);
 }
 
-rb200_set_t *rb200_set_from_uint32_device(const uint32_t *d_vals, const uint64_t *d_off, size_t n) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!check_bitmap_count(n)) return nullptr;
-    if (!d_off) { t_err = "set_from_uint32_device: offsets are NULL"; return nullptr; }
-    if (!ctx_init()) return nullptr;
-    // the offsets are checked on the host before any kernel reads values through them
-    uint64_t *h_off = (uint64_t *)pin_alloc(8 * (n + 1));
-    if (!h_off) return nullptr;
-    rb200_set *s = nullptr;
-    if (cudaMemcpyAsync(h_off, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
+// The offsets of a *_device builder, read back into h_off and checked on the host before any kernel
+// reads values through them.  `check` names the builder in the checks of the offsets, `entry` the
+// entry point in the others.
+static bool device_offsets(const uint64_t *d_off, const void *d_vals, size_t n, const char *check, const char *entry,
+                           PinBlock<uint64_t> &h_off) {
+    if (!check_bitmap_count(n, check)) return false;
+    if (!d_off) { t_err = std::string(entry) + ": offsets are NULL"; return false; }
+    if (!ctx_init() || !h_off.reset(n + 1)) return false;
+    if (cudaMemcpyAsync(h_off.get(), d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
         cudaStreamSynchronize(g.stream) != cudaSuccess) {
         (void)cudaGetLastError();
-        t_err = "set_from_uint32_device: offsets are not readable device memory of the library's device";
-    } else if (check_value_offsets(h_off, n)) {
-        if (!d_vals && h_off[n]) t_err = "set_from_uint32_device: values are NULL";
-        else s = from_uint32_impl(nullptr, d_vals, h_off, n);
+        t_err = std::string(entry) + ": offsets are not readable device memory of the library's device";
+        return false;
     }
-    pin_free(h_off, 8 * (n + 1));
-    return s;
+    if (!check_value_offsets(h_off.get(), n, check)) return false;
+    if (!d_vals && h_off.get()[n]) { t_err = std::string(entry) + ": values are NULL"; return false; }
+    return true;
+}
+
+rb200_set_t *rb200_set_from_uint32_device(const uint32_t *d_vals, const uint64_t *d_off, size_t n) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    PinBlock<uint64_t> h_off;
+    if (!device_offsets(d_off, d_vals, n, "set_from_uint32", "set_from_uint32_device", h_off)) return nullptr;
+    return from_uint32_impl(nullptr, d_vals, h_off.get(), n);
 }
 
 // Device-side portable serialization of every bitmap of a set + one D2H copy.
@@ -2985,84 +2976,61 @@ int rb200_set_serialize_frozen(const rb200_set_t *s, char **buf, uint64_t **off_
     return serialize_impl(s, buf, off_out, len_out, true);
 }
 static int serialize_impl(const rb200_set *s, char **buf, uint64_t **off_out, uint64_t **len_out, bool frozen) {
+    *buf = nullptr;
+    *off_out = *len_out = nullptr;
     if (!ctx_init()) return -1;
     if (!resolve(s)) return -1;
     if (reject_lazy(s, "serialize")) return -1;
     const size_t nb = s->n_bitmaps;
-    *buf = nullptr;
-    *off_out = (uint64_t *)malloc(8 * (nb + 1));
-    *len_out = (uint64_t *)malloc(8 * (nb + 1));
-    if (!*off_out || !*len_out) return -1;
-    (*off_out)[0] = 0;
-    if (nb == 0) return 0;
-    uint64_t *d_sz = (uint64_t *)dev_alloc(8 * nb), *d_off = (uint64_t *)dev_alloc(8 * (nb + 1)),
-             *d_dummy = (uint64_t *)dev_alloc(8 * (nb + 1));
-    uint32_t *d_exact = (uint32_t *)dev_alloc(4 * nb), *d_hasrun = (uint32_t *)dev_alloc(4 * nb);
-    uint8_t *h_meta = (uint8_t *)pin_alloc(8 * (nb + 1) + 4 * nb);
-    uint8_t *d_blob = nullptr, *h_blob = nullptr;
+    HostArrays out;
+    if (!out.alloc(nb, true)) return -1;
+    if (nb == 0) return out.hand_out(buf, off_out, len_out);
+    DevBlock<uint64_t> d_sz(nb), d_off(nb + 1), d_dummy(nb + 1);
+    DevBlock<uint32_t> d_exact(nb), d_hasrun(nb);
+    DevBlock<uint8_t> d_blob;
+    PinBlock<uint8_t> h_meta(8 * (nb + 1) + 4 * nb);
+    SyncCall call;
     uint64_t total = 0;
     bool ok = d_sz && d_off && d_dummy && d_exact && d_hasrun && h_meta;
     if (ok) {
         const SetView v = s->view();
-        if (frozen) launch_frozen_measure(v, (uint32_t)nb, d_sz, d_exact, d_hasrun, g.stream);
-        else launch_serialize_measure(v, (uint32_t)nb, d_sz, d_exact, d_hasrun, g.stream);
-        launch_pack_scan(d_sz, d_hasrun, (uint32_t)nb, d_off, d_dummy, g.stream);
-        ok = cudaMemcpyAsync(h_meta, d_off, 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaMemcpyAsync(h_meta + 8 * (nb + 1), d_exact, 4 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+        if (frozen) launch_frozen_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
+        else launch_serialize_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
+        launch_pack_scan(d_sz.get(), d_hasrun.get(), (uint32_t)nb, d_off.get(), d_dummy.get(), g.stream);
+        ok = cudaMemcpyAsync(h_meta.get(), d_off.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+             cudaMemcpyAsync(h_meta.get() + 8 * (nb + 1), d_exact.get(), 4 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;
     }
     if (ok) {
-        const uint64_t *h_off = (const uint64_t *)h_meta;
-        const uint32_t *h_exact = (const uint32_t *)(h_meta + 8 * (nb + 1));
+        const uint64_t *h_off = (const uint64_t *)h_meta.get();
+        const uint32_t *h_exact = (const uint32_t *)(h_meta.get() + 8 * (nb + 1));
         total = h_off[nb];
-        for (size_t i = 0; i < nb; i++) { (*off_out)[i] = h_off[i]; (*len_out)[i] = h_exact[i]; }
-        (*off_out)[nb] = total;
-        d_blob = (uint8_t *)dev_alloc(total);
-        h_blob = (uint8_t *)pin_alloc(total);
-        ok = d_blob && h_blob;
+        for (size_t i = 0; i < nb; i++) { out.off[i] = h_off[i]; out.len[i] = h_exact[i]; }
+        out.off[nb] = total;
+        ok = d_blob.reset(total) && out.blob.reset(total);
     }
     if (ok) {
         if (frozen) {
-            uint64_t *d_cdst = (uint64_t *)dev_alloc(8 * (s->n_containers ? s->n_containers : 1));
-            ok = d_cdst != nullptr;
-            if (ok) launch_frozen_write(s->view(), (uint32_t)nb, s->n_containers, d_off, d_blob, d_cdst, g.stream);
-            dev_free(d_cdst, 8 * (s->n_containers ? s->n_containers : 1));  // stream-ordered reuse only
+            DevBlock<uint64_t> d_cdst(s->n_containers);   // released at once: stream-ordered reuse only
+            ok = (bool)d_cdst;
+            if (ok) launch_frozen_write(s->view(), (uint32_t)nb, s->n_containers, d_off.get(), d_blob.get(), d_cdst.get(), g.stream);
         } else {
-            launch_serialize_write(s->view(), (uint32_t)nb, d_off, d_hasrun, d_blob, g.stream);
+            launch_serialize_write(s->view(), (uint32_t)nb, d_off.get(), d_hasrun.get(), d_blob.get(), g.stream);
         }
-        ok = cudaMemcpyAsync(h_blob, d_blob, total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess && cudaGetLastError() == cudaSuccess;
+        ok = ok && cudaMemcpyAsync(out.blob.get(), d_blob.get(), total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok, false);
     }
     g.last_download_bytes = total;
-    dev_free(d_sz, 8 * nb);
-    dev_free(d_off, 8 * (nb + 1));
-    dev_free(d_dummy, 8 * (nb + 1));
-    dev_free(d_exact, 4 * nb);
-    dev_free(d_hasrun, 4 * nb);
-    dev_free(d_blob, total);
-    pin_free(h_meta, 8 * (nb + 1) + 4 * nb);
     if (!ok) {
-        pin_free(h_blob, total);
-        free(*off_out);
-        free(*len_out);
-        *off_out = *len_out = nullptr;
         if (t_err.empty()) t_err = "set_serialize failed";
         return -1;
     }
-    *buf = (char *)h_blob;
-    g_serialized_sizes[h_blob] = total;
-    return 0;
+    return out.hand_out(buf, off_out, len_out);
 }
 
 void rb200_serialized_free(char *buf, uint64_t *off, uint64_t *len) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (buf) {
-        auto it = g_serialized_sizes.find((uint8_t *)buf);
-        if (it != g_serialized_sizes.end()) {
-            pin_free(buf, it->second);
-            g_serialized_sizes.erase(it);
-        }
-    }
+    if (buf) g_serialized.erase((uint8_t *)buf);
     free(off);
     free(len);
 }
@@ -3084,17 +3052,11 @@ int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_
         ia[p] = (uint32_t)p;
         ib[p] = (uint32_t)(np + p);
     }
-    rb200_set *S = rb200_set_upload(all.data(), all.size());
+    SetPtr S(rb200_set_upload(all.data(), all.size()));
     if (!S) return -1;
-    rb200_set_bind_host(S, 1);  // the inputs outlive this call
-    rb200_set *R = batch_op_impl(op, S, S, ia.data(), ib.data(), np);
-    int rc = -1;
-    if (R) {
-        rc = rb200_set_download_all(R, out);
-        set_delete(R);
-    }
-    set_delete(S);
-    return rc;
+    rb200_set_bind_host(S.get(), 1);  // the inputs outlive this call
+    SetPtr R(batch_op_impl(op, S.get(), S.get(), ia.data(), ib.data(), np));
+    return R ? rb200_set_download_all(R.get(), out) : -1;
 }
 
 }  // extern "C"
@@ -3248,16 +3210,10 @@ roaring_bitmap_t *roaring_bitmap_andnot(const roaring_bitmap_t *r1, const roarin
 
 roaring_bitmap_t *roaring_bitmap_or_many(size_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    rb200_set *S = rb200_set_upload(rs, number);
+    SetPtr S(rb200_set_upload(rs, number));
     if (!S) return nullptr;
-    rb200_set *R = rb200_or_many(S, nullptr, number);
-    roaring_bitmap_t *out = nullptr;
-    if (R) {
-        out = rb200_set_download(R, 0);
-        set_delete(R);
-    }
-    set_delete(S);
-    return out;
+    SetPtr R(rb200_or_many(S.get(), nullptr, number));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 
 // In-place twins (src/roaring.c:812 and_inplace, :1063 or_inplace, :1200 xor_inplace, :1342
@@ -3274,14 +3230,12 @@ static void dropin_inplace(int op, roaring_bitmap_t *x1, const roaring_bitmap_t 
         if (f < 0) { dropin_failed("roaring_bitmap_*_inplace"); return; }
     }
     const roaring_bitmap_t *both[2] = {x1, x2};
-    rb200_set *S = rb200_set_upload(both, 2);
+    SetPtr S(rb200_set_upload(both, 2));
     if (!S) { dropin_failed("roaring_bitmap_*_inplace"); return; }
-    rb200_set_bind_host(S, 1);
+    rb200_set_bind_host(S.get(), 1);
     const uint32_t ia = 0, ib = 1;
-    rb200_set *R = batch_op_impl(op, S, S, &ia, &ib, 1, rules);
-    roaring_bitmap_t *out = R ? rb200_set_download(R, 0) : nullptr;
-    set_delete(R);
-    set_delete(S);
+    roaring_bitmap_t *out = nullptr;
+    if (SetPtr R{batch_op_impl(op, S.get(), S.get(), &ia, &ib, 1, rules)}) out = rb200_set_download(R.get(), 0);
     if (!out) { dropin_failed("roaring_bitmap_*_inplace"); return; }  // x1 is left untouched
     swap_into(x1, out);
 }
@@ -3306,27 +3260,20 @@ void roaring_bitmap_andnot_inplace(roaring_bitmap_t *x1, const roaring_bitmap_t 
 
 roaring_bitmap_t *roaring_bitmap_xor_many(size_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    rb200_set *S = rb200_set_upload(rs, number);
+    SetPtr S(rb200_set_upload(rs, number));
     if (!S) return nullptr;
-    rb200_set *R = rb200_xor_many(S, nullptr, number);
-    roaring_bitmap_t *out = nullptr;
-    if (R) {
-        out = rb200_set_download(R, 0);
-        set_delete(R);
-    }
-    set_delete(S);
-    return out;
+    SetPtr R(rb200_xor_many(S.get(), nullptr, number));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 
 uint64_t roaring_bitmap_and_cardinality(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const roaring_bitmap_t *both[2] = {r1, r2};
-    rb200_set *S = rb200_set_upload(both, 2);
+    SetPtr S(rb200_set_upload(both, 2));
     if (!S) return UINT64_MAX;
     const uint32_t ia = 0, ib = 1;
     uint64_t out = UINT64_MAX;
-    if (rb200_batch_and_cardinality(S, S, &ia, &ib, 1, &out) != 0) out = UINT64_MAX;
-    set_delete(S);
+    if (rb200_batch_and_cardinality(S.get(), S.get(), &ia, &ib, 1, &out) != 0) out = UINT64_MAX;
     return out;
 }
 
@@ -3379,12 +3326,11 @@ int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint
 static int dropin_relation(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const roaring_bitmap_t *both[2] = {r1, r2};
-    rb200_set *S = rb200_set_upload(both, 2);
+    SetPtr S(rb200_set_upload(both, 2));
     if (!S) { dropin_failed("roaring_bitmap_equals / is_subset / is_strict_subset"); return -1; }
     const uint32_t ia = 0, ib = 1;
     uint8_t out = 0;
-    const int rc = rb200_batch_relations(S, S, &ia, &ib, 1, &out);
-    set_delete(S);
+    const int rc = rb200_batch_relations(S.get(), S.get(), &ia, &ib, 1, &out);
     if (rc != 0) dropin_failed("roaring_bitmap_equals / is_subset / is_strict_subset");
     return rc != 0 ? -1 : out;
 }
@@ -3447,23 +3393,18 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     }
     const char *bp = (const char *)blob.data();
     const size_t bl = blob.size();
-    rb200_set *Rg = upload_blobs_impl(&bp, &bl, 1, false);
+    SetPtr Rg(upload_blobs_impl(&bp, &bl, 1, false));
     if (!Rg) return nullptr;
-    rb200_set *R = batch_op_impl(OP_XOR, S, Rg, ia.data(), ib.data(), n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
-    set_delete(Rg);
-    return R;
+    return batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
 }
 roaring_bitmap_t *roaring_bitmap_flip(const roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const roaring_bitmap_t *one[1] = {r1};
-    rb200_set *S = rb200_set_upload(one, 1);
+    SetPtr S(rb200_set_upload(one, 1));
     if (!S) return nullptr;
-    rb200_set_bind_host(S, 1);
-    rb200_set *R = rb200_batch_flip(S, nullptr, 1, range_start, range_end);
-    roaring_bitmap_t *out = R ? rb200_set_download(R, 0) : nullptr;
-    set_delete(R);
-    set_delete(S);
-    return out;
+    rb200_set_bind_host(S.get(), 1);
+    SetPtr R(rb200_batch_flip(S.get(), nullptr, 1, range_start, range_end));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 void roaring_bitmap_flip_inplace(roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {
     if (range_start >= range_end || range_start > (uint64_t)UINT32_MAX + 1) return;  // roaring.c:2353
@@ -3488,15 +3429,15 @@ void roaring_bitmap_flip_inplace(roaring_bitmap_t *r1, uint64_t range_start, uin
 // serialized, as the reference never keeps an empty container.
 }  // extern "C"
 struct rb200_set64 {
-    rb200_set *inner = nullptr;
+    SetPtr inner;
     uint32_t n = 0, nbuckets = 0;   // 64-bit bitmaps; inner bitmaps, the sentinel included
-    uint32_t *h_dir = nullptr;      // pinned host mirror: [b_beg (n) | b_cnt (n) | high (nbuckets)]
-    uint32_t *d_dir = nullptr;      // the same in device memory (copied there when a kernel first needs it)
+    PinBlock<uint32_t> h_dir;       // host mirror: [b_beg (n) | b_cnt (n) | high (nbuckets)]
+    DevBlock<uint32_t> d_dir;       // the same in device memory (copied there when a kernel first needs it)
     bool dir_on_device = false;
     size_t dir_bytes = 0;
-    const uint32_t *b_beg() const { return h_dir; }
-    const uint32_t *b_cnt() const { return h_dir + n; }
-    const uint32_t *high() const { return h_dir + 2 * (size_t)n; }
+    const uint32_t *b_beg() const { return h_dir.get(); }
+    const uint32_t *b_cnt() const { return h_dir.get() + n; }
+    const uint32_t *high() const { return h_dir.get() + 2 * (size_t)n; }
 };
 extern "C" {
 namespace {
@@ -3563,25 +3504,15 @@ const char *parse_r64(const char *buf, size_t len, std::vector<R64Bucket> &out) 
     return nullptr;
 }
 
-void set64_delete(rb200_set64 *s) {
-    if (!s) return;
-    set_delete(s->inner);
-    pin_free(s->h_dir, s->dir_bytes);
-    dev_free(s->d_dir, s->dir_bytes);
-    delete s;
-}
+void set64_delete(rb200_set64 *s) { delete s; }   // the inner set and both directories go back with it
+void Set64Free::operator()(rb200_set64 *s) const { set64_delete(s); }
 // A set of n 64-bit bitmaps over nbuckets inner bitmaps; the caller fills h_dir (or d_dir).
-rb200_set64 *set64_new(uint32_t n, uint32_t nbuckets) {
-    rb200_set64 *s = new rb200_set64();
+Set64Ptr set64_new(uint32_t n, uint32_t nbuckets) {
+    Set64Ptr s(new rb200_set64());
     s->n = n;
     s->nbuckets = nbuckets;
     s->dir_bytes = 4 * (2 * (size_t)n + nbuckets);
-    s->h_dir = (uint32_t *)pin_alloc(s->dir_bytes);
-    s->d_dir = (uint32_t *)dev_alloc(s->dir_bytes);
-    if (!s->h_dir || !s->d_dir) {
-        set64_delete(s);
-        return nullptr;
-    }
+    if (!s->h_dir.reset(2 * (size_t)n + nbuckets) || !s->d_dir.reset(2 * (size_t)n + nbuckets)) return nullptr;
     return s;
 }
 // The device copy of the directory, for the serialization kernels; a set that is only an operand
@@ -3590,7 +3521,7 @@ rb200_set64 *set64_new(uint32_t n, uint32_t nbuckets) {
 bool set64_dir_on_device(const rb200_set64 *cs) {
     rb200_set64 *s = const_cast<rb200_set64 *>(cs);
     if (s->dir_on_device) return true;
-    if (cudaMemcpyAsync(s->d_dir, s->h_dir, s->dir_bytes, cudaMemcpyHostToDevice, g.stream) != cudaSuccess) {
+    if (cudaMemcpyAsync(s->d_dir.get(), s->h_dir.get(), s->dir_bytes, cudaMemcpyHostToDevice, g.stream) != cudaSuccess) {
         t_err = "set64: directory upload failed";
         return false;
     }
@@ -3625,20 +3556,16 @@ rb200_set64 *set64_upload_impl(const char *const *bufs, const size_t *lens, size
     blens.push_back(8);
     highs.push_back(0);
     if (!ctx_init()) return nullptr;
-    rb200_set64 *s = set64_new((uint32_t)n, (uint32_t)ptrs.size());
+    Set64Ptr s = set64_new((uint32_t)n, (uint32_t)ptrs.size());
     if (!s) return nullptr;
-    uint32_t *beg = s->h_dir, *bc = s->h_dir + n;
+    uint32_t *beg = s->h_dir.get(), *bc = beg + n;
     for (size_t i = 0, b = 0; i < n; b += cnt[i], i++) {
         beg[i] = (uint32_t)b;
         bc[i] = cnt[i];
     }
-    memcpy(s->h_dir + 2 * n, highs.data(), 4 * highs.size());
-    s->inner = upload_blobs_impl(ptrs.data(), blens.data(), ptrs.size(), false);
-    if (!s->inner) {
-        set64_delete(s);
-        return nullptr;
-    }
-    return s;
+    memcpy(beg + 2 * n, highs.data(), 4 * highs.size());
+    s->inner.reset(upload_blobs_impl(ptrs.data(), blens.data(), ptrs.size(), false));
+    return s->inner ? s.release() : nullptr;
 }
 
 // Bucket pairs of result[p] = A[ia[p]] op B[ib[p]] from the host mirrors: the two high-32 lists
@@ -3647,7 +3574,7 @@ rb200_set64 *set64_upload_impl(const char *const *bufs, const size_t *lens, size
 struct Plan64 { std::vector<uint32_t> pa, pb, high, cnt; };
 bool plan64(int op, const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia, const uint32_t *ib, size_t np,
             Plan64 &P) {
-    if (!ensure_mirrors(A->inner) || !ensure_mirrors(B->inner)) return false;
+    if (!ensure_mirrors(A->inner.get()) || !ensure_mirrors(B->inner.get())) return false;
     const uint32_t *ca = A->inner->h_cnt.data(), *cb = B->inner->h_cnt.data();
     const uint32_t *ha = A->high(), *hb = B->high();
     const uint32_t EA = A->nbuckets - 1, EB = B->nbuckets - 1;
@@ -3692,19 +3619,16 @@ rb200_set64 *batch_op64_impl(int op, const rb200_set64 *A, const rb200_set64 *B,
     P.pa.push_back(A->nbuckets - 1);   // (sentinel, sentinel): the result's own sentinel
     P.pb.push_back(B->nbuckets - 1);
     P.high.push_back(0);
-    rb200_set64 *R = set64_new((uint32_t)np, (uint32_t)P.pa.size());
+    Set64Ptr R = set64_new((uint32_t)np, (uint32_t)P.pa.size());
     if (!R) return nullptr;
+    uint32_t *dir = R->h_dir.get();
     for (size_t p = 0, b = 0; p < np; b += P.cnt[p], p++) {
-        R->h_dir[p] = (uint32_t)b;
-        R->h_dir[np + p] = P.cnt[p];
+        dir[p] = (uint32_t)b;
+        dir[np + p] = P.cnt[p];
     }
-    memcpy(R->h_dir + 2 * np, P.high.data(), 4 * P.high.size());
-    R->inner = batch_op_impl(op, A->inner, B->inner, P.pa.data(), P.pb.data(), P.pa.size());
-    if (!R->inner) {
-        set64_delete(R);
-        return nullptr;
-    }
-    return R;
+    memcpy(dir + 2 * np, P.high.data(), 4 * P.high.size());
+    R->inner.reset(batch_op_impl(op, A->inner.get(), B->inner.get(), P.pa.data(), P.pb.data(), P.pa.size()));
+    return R->inner ? R.release() : nullptr;
 }
 
 int and_cardinality64_impl(const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia, const uint32_t *ib,
@@ -3714,7 +3638,8 @@ int and_cardinality64_impl(const rb200_set64 *A, const rb200_set64 *B, const uin
     Plan64 P;
     if (!plan64(OP_AND, A, B, ia, ib, np, P)) return -1;
     std::vector<uint64_t> c(P.pa.size());
-    if (!P.pa.empty() && rb200_batch_and_cardinality(A->inner, B->inner, P.pa.data(), P.pb.data(), P.pa.size(), c.data()) != 0)
+    if (!P.pa.empty() &&
+        rb200_batch_and_cardinality(A->inner.get(), B->inner.get(), P.pa.data(), P.pb.data(), P.pa.size(), c.data()) != 0)
         return -1;
     for (size_t p = 0, q = 0; p < np; p++) {
         uint64_t sum = 0;
@@ -3730,176 +3655,97 @@ int and_cardinality64_impl(const rb200_set64 *A, const rb200_set64 *B, const uin
 // the buckets themselves (k_ser_write) into one buffer that leaves in one D2H.  Blob starts are
 // 16-byte aligned; blob i = *buf + (*off)[i], (*len)[i] bytes.
 int serialize64_impl(const rb200_set64 *s, char **buf, uint64_t **off_out, uint64_t **len_out) {
-    if (!ctx_init()) return -1;
-    if (!resolve(s->inner)) return -1;
-    const size_t n = s->n, nb = s->nbuckets;
     *buf = nullptr;
-    *off_out = (uint64_t *)malloc(8 * (n + 1));
-    *len_out = (uint64_t *)malloc(8 * (n + 1));
-    if (!*off_out || !*len_out) {
-        free(*off_out);
-        free(*len_out);
-        *off_out = *len_out = nullptr;
+    *off_out = *len_out = nullptr;
+    if (!ctx_init()) return -1;
+    if (!resolve(s->inner.get())) return -1;
+    const size_t n = s->n, nb = s->nbuckets;
+    HostArrays out;
+    if (!out.alloc(n, true)) {
         t_err = "set64_serialize: host allocation failed";
         return -1;
     }
-    (*off_out)[0] = 0;
-    if (n == 0) return 0;
-    const uint32_t *d_beg = s->d_dir, *d_cnt = s->d_dir + n, *d_high = s->d_dir + 2 * n;
-    uint64_t *d_sz = (uint64_t *)dev_alloc(8 * nb), *d_boff = (uint64_t *)dev_alloc(8 * nb);
-    uint32_t *d_exact = (uint32_t *)dev_alloc(4 * nb), *d_hasrun = (uint32_t *)dev_alloc(4 * nb);
-    uint64_t *d_s16 = (uint64_t *)dev_alloc(8 * n), *d_e64 = (uint64_t *)dev_alloc(8 * n),
-             *d_off = (uint64_t *)dev_alloc(8 * (n + 1)), *d_dummy = (uint64_t *)dev_alloc(8 * (n + 1));
-    uint64_t *h_meta = (uint64_t *)pin_alloc(8 * (2 * n + 1));
-    uint8_t *d_blob = nullptr, *h_blob = nullptr;
+    if (n == 0) return out.hand_out(buf, off_out, len_out);
+    const uint32_t *d_beg = s->d_dir.get(), *d_cnt = d_beg + n, *d_high = d_beg + 2 * n;
+    DevBlock<uint64_t> d_sz(nb), d_boff(nb), d_s16(n), d_e64(n), d_off(n + 1), d_dummy(n + 1);
+    DevBlock<uint32_t> d_exact(nb), d_hasrun(nb);
+    DevBlock<uint8_t> d_blob;
+    PinBlock<uint64_t> h_meta(2 * n + 1);
+    SyncCall call;
     uint64_t total = 0;
     const SetView v = s->inner->view();
     bool ok = d_sz && d_boff && d_exact && d_hasrun && d_s16 && d_e64 && d_off && d_dummy && h_meta &&
               set64_dir_on_device(s);
     if (ok) {
-        launch_serialize_measure(v, (uint32_t)nb, d_sz, d_exact, d_hasrun, g.stream);
-        launch_r64_ser_sizes(d_beg, d_cnt, (uint32_t)n, v.bm_cnt, d_exact, d_s16, d_e64, g.stream);
-        launch_pack_scan(d_s16, d_cnt, (uint32_t)n, d_off, d_dummy, g.stream);
-        ok = cudaMemcpyAsync(h_meta, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaMemcpyAsync(h_meta + n + 1, d_e64, 8 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+        launch_serialize_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
+        launch_r64_ser_sizes(d_beg, d_cnt, (uint32_t)n, v.bm_cnt, d_exact.get(), d_s16.get(), d_e64.get(), g.stream);
+        launch_pack_scan(d_s16.get(), d_cnt, (uint32_t)n, d_off.get(), d_dummy.get(), g.stream);
+        ok = cudaMemcpyAsync(h_meta.get(), d_off.get(), 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+             cudaMemcpyAsync(h_meta.get() + n + 1, d_e64.get(), 8 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;
     }
     if (ok) {
-        total = h_meta[n];
-        memcpy(*off_out, h_meta, 8 * (n + 1));
-        memcpy(*len_out, h_meta + n + 1, 8 * n);
-        d_blob = (uint8_t *)dev_alloc(total + 16);   // + the scratch empty buckets write to
-        h_blob = (uint8_t *)pin_alloc(total);
-        ok = d_blob && h_blob;
+        total = h_meta.get()[n];
+        memcpy(out.off, h_meta.get(), 8 * (n + 1));
+        memcpy(out.len, h_meta.get() + n + 1, 8 * n);
+        ok = d_blob.reset(total + 16) && out.blob.reset(total);   // + the scratch empty buckets write to
     }
     if (ok) {
-        launch_r64_ser_layout(d_beg, d_cnt, d_high, (uint32_t)n, (uint32_t)nb, v.bm_cnt, d_exact, d_off, d_boff,
-                              d_blob, g.stream);
-        launch_serialize_write(v, (uint32_t)nb, d_boff, d_hasrun, d_blob, g.stream);
-        ok = cudaMemcpyAsync(h_blob, d_blob, total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess && cudaGetLastError() == cudaSuccess;
+        launch_r64_ser_layout(d_beg, d_cnt, d_high, (uint32_t)n, (uint32_t)nb, v.bm_cnt, d_exact.get(), d_off.get(),
+                              d_boff.get(), d_blob.get(), g.stream);
+        launch_serialize_write(v, (uint32_t)nb, d_boff.get(), d_hasrun.get(), d_blob.get(), g.stream);
+        ok = cudaMemcpyAsync(out.blob.get(), d_blob.get(), total, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok, false);
     }
     g.last_download_bytes = total;
-    dev_free(d_sz, 8 * nb);
-    dev_free(d_boff, 8 * nb);
-    dev_free(d_exact, 4 * nb);
-    dev_free(d_hasrun, 4 * nb);
-    dev_free(d_s16, 8 * n);
-    dev_free(d_e64, 8 * n);
-    dev_free(d_off, 8 * (n + 1));
-    dev_free(d_dummy, 8 * (n + 1));
-    dev_free(d_blob, total + 16);
-    pin_free(h_meta, 8 * (2 * n + 1));
     if (!ok) {
-        pin_free(h_blob, total);
-        free(*off_out);
-        free(*len_out);
-        *off_out = *len_out = nullptr;
         if (t_err.empty()) t_err = "set64_serialize failed";
         return -1;
     }
-    *buf = (char *)h_blob;
-    g_serialized_sizes[h_blob] = total;
-    return 0;
+    return out.hand_out(buf, off_out, len_out);
 }
 
 // roaring64_bitmap_of_ptr of every bitmap (rb200_build.cu): values from the host (staged through
 // pinned chunks) or the device (read in place); h_off: checked host offsets.
 rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, const uint64_t *h_off, size_t n) {
-    const uint64_t N = h_off[n];
-    const uint64_t ntiles = build_tile_count(N);
-    if (ntiles >= (1ull << 31) - 1) { t_err = "set64_from_uint64: too many values for one call"; return nullptr; }
-    uint64_t *d_off = (uint64_t *)dev_alloc(8 * (n + 1));
-    uint64_t *d_vals = h_vals ? (uint64_t *)dev_alloc(8 * N) : nullptr, *d_sorted = nullptr;
-    uint64_t *d_tcnt = (uint64_t *)dev_alloc(8 * (ntiles + 1)), *d_tbase = (uint64_t *)dev_alloc(8 * (ntiles + 1));
-    uint32_t *d_flag = (uint32_t *)dev_alloc(4), *d_lo = nullptr;
-    uint64_t *h_meta = (uint64_t *)pin_alloc(32), *d_bpos = nullptr;
-    void *d_temp = nullptr;
-    size_t temp_bytes = 0;
+    BuildInput<uint64_t> in("set64_from_uint64", h_off, n, h_off[n]);
+    const uint64_t N = in.N;
+    Set64Ptr R;
+    DevBlock<uint32_t> d_lo;
+    DevBlock<uint64_t> d_bpos;
+    SyncCall call;
     uint64_t nbk = 0;
-    rb200_set64 *R = nullptr;
-    bool ok = d_off && (d_vals || !h_vals) && d_tcnt && d_tbase && d_flag && h_meta &&
-              cudaMemcpyAsync(d_off, h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
-    if (ok && h_vals && N) {
-        H2DStager stage((uint8_t *)d_vals);
-        ok = stage.ok && stage.put(h_vals, 8 * N) && stage.flush();
-        ok = cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
-    }
-    const uint64_t *src = h_vals ? d_vals : d_in;
     // bucket starts per tile, scanned: the total is the bucket count if the values are sorted
-    auto measure = [&]() -> bool {
-        size_t b = 0;
-        if (!build_scan(nullptr, &b, d_tcnt, d_tbase, ntiles + 1, g.stream)) return false;
-        if (b > temp_bytes) {
-            dev_free(d_temp, temp_bytes);
-            temp_bytes = b;
-            if (!(d_temp = dev_alloc(temp_bytes))) return false;
-        }
-        launch_build64_measure(src, d_off, (uint32_t)n, N, d_tcnt, d_flag, g.stream);
-        return build_scan(d_temp, &b, d_tcnt, d_tbase, ntiles + 1, g.stream) &&
-               cudaMemcpyAsync(h_meta, d_tbase + ntiles, 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-               cudaMemcpyAsync(h_meta + 1, d_flag, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-               cudaStreamSynchronize(g.stream) == cudaSuccess;
-    };
-    if (ok) h_meta[1] = 0;
-    ok = ok && cudaMemsetAsync(d_flag, 0, 4, g.stream) == cudaSuccess &&
-         cudaMemsetAsync(d_tcnt + ntiles, 0, 8, g.stream) == cudaSuccess && measure();
-    const uint32_t unsorted = ok ? (uint32_t)h_meta[1] : 0u;
-    if (ok && (unsorted & 2u)) {
-        t_err = "set64_from_uint64: a bitmap of 2^31 values or more is not sorted; pass it sorted";
-        ok = false;
-    }
-    if (ok && unsorted) {
-        ok = sort_segments(src, h_off, d_off, n, &d_sorted, d_temp, temp_bytes);
-        if (ok) {
-            src = d_sorted;
-            ok = measure();
-        }
-        if (!ok && t_err.empty()) t_err = "set64_from_uint64: segmented sort failed";
-    }
-    if (ok) {
-        nbk = h_meta[0];
-        if (nbk >= 0xffffffffull) { t_err = "set64_from_uint64: more than 2^32 - 2 buckets"; ok = false; }
-    }
+    bool ok = in.load(h_vals, d_in, nullptr) && in.measure_sorted([&](const uint64_t *src) {
+        launch_build64_measure(src, in.offs, (uint32_t)n, N, in.tcnt.get(), in.flag.get(), g.stream);
+    }, nbk);
+    if (ok && nbk >= 0xffffffffull) { t_err = "set64_from_uint64: more than 2^32 - 2 buckets"; ok = false; }
     if (ok) ok = (R = set64_new((uint32_t)n, (uint32_t)(nbk + 1))) != nullptr;
     if (ok) {
         // bucket k of the inner set = the sorted low halves lo[b_pos[k] .. b_pos[k + 1]); the sentinel
         // is the empty segment [N, N)
-        uint32_t *d_high = R->d_dir + 2 * n;
+        uint32_t *d_dir = R->d_dir.get(), *d_high = d_dir + 2 * n;
+        uint64_t *h_meta = in.meta.get();
         h_meta[2] = h_meta[3] = N;
-        ok = (d_lo = (uint32_t *)dev_alloc(4 * (N ? N : 1))) && (d_bpos = (uint64_t *)dev_alloc(8 * (nbk + 2))) &&
-             cudaMemcpyAsync(d_bpos + nbk, h_meta + 2, 16, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+        ok = d_lo.reset(N) && d_bpos.reset(nbk + 2) &&
+             cudaMemcpyAsync(d_bpos.get() + nbk, h_meta + 2, 16, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
              cudaMemsetAsync(d_high + nbk, 0, 4, g.stream) == cudaSuccess;
         if (ok) {
-            launch_build64_split(src, d_off, (uint32_t)n, N, d_tbase, d_lo, d_bpos, d_high, g.stream);
-            launch_build_bitmaps(d_off, (uint32_t)n, d_bpos, nbk, R->d_dir, R->d_dir + n, g.stream);
-            dev_free(d_vals, 8 * N);     // stream-ordered reuse: the inner build may take their memory
-            dev_free(d_sorted, 8 * N);
-            d_vals = d_sorted = nullptr;
-            R->inner = from_uint32_impl(nullptr, d_lo, nullptr, nbk + 1, d_bpos, N);
-            ok = R->inner && cudaMemcpyAsync(R->h_dir, R->d_dir, R->dir_bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-                 cudaStreamSynchronize(g.stream) == cudaSuccess;
+            launch_build64_split(in.src, in.offs, (uint32_t)n, N, in.tbase.get(), d_lo.get(), d_bpos.get(), d_high, g.stream);
+            launch_build_bitmaps(in.offs, (uint32_t)n, d_bpos.get(), nbk, d_dir, d_dir + n, g.stream);
+            in.vals.reset();     // stream-ordered reuse: the inner build may take their memory
+            in.sorted.reset();
+            R->inner.reset(from_uint32_impl(nullptr, d_lo.get(), nullptr, nbk + 1, d_bpos.get(), N));
+            ok = R->inner && cudaMemcpyAsync(R->h_dir.get(), d_dir, R->dir_bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+            ok = call.finish(ok, false);
             R->dir_on_device = true;
         }
-    } else {
-        cudaStreamSynchronize(g.stream);
     }
-    dev_free(d_off, 8 * (n + 1));
-    dev_free(d_vals, 8 * N);
-    dev_free(d_sorted, 8 * N);
-    dev_free(d_tcnt, 8 * (ntiles + 1));
-    dev_free(d_tbase, 8 * (ntiles + 1));
-    dev_free(d_flag, 4);
-    dev_free(d_lo, 4 * (N ? N : 1));
-    dev_free(d_bpos, 8 * (nbk + 2));
-    dev_free(d_temp, temp_bytes);
-    pin_free(h_meta, 32);
     if (!ok) {
         if (t_err.empty()) t_err = "set64_from_uint64 failed";
-        set64_delete(R);
         return nullptr;
     }
-    return R;
+    return R.release();
 }
 
 // a[] then b[] as ONE resident set (one H2D); ib2 = ib shifted past a[]
@@ -3934,23 +3780,9 @@ rb200_set64_t *rb200_set64_from_uint64(const uint64_t *vals, const uint64_t *off
 }
 rb200_set64_t *rb200_set64_from_uint64_device(const uint64_t *d_vals, const uint64_t *d_off, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!check_bitmap_count(n, "set64_from_uint64_device")) return nullptr;
-    if (!d_off) { t_err = "set64_from_uint64_device: offsets are NULL"; return nullptr; }
-    if (!ctx_init()) return nullptr;
-    // the offsets are checked on the host before any kernel reads values through them
-    uint64_t *h_off = (uint64_t *)pin_alloc(8 * (n + 1));
-    if (!h_off) return nullptr;
-    rb200_set64 *s = nullptr;
-    if (cudaMemcpyAsync(h_off, d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
-        cudaStreamSynchronize(g.stream) != cudaSuccess) {
-        (void)cudaGetLastError();
-        t_err = "set64_from_uint64_device: offsets are not readable device memory of the library's device";
-    } else if (check_value_offsets(h_off, n, "set64_from_uint64_device")) {
-        if (!d_vals && h_off[n]) t_err = "set64_from_uint64_device: values are NULL";
-        else s = from_uint64_impl(nullptr, d_vals, h_off, n);
-    }
-    pin_free(h_off, 8 * (n + 1));
-    return s;
+    PinBlock<uint64_t> h_off;
+    if (!device_offsets(d_off, d_vals, n, "set64_from_uint64_device", "set64_from_uint64_device", h_off)) return nullptr;
+    return from_uint64_impl(nullptr, d_vals, h_off.get(), n);
 }
 void rb200_set64_free(rb200_set64_t *s) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
@@ -3961,7 +3793,7 @@ int rb200_set64_cardinalities(const rb200_set64_t *s, uint64_t *out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (s->n == 0) return 0;
     std::vector<uint64_t> c(s->nbuckets);
-    if (rb200_set_cardinalities(s->inner, c.data()) != 0) return -1;
+    if (rb200_set_cardinalities(s->inner.get(), c.data()) != 0) return -1;
     for (uint32_t i = 0; i < s->n; i++) {
         uint64_t sum = 0;
         for (uint32_t k = 0; k < s->b_cnt()[i]; k++) sum += c[s->b_beg()[i] + k];
@@ -3982,15 +3814,11 @@ int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return nullptr;
-    rb200_set64 *R = set64_new(S->n, S->nbuckets);
+    Set64Ptr R = set64_new(S->n, S->nbuckets);
     if (!R) return nullptr;
-    memcpy(R->h_dir, S->h_dir, S->dir_bytes);
-    R->inner = convert_impl(S->inner, mode ? 1 : 0);
-    if (!R->inner) {
-        set64_delete(R);
-        return nullptr;
-    }
-    return R;
+    memcpy(R->h_dir.get(), S->h_dir.get(), S->dir_bytes);
+    R->inner.reset(convert_impl(S->inner.get(), mode ? 1 : 0));
+    return R->inner ? R.release() : nullptr;
 }
 int rb200_set64_serialize(const rb200_set64_t *s, char **buf, uint64_t **off, uint64_t **len) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
@@ -4009,13 +3837,10 @@ int rb200_r64_batch_op_serialized(int op, const char *const *a, const size_t *al
     *out = nullptr;
     *off_out = *len_out = nullptr;
     std::vector<uint32_t> ib2;
-    rb200_set64 *S = r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2);
+    Set64Ptr S(r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2));
     if (!S) return -1;
-    rb200_set64 *R = batch_op64_impl(op, S, S, ia, ib2.data(), np);
-    const int rc = R ? serialize64_impl(R, out, off_out, len_out) : -1;
-    set64_delete(R);
-    set64_delete(S);
-    return rc;
+    Set64Ptr R(batch_op64_impl(op, S.get(), S.get(), ia, ib2.data(), np));
+    return R ? serialize64_impl(R.get(), out, off_out, len_out) : -1;
 }
 
 // out[k] = roaring64_bitmap_and_cardinality(a[ia[k]], b[ib[k]]) (roaring64.c:1375)
@@ -4025,11 +3850,9 @@ int rb200_r64_batch_and_cardinality_serialized(const char *const *a, const size_
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!ctx_init()) return -1;
     std::vector<uint32_t> ib2;
-    rb200_set64 *S = r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2);
+    Set64Ptr S(r64_operands(a, alen, na, b, blen, nb, ia, ib, np, ib2));
     if (!S) return -1;
-    const int rc = and_cardinality64_impl(S, S, ia, ib2.data(), np, out);
-    set64_delete(S);
-    return rc;
+    return and_cardinality64_impl(S.get(), S.get(), ia, ib2.data(), np, out);
 }
 
 // ---- in-memory roaring64_bitmap_t (include/roaring/roaring64.h:423-522; src/roaring64.c:1332-1895)
@@ -4091,6 +3914,25 @@ bool r64_deserialize_all(const char *blob, const uint64_t *off, const uint64_t *
     t_err = "roaring64: the host library refused a result blob";
     return false;
 }
+
+// The in-memory operands of rb200_r64_batch_*: a[k] and b[k] written by the host library, pair k
+// made of a[k] and b[k].
+struct R64Pairs {
+    std::vector<std::vector<char>> sa, sb;
+    std::vector<const char *> pa, pb;
+    std::vector<size_t> la, lb;
+    std::vector<uint32_t> idx;   // 0 .. npairs - 1, the pair list of either side
+    bool build(const roaring64_bitmap_t *const *a, const roaring64_bitmap_t *const *b, size_t npairs) {
+        if (!r64_serialize_all(a, npairs, sa) || !r64_serialize_all(b, npairs, sb)) return false;
+        pa.resize(npairs), pb.resize(npairs), la.resize(npairs), lb.resize(npairs), idx.resize(npairs);
+        for (size_t k = 0; k < npairs; k++) {
+            pa[k] = sa[k].data(); la[k] = g_r64.size(a[k]);
+            pb[k] = sb[k].data(); lb[k] = g_r64.size(b[k]);
+            idx[k] = (uint32_t)k;
+        }
+        return true;
+    }
+};
 }  // namespace
 
 rb200_set64_t *rb200_set64_upload(const roaring64_bitmap_t *const *bitmaps, size_t n) {
@@ -4126,20 +3968,12 @@ int rb200_r64_batch_op(int op, const roaring64_bitmap_t *const *a, const roaring
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!g_r64.ok()) return -1;
     if (npairs == 0) return 0;
-    std::vector<std::vector<char>> sa, sb;
-    if (!r64_serialize_all(a, npairs, sa) || !r64_serialize_all(b, npairs, sb)) return -1;
-    std::vector<const char *> pa(npairs), pb(npairs);
-    std::vector<size_t> la(npairs), lb(npairs);
-    std::vector<uint32_t> ia(npairs), ib(npairs);
-    for (size_t k = 0; k < npairs; k++) {
-        pa[k] = sa[k].data(); la[k] = g_r64.size(a[k]);
-        pb[k] = sb[k].data(); lb[k] = g_r64.size(b[k]);
-        ia[k] = ib[k] = (uint32_t)k;
-    }
+    R64Pairs P;
+    if (!P.build(a, b, npairs)) return -1;
     char *blob = nullptr;
     uint64_t *off = nullptr, *len = nullptr;
-    if (rb200_r64_batch_op_serialized(op, pa.data(), la.data(), npairs, pb.data(), lb.data(), npairs, ia.data(),
-                                      ib.data(), npairs, &blob, &off, &len) != 0)
+    if (rb200_r64_batch_op_serialized(op, P.pa.data(), P.la.data(), npairs, P.pb.data(), P.lb.data(), npairs,
+                                      P.idx.data(), P.idx.data(), npairs, &blob, &off, &len) != 0)
         return -1;
     const bool ok = r64_deserialize_all(blob, off, len, npairs, out);
     rb200_serialized_free(blob, off, len);
@@ -4151,18 +3985,10 @@ int rb200_r64_batch_and_cardinality(const roaring64_bitmap_t *const *a, const ro
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!g_r64.ok()) return -1;
     if (npairs == 0) return 0;
-    std::vector<std::vector<char>> sa, sb;
-    if (!r64_serialize_all(a, npairs, sa) || !r64_serialize_all(b, npairs, sb)) return -1;
-    std::vector<const char *> pa(npairs), pb(npairs);
-    std::vector<size_t> la(npairs), lb(npairs);
-    std::vector<uint32_t> ia(npairs), ib(npairs);
-    for (size_t k = 0; k < npairs; k++) {
-        pa[k] = sa[k].data(); la[k] = g_r64.size(a[k]);
-        pb[k] = sb[k].data(); lb[k] = g_r64.size(b[k]);
-        ia[k] = ib[k] = (uint32_t)k;
-    }
-    return rb200_r64_batch_and_cardinality_serialized(pa.data(), la.data(), npairs, pb.data(), lb.data(), npairs,
-                                                      ia.data(), ib.data(), npairs, out);
+    R64Pairs P;
+    if (!P.build(a, b, npairs)) return -1;
+    return rb200_r64_batch_and_cardinality_serialized(P.pa.data(), P.la.data(), npairs, P.pb.data(), P.lb.data(), npairs,
+                                                      P.idx.data(), P.idx.data(), npairs, out);
 }
 
 // drop-in symbols, include/roaring/roaring64.h:423-522
@@ -4209,15 +4035,12 @@ bool roaring64_bitmap_intersect(const roaring64_bitmap_t *r1, const roaring64_bi
 static roaring_bitmap_t *dropin_lazy_pair(int op, const roaring_bitmap_t *r1, const roaring_bitmap_t *r2, int rules) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const roaring_bitmap_t *both[2] = {r1, r2};
-    rb200_set *S = rb200_set_upload(both, 2);
+    SetPtr S(rb200_set_upload(both, 2));
     if (!S) return nullptr;
-    rb200_set_bind_host(S, 1);
+    rb200_set_bind_host(S.get(), 1);
     const uint32_t ia = 0, ib = 1;
-    rb200_set *R = batch_op_impl(op, S, S, &ia, &ib, 1, rules);
-    roaring_bitmap_t *out = R ? rb200_set_download(R, 0) : nullptr;
-    set_delete(R);
-    set_delete(S);
-    return out;
+    SetPtr R(batch_op_impl(op, S.get(), S.get(), &ia, &ib, 1, rules));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 roaring_bitmap_t *roaring_bitmap_lazy_or(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2, const bool bitsetconversion) {
     return dropin_lazy_pair(OP_OR, r1, r2, RULES_LAZY | (bitsetconversion ? RULES_CONV : 0));
@@ -4234,12 +4057,10 @@ void roaring_bitmap_lazy_xor_inplace(roaring_bitmap_t *r1, const roaring_bitmap_
 void roaring_bitmap_repair_after_lazy(roaring_bitmap_t *r1) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const roaring_bitmap_t *one[1] = {r1};
-    rb200_set *S = rb200_set_upload(one, 1);
+    SetPtr S(rb200_set_upload(one, 1));
     if (!S) { dropin_failed("roaring_bitmap_repair_after_lazy"); return; }
-    rb200_set *R = rb200_set_repair_after_lazy(S);
-    roaring_bitmap_t *out = R ? rb200_set_download(R, 0) : nullptr;
-    set_delete(R);
-    set_delete(S);
+    roaring_bitmap_t *out = nullptr;
+    if (SetPtr R{rb200_set_repair_after_lazy(S.get())}) out = rb200_set_download(R.get(), 0);
     if (out) swap_into(r1, out);
     else dropin_failed("roaring_bitmap_repair_after_lazy");
 }
@@ -4294,20 +4115,17 @@ bool portable_sizes(const rb200_set *S, std::vector<uint32_t> &out) {
     const size_t nb = S->n_bitmaps;
     out.assign(nb, 0);
     if (!nb) return true;
-    uint64_t *d16 = (uint64_t *)dev_alloc(8 * nb);
-    uint32_t *dex = (uint32_t *)dev_alloc(4 * nb), *dhr = (uint32_t *)dev_alloc(4 * nb);
-    uint32_t *h = (uint32_t *)pin_alloc(4 * nb);
+    DevBlock<uint64_t> d16(nb);
+    DevBlock<uint32_t> dex(nb), dhr(nb);
+    PinBlock<uint32_t> h(nb);
+    SyncCall call;
     bool ok = d16 && dex && dhr && h;
     if (ok) {
-        launch_serialize_measure(S->view(), (uint32_t)nb, d16, dex, dhr, g.stream);
-        ok = cudaMemcpyAsync(h, dex, 4 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
-             cudaStreamSynchronize(g.stream) == cudaSuccess;
-        if (ok) out.assign(h, h + nb);
+        launch_serialize_measure(S->view(), (uint32_t)nb, d16.get(), dex.get(), dhr.get(), g.stream);
+        ok = cudaMemcpyAsync(h.get(), dex.get(), 4 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        ok = call.finish(ok, false);
+        if (ok) out.assign(h.get(), h.get() + nb);
     }
-    dev_free(d16, 8 * nb);
-    dev_free(dex, 4 * nb);
-    dev_free(dhr, 4 * nb);
-    pin_free(h, 4 * nb);
     if (!ok && t_err.empty()) t_err = "portable_sizes failed";
     return ok;
 }
@@ -4325,13 +4143,11 @@ rb200_set_t *rb200_or_many_heap(const rb200_set_t *S, const uint32_t *idx, size_
         roaring_bitmap_t *e = bitmap_alloc(0);
         if (!e) return nullptr;
         const roaring_bitmap_t *one[1] = {e};
-        rb200_set *E = rb200_set_upload(one, 1);
+        SetPtr E(rb200_set_upload(one, 1));
         bitmap_free_host(e);
         if (!E) return nullptr;
         const uint32_t a = idx ? idx[0] : 0u, z = 0;
-        rb200_set *R = batch_op_impl(OP_OR, S, E, &a, &z, 1, 0);
-        set_delete(E);
-        return R;
+        return batch_op_impl(OP_OR, S, E.get(), &a, &z, 1, 0);
     }
     std::vector<uint32_t> sz;
     if (!portable_sizes(S, sz)) return nullptr;
@@ -4345,39 +4161,33 @@ rb200_set_t *rb200_or_many_heap(const rb200_set_t *S, const uint32_t *idx, size_
     bool ok = true;
     while (cnt > 1 && ok) {
         const HeapEl a = heap_pop(e, cnt), b = heap_pop(e, cnt);
-        rb200_set *R;
+        const SetPtr a_temp(a.temp ? a.set : nullptr), b_temp(b.temp ? b.set : nullptr);  // consumed here
+        SetPtr R;
         if (a.temp && b.temp)
-            R = batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY | RULES_INPLACE | RULES_NOFULL);
+            R.reset(batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY | RULES_INPLACE | RULES_NOFULL));
         else if (b.temp)  // roaring_bitmap_lazy_or_inplace(x2, x1, false)
-            R = batch_op_impl(OP_OR, b.set, a.set, &b.index, &a.index, 1, RULES_LAZY | RULES_INPLACE);
+            R.reset(batch_op_impl(OP_OR, b.set, a.set, &b.index, &a.index, 1, RULES_LAZY | RULES_INPLACE));
         else if (a.temp)
-            R = batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY | RULES_INPLACE);
+            R.reset(batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY | RULES_INPLACE));
         else
-            R = batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY);
-        if (a.temp) set_delete(a.set);
-        if (b.temp) set_delete(b.set);
-        if (!R || !resolve(R)) { set_delete(R); ok = false; break; }
-        heap_push(e, cnt, HeapEl{R->out_portable, true, R, 0});  // size measured by k_finalize_pairs
+            R.reset(batch_op_impl(OP_OR, a.set, b.set, &a.index, &b.index, 1, RULES_LAZY));
+        if (!R || !resolve(R.get())) { ok = false; break; }
+        heap_push(e, cnt, HeapEl{R->out_portable, true, R.release(), 0});  // size measured by k_finalize_pairs
     }
     if (!ok) {
-        for (uint32_t i = 0; i < cnt; i++) if (e[i].temp) set_delete(e[i].set);
+        for (uint32_t i = 0; i < cnt; i++) if (e[i].temp) SetFree()(e[i].set);
         return nullptr;
     }
-    const HeapEl top = heap_pop(e, cnt);
-    rb200_set *out = convert_impl(top.set, 2);  // roaring_bitmap_repair_after_lazy
-    set_delete(top.set);
-    return out;
+    const SetPtr top(heap_pop(e, cnt).set);   // n >= 2: a temporary
+    return convert_impl(top.get(), 2);        // roaring_bitmap_repair_after_lazy
 }
 
 roaring_bitmap_t *roaring_bitmap_or_many_heap(uint32_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    rb200_set *S = rb200_set_upload(rs, number);
+    SetPtr S(rb200_set_upload(rs, number));
     if (!S) return nullptr;
-    rb200_set *R = rb200_or_many_heap(S, nullptr, number);
-    roaring_bitmap_t *out = R ? rb200_set_download(R, 0) : nullptr;
-    set_delete(R);
-    set_delete(S);
-    return out;
+    SetPtr R(rb200_or_many_heap(S.get(), nullptr, number));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 
 }  // extern "C"
