@@ -18,6 +18,11 @@ constexpr int MAX_ARRAY = 4096;
 constexpr int BITSET_BYTES = 8192;
 constexpr int ACC_WORDS = 2048;  // 65536 bits as 32-bit words
 
+// Serialized formats: portable cookies and the container count from which a blob with run containers
+// carries an offset header (include/roaring/roaring_array.h:35-40), frozen cookie (src/roaring.c:3180)
+constexpr uint32_t SERIAL_COOKIE_NO_RUN = 12346, SERIAL_COOKIE = 12347, FROZEN_COOKIE = 13766;
+constexpr uint32_t NO_OFFSET_THRESHOLD = 4;
+
 enum Op { OP_AND = 0, OP_OR = 1, OP_XOR = 2, OP_ANDNOT = 3 };
 
 // work-item kinds produced by the planner

@@ -126,6 +126,11 @@ __host__ __device__ __forceinline__ uint32_t stored_bytes(int t, uint32_t len) {
 __host__ __device__ __forceinline__ uint32_t portable_bytes(int t, uint32_t len) {
     return t == T_BITSET ? (uint32_t)BITSET_BYTES : (t == T_ARRAY ? 2u * len : 2u + 4u * len);
 }
+// header bytes of a portable bitmap of n containers (roaring_array.c:469-500)
+__host__ __device__ __forceinline__ uint32_t portable_header_bytes(uint32_t n, bool hasrun) {
+    if (!hasrun) return 8u + 8u * n;
+    return 4u + ((n + 7u) >> 3) + (n < NO_OFFSET_THRESHOLD ? 4u * n : 8u * n);
+}
 
 // "Effective bytes" of a container: what it can contribute to the result of a later op on it — its
 // stored size, or the size of its values as an array / bitset if that is larger (a run of 4 bytes

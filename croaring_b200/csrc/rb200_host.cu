@@ -37,6 +37,7 @@
 #include "rb200_common.h"
 #include "rb200_device.cuh"
 #include "rb200_internal.h"
+#include "rb200_portable.h"
 
 using namespace rb200;
 
@@ -50,8 +51,6 @@ struct run_container_t { int32_t n_runs; int32_t capacity; rle16_t *runs; };    
 struct shared_container_t { void *container; uint8_t typecode; uint32_t counter; };      // containers.h:71-75
 
 constexpr uint8_t FLAG_COW = 1, FLAG_FROZEN = 2;  // roaring_types.h:46-49
-constexpr uint32_t SERIAL_COOKIE_NO_RUN = 12346, SERIAL_COOKIE = 12347;  // roaring_array.h:35-40
-constexpr int32_t NO_OFFSET_THRESHOLD = 4;
 constexpr uint32_t M2_SCRATCH_SLOTS = 2048, M2_SCRATCH_WORDS = 2 * ACC_WORDS + 32;  // rb200_many2.cu split keys
 
 // ------------------------------------------------------------------ host allocation hooks
@@ -772,6 +771,30 @@ inline uint32_t host_container_card(const void *c, uint8_t type) {
     return s;
 }
 
+// Container i of a host bitmap, SHARED unwrapped (*was_shared tells whether it was), payload in the
+// slab's layout.  A lazy bitset (cardinality field negative, bitset.h:42) has CARD_UNKNOWN set.
+inline PortableEntry entry_of(const roaring_array_t *ra, int32_t i, bool *was_shared = nullptr) {
+    uint8_t t = ra->typecodes[i];
+    if (was_shared) *was_shared = t == T_SHARED;
+    const void *c = unwrap_shared(ra->containers[i], t);
+    PortableEntry e;
+    e.key = ra->keys[i];
+    e.type = t;
+    e.card = host_container_card(c, t);
+    if (t == T_BITSET) {
+        e.len = 1024;
+        e.payload = (const uint8_t *)((const bitset_container_t *)c)->words;
+        if (((const bitset_container_t *)c)->cardinality < 0) e.card |= CARD_UNKNOWN;
+    } else if (t == T_ARRAY) {
+        e.len = e.card;
+        e.payload = (const uint8_t *)((const array_container_t *)c)->array;
+    } else {
+        e.len = (uint32_t)((const run_container_t *)c)->n_runs;
+        e.payload = (const uint8_t *)((const run_container_t *)c)->runs;
+    }
+    return e;
+}
+
 }  // namespace
 
 // =================================================================== C ABI: helpers
@@ -818,11 +841,7 @@ void rb200_bitmap_free(roaring_bitmap_t *r) { bitmap_free_host(r); }
 uint64_t rb200_bitmap_get_cardinality(const roaring_bitmap_t *r) {
     const roaring_array_t *ra = &r->high_low_container;
     uint64_t s = 0;
-    for (int32_t i = 0; i < ra->size; i++) {
-        uint8_t t = ra->typecodes[i];
-        const void *c = unwrap_shared(ra->containers[i], t);
-        s += host_container_card(c, t);
-    }
+    for (int32_t i = 0; i < ra->size; i++) s += entry_of(ra, i).card & CARD_MASK;
     return s;
 }
 
@@ -873,235 +892,53 @@ bool rb200_bitmap_validate(const roaring_bitmap_t *r, const char **reason) {
 // ---- portable format ------------------------------------------------------------------
 size_t rb200_bitmap_portable_size_in_bytes(const roaring_bitmap_t *r) {
     const roaring_array_t *ra = &r->high_low_container;
-    bool hasrun = false;
-    size_t payload = 0;
-    for (int32_t i = 0; i < ra->size; i++) {
-        uint8_t t = ra->typecodes[i];
-        const void *c = unwrap_shared(ra->containers[i], t);
-        if (t == T_RUN) {
-            hasrun = true;
-            payload += 2 + 4 * (size_t)((const run_container_t *)c)->n_runs;
-        } else if (t == T_ARRAY) {
-            payload += 2 * (size_t)((const array_container_t *)c)->cardinality;
-        } else {
-            payload += BITSET_BYTES;
-        }
-    }
-    const size_t n = (size_t)ra->size;
-    size_t hdr;
-    if (hasrun) hdr = 4 + (n + 7) / 8 + (ra->size < NO_OFFSET_THRESHOLD ? 4 * n : 8 * n);
-    else hdr = 8 + 8 * n;
-    return hdr + payload;
+    return portable_size((uint32_t)ra->size, [ra](uint32_t i) { return entry_of(ra, (int32_t)i); });
 }
 
 size_t rb200_bitmap_portable_serialize(const roaring_bitmap_t *r, char *buf) {
     const roaring_array_t *ra = &r->high_low_container;
-    const size_t n = (size_t)ra->size;
-    bool hasrun = false;
-    for (int32_t i = 0; i < ra->size; i++) {
-        uint8_t t = ra->typecodes[i];
-        unwrap_shared(ra->containers[i], t);
-        hasrun |= (t == T_RUN);
-    }
-    uint8_t *p = (uint8_t *)buf;
-    uint32_t start;
-    if (hasrun) {
-        const uint32_t cookie = SERIAL_COOKIE | ((uint32_t)(ra->size - 1) << 16);
-        memcpy(p, &cookie, 4);
-        p += 4;
-        const size_t s = (n + 7) / 8;
-        memset(p, 0, s);
-        for (int32_t i = 0; i < ra->size; i++) {
-            uint8_t t = ra->typecodes[i];
-            unwrap_shared(ra->containers[i], t);
-            if (t == T_RUN) p[i / 8] |= (uint8_t)(1 << (i % 8));
-        }
-        p += s;
-        start = (uint32_t)(4 + s + (ra->size < NO_OFFSET_THRESHOLD ? 4 * n : 8 * n));
-    } else {
-        const uint32_t cookie = SERIAL_COOKIE_NO_RUN, sz = (uint32_t)ra->size;
-        memcpy(p, &cookie, 4);
-        memcpy(p + 4, &sz, 4);
-        p += 8;
-        start = (uint32_t)(8 + 8 * n);
-    }
-    for (int32_t i = 0; i < ra->size; i++) {
-        uint8_t t = ra->typecodes[i];
-        const void *c = unwrap_shared(ra->containers[i], t);
-        const uint16_t key = ra->keys[i], cm1 = (uint16_t)(host_container_card(c, t) - 1);
-        memcpy(p, &key, 2);
-        memcpy(p + 2, &cm1, 2);
-        p += 4;
-    }
-    if (!hasrun || ra->size >= NO_OFFSET_THRESHOLD) {
-        uint32_t off = start;
-        for (int32_t i = 0; i < ra->size; i++) {
-            memcpy(p, &off, 4);
-            p += 4;
-            uint8_t t = ra->typecodes[i];
-            const void *c = unwrap_shared(ra->containers[i], t);
-            off += t == T_BITSET ? (uint32_t)BITSET_BYTES
-                   : t == T_ARRAY ? 2u * (uint32_t)((const array_container_t *)c)->cardinality
-                                  : 2u + 4u * (uint32_t)((const run_container_t *)c)->n_runs;
-        }
-    }
-    for (int32_t i = 0; i < ra->size; i++) {
-        uint8_t t = ra->typecodes[i];
-        const void *c = unwrap_shared(ra->containers[i], t);
-        if (t == T_BITSET) {
-            memcpy(p, ((const bitset_container_t *)c)->words, BITSET_BYTES);
-            p += BITSET_BYTES;
-        } else if (t == T_ARRAY) {
-            const array_container_t *a = (const array_container_t *)c;
-            memcpy(p, a->array, 2 * (size_t)a->cardinality);
-            p += 2 * (size_t)a->cardinality;
-        } else {
-            const run_container_t *rc = (const run_container_t *)c;
-            const uint16_t nr = (uint16_t)rc->n_runs;
-            memcpy(p, &nr, 2);
-            memcpy(p + 2, rc->runs, 4 * (size_t)rc->n_runs);
-            p += 2 + 4 * (size_t)rc->n_runs;
-        }
-    }
-    return (size_t)(p - (uint8_t *)buf);
+    return write_portable((uint8_t *)buf, (uint32_t)ra->size, [ra](uint32_t i) { return entry_of(ra, (int32_t)i); });
 }
 
-}  // extern "C"
-
-namespace {
-
-// Parsed view of one portable-serialized bitmap (no allocation): per container key, type,
-// cardinality, length and a pointer to the stored payload inside the buffer.
-struct PView {
-    int32_t size = 0;
-    std::vector<uint16_t> key;
-    std::vector<uint8_t> type;
-    std::vector<uint32_t> card, len;
-    std::vector<const uint8_t *> ptr;
-};
-
-bool parse_portable(const uint8_t *buf, size_t len, PView &v) {
-    if (len < 4) return false;
-    uint32_t cookie;
-    memcpy(&cookie, buf, 4);
-    size_t pos = 4;
-    int32_t size;
-    const uint8_t *runflags = nullptr;
-    bool hasrun = false;
-    if ((cookie & 0xFFFF) == SERIAL_COOKIE) {
-        size = (int32_t)(cookie >> 16) + 1;
-        hasrun = true;
-        runflags = buf + pos;
-        pos += (size_t)(size + 7) / 8;
-    } else if (cookie == SERIAL_COOKIE_NO_RUN) {
-        if (len < 8) return false;
-        uint32_t s;
-        memcpy(&s, buf + 4, 4);
-        size = (int32_t)s;
-        pos = 8;
-    } else {
-        return false;
-    }
-    if (size < 0 || size > 65536) return false;
-    if (pos + 4 * (size_t)size > len) return false;
-    const uint8_t *kc = buf + pos;
-    pos += 4 * (size_t)size;
-    if (!hasrun || size >= NO_OFFSET_THRESHOLD) pos += 4 * (size_t)size;
-    v.size = size;
-    v.key.resize(size);
-    v.type.resize(size);
-    v.card.resize(size);
-    v.len.resize(size);
-    v.ptr.resize(size);
-    for (int32_t i = 0; i < size; i++) {
-        uint16_t key, cm1;
-        memcpy(&key, kc + 4 * i, 2);
-        memcpy(&cm1, kc + 4 * i + 2, 2);
-        if (i > 0 && key <= v.key[i - 1]) return false;
-        const uint32_t card = (uint32_t)cm1 + 1;
-        v.key[i] = key;
-        v.card[i] = card;
-        const bool isrun = hasrun && ((runflags[i / 8] >> (i % 8)) & 1);
-        if (isrun) {
-            if (pos + 2 > len) return false;
-            uint16_t nr;
-            memcpy(&nr, buf + pos, 2);
-            pos += 2;
-            if (pos + 4 * (size_t)nr > len) return false;
-            v.type[i] = T_RUN;
-            v.len[i] = nr;
-            v.ptr[i] = buf + pos;
-            pos += 4 * (size_t)nr;
-        } else if (card > (uint32_t)MAX_ARRAY) {
-            if (pos + BITSET_BYTES > len) return false;
-            v.type[i] = T_BITSET;
-            v.len[i] = 1024;
-            v.ptr[i] = buf + pos;
-            pos += BITSET_BYTES;
-        } else {
-            if (pos + 2 * (size_t)card > len) return false;
-            v.type[i] = T_ARRAY;
-            v.len[i] = card;
-            v.ptr[i] = buf + pos;
-            pos += 2 * (size_t)card;
-        }
-    }
-    return true;
-}
-
-}  // namespace
-
-extern "C" roaring_bitmap_t *rb200_bitmap_portable_deserialize_safe(const char *buf, size_t maxbytes) {
-    PView v;
-    if (!parse_portable((const uint8_t *)buf, maxbytes, v)) return nullptr;
-    roaring_bitmap_t *r = bitmap_alloc(v.size);
+roaring_bitmap_t *rb200_bitmap_portable_deserialize_safe(const char *buf, size_t maxbytes) {
+    std::vector<PortableEntry> c;
+    if (!walk_portable((const uint8_t *)buf, maxbytes, [&c](const PortableEntry &e) { c.push_back(e); })) return nullptr;
+    roaring_bitmap_t *r = bitmap_alloc((int32_t)c.size());
     if (!r) return nullptr;
     roaring_array_t *ra = &r->high_low_container;
-    for (int32_t i = 0; i < v.size; i++) {
-        void *c = container_from_payload(v.type[i], v.card[i], v.len[i], v.ptr[i]);
-        if (!c) {
+    for (const PortableEntry &e : c) {
+        void *hc = container_from_payload(e.type, e.card, e.len, e.payload);
+        if (!hc) {
             bitmap_free_host(r);
             return nullptr;
         }
-        ra->containers[i] = c;
-        ra->keys[i] = v.key[i];
-        ra->typecodes[i] = v.type[i];
-        ra->size = i + 1;
+        ra->containers[ra->size] = hc;
+        ra->keys[ra->size] = e.key;
+        ra->typecodes[ra->size] = e.type;
+        ra->size++;
     }
     return r;
 }
 
+}  // extern "C"
+
 // =================================================================== upload
 namespace {
 
-// Source of containers for packing: either host bitmaps or parsed portable buffers.
-struct PackSrc {
-    const roaring_bitmap_t *const *bms = nullptr;
-    const std::vector<PView> *views = nullptr;
-    size_t n = 0;
-};
-
-rb200_set *upload_impl(const PackSrc &src) {
+rb200_set *upload_impl(const roaring_bitmap_t *const *bms, size_t nb) {
     if (!ctx_init()) return nullptr;
-    const size_t nb = src.n;
     // pass 1: sizes
     uint64_t nc = 0, slab = 0;
     for (size_t b = 0; b < nb; b++) {
-        if (src.bms) {
-            const roaring_array_t *ra = &src.bms[b]->high_low_container;
-            nc += (uint64_t)ra->size;
-            for (int32_t i = 0; i < ra->size; i++) {
-                uint8_t t = ra->typecodes[i];
-                const void *c = unwrap_shared(ra->containers[i], t);
-                uint32_t len = t == T_BITSET ? 1024u
-                               : t == T_ARRAY ? (uint32_t)((const array_container_t *)c)->cardinality
-                                              : (uint32_t)((const run_container_t *)c)->n_runs;
-                slab += round16(stored_bytes(t, len));
-            }
-        } else {
-            const PView &v = (*src.views)[b];
-            nc += (uint64_t)v.size;
-            for (int32_t i = 0; i < v.size; i++) slab += round16(stored_bytes(v.type[i], v.len[i]));
+        const roaring_array_t *ra = &bms[b]->high_low_container;
+        nc += (uint64_t)ra->size;
+        for (int32_t i = 0; i < ra->size; i++) {
+            uint8_t t = ra->typecodes[i];
+            const void *c = unwrap_shared(ra->containers[i], t);
+            uint32_t len = t == T_BITSET ? 1024u
+                           : t == T_ARRAY ? (uint32_t)((const array_container_t *)c)->cardinality
+                                          : (uint32_t)((const run_container_t *)c)->n_runs;
+            slab += round16(stored_bytes(t, len));
         }
     }
     SetPtr s = set_new((uint32_t)nb, nc, slab);
@@ -1121,73 +958,34 @@ rb200_set *upload_impl(const PackSrc &src) {
         uint32_t *c_card = (uint32_t *)(hd + s->L.o_card), *c_len = (uint32_t *)(hd + s->L.o_len);
         uint64_t *c_off = (uint64_t *)(hd + s->L.o_off);
         uint32_t *c_src = (uint32_t *)(hd + s->L.o_src);
-        if (src.bms) s->h_ptr_all = std::make_shared<std::vector<const void *>>(nc);
+        s->h_ptr_all = std::make_shared<std::vector<const void *>>(nc);
         uint64_t ci = 0, off = 0;
         for (size_t b = 0; b < nb && ok; b++) {
-            const roaring_array_t *ra = src.bms ? &src.bms[b]->high_low_container : nullptr;
-            const PView *pv = src.views ? &(*src.views)[b] : nullptr;
-            const int32_t size = ra ? ra->size : pv->size;
+            const roaring_array_t *ra = &bms[b]->high_low_container;
             bm_beg[b] = (uint32_t)ci;
-            bm_cnt[b] = (uint32_t)size;
-            s->h_cnt[b] = (uint32_t)size;
-            s->h_flags[b] = ra ? (ra->flags & FLAG_COW) : 0;
+            bm_cnt[b] = (uint32_t)ra->size;
+            s->h_cnt[b] = (uint32_t)ra->size;
+            s->h_flags[b] = ra->flags & FLAG_COW;
             uint64_t bcard = 0, bbytes = 0, bebytes = 0;
-            for (int32_t i = 0; i < size; i++, ci++) {
-                uint8_t t;
-                uint32_t card, len;
-                const uint8_t *p;
-                uint16_t key;
-                bool was_shared = false;
-                if (ra) {
-                    t = ra->typecodes[i];
-                    was_shared = t == T_SHARED;
-                    const void *c = unwrap_shared(ra->containers[i], t);
-                    key = ra->keys[i];
-                    card = host_container_card(c, t);
-                    if (t == T_BITSET) {
-                        len = 1024;
-                        p = (const uint8_t *)((const bitset_container_t *)c)->words;
-                        if (((const bitset_container_t *)c)->cardinality < 0) {  // lazy state
-                            card |= CARD_UNKNOWN;
-                            s->lazy = true;
-                        }
-                    }
-                    else if (t == T_ARRAY) { len = card; p = (const uint8_t *)((const array_container_t *)c)->array; }
-                    else {
-                        len = (uint32_t)((const run_container_t *)c)->n_runs;
-                        p = (const uint8_t *)((const run_container_t *)c)->runs;
-                        if (4 * (uint64_t)len > BITSET_BYTES) s->lazy = true;  // only lazy unions leave such runs
-                    }
-                } else {
-                    t = pv->type[i];
-                    key = pv->key[i];
-                    len = pv->len[i];
-                    p = pv->ptr[i];
-                    if (t == T_RUN) {
-                        card = 0;
-                        for (uint32_t k = 0; k < len; k++) {
-                            uint16_t l;
-                            memcpy(&l, p + 4 * k + 2, 2);
-                            card += (uint32_t)l + 1;
-                        }
-                    } else {
-                        card = pv->card[i];
-                    }
-                }
-                const uint32_t sb = stored_bytes(t, len), sb16 = round16(sb);
-                ok = ok && stage.put(p, sb) && stage.put(nullptr, sb16 - sb);
-                c_key[ci] = key;
-                c_type[ci] = t;
-                c_card[ci] = card;
-                c_len[ci] = len;
+            for (int32_t i = 0; i < ra->size; i++, ci++) {
+                bool was_shared;
+                const PortableEntry e = entry_of(ra, i, &was_shared);
+                if (e.card & CARD_UNKNOWN) s->lazy = true;
+                if (e.type == T_RUN && 4 * (uint64_t)e.len > BITSET_BYTES) s->lazy = true;  // only lazy unions leave such runs
+                const uint32_t sb = stored_bytes(e.type, e.len), sb16 = round16(sb);
+                ok = ok && stage.put(e.payload, sb) && stage.put(nullptr, sb16 - sb);
+                c_key[ci] = e.key;
+                c_type[ci] = e.type;
+                c_card[ci] = e.card;
+                c_len[ci] = e.len;
                 c_off[ci] = off;
                 c_src[ci] = was_shared ? SRC_SHARED : SRC_NONE;
-                if (s->h_ptr_all) (*s->h_ptr_all)[ci] = p;
+                (*s->h_ptr_all)[ci] = e.payload;
                 off += sb16;
-                bcard += card & CARD_MASK;
+                bcard += e.card & CARD_MASK;
                 bbytes += sb16;
-                bebytes += effective_bytes(t, len, card & CARD_MASK);
-                s->portable_bytes += portable_bytes(t, len);
+                bebytes += effective_bytes(e.type, e.len, e.card & CARD_MASK);
+                s->portable_bytes += portable_bytes(e.type, e.len);
             }
             bm_card[b] = bcard;
             s->h_bytes[b] = bbytes;
@@ -1210,10 +1008,7 @@ extern "C" {
 
 rb200_set_t *rb200_set_upload(const roaring_bitmap_t *const *bitmaps, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    PackSrc src;
-    src.bms = bitmaps;
-    src.n = n;
-    return upload_impl(src);
+    return upload_impl(bitmaps, n);
 }
 
 // Portable-serialized inputs are parsed ON THE DEVICE (src/roaring_array.c:633-813 restated as
@@ -1234,22 +1029,21 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
     if (!ctx_init()) return nullptr;
     if (n > 0xffffffffull) { t_err = "too many bitmaps"; return nullptr; }
     // pass 1 (host): container count of every blob from its cookie; staging offsets
-    uint64_t nc = 0, raw_total = 0, slab_total = 0;
+    uint64_t nc = 0, raw_total = 0, slab_total = 0, payload = 0;
     std::vector<uint32_t> cnt(n);
     for (size_t i = 0; i < n; i++) {
-        uint32_t cookie = 0, size = 0;
-        bool ok = lens[i] >= 4;
-        if (ok && frozen) {
-            memcpy(&cookie, bufs[i] + lens[i] - 4, 4);   // the header is the LAST word
+        uint32_t size = 0;
+        bool hasrun = false, ok;
+        if (frozen) {
+            uint32_t cookie = 0;
+            ok = lens[i] >= 4;
+            if (ok) memcpy(&cookie, bufs[i] + lens[i] - 4, 4);   // the header is the LAST word
             size = cookie >> 15;
-            ok = (cookie & 0x7FFF) == 13766 /* FROZEN_COOKIE */ && 5ull * size + 4 <= lens[i];
-        } else if (ok) {
-            memcpy(&cookie, bufs[i], 4);
-            if ((cookie & 0xFFFF) == SERIAL_COOKIE) size = (cookie >> 16) + 1;
-            else if (cookie == SERIAL_COOKIE_NO_RUN && lens[i] >= 8) memcpy(&size, bufs[i] + 4, 4);
-            else ok = false;
+            ok = ok && (cookie & 0x7FFF) == FROZEN_COOKIE && 5ull * size + 4 <= lens[i] && size <= 65536;
+        } else {
+            ok = portable_count((const uint8_t *)bufs[i], lens[i], size, hasrun);
         }
-        if (!ok || size > 65536 || 4ull * size > lens[i]) {
+        if (!ok) {
             t_err = std::string(frozen ? "malformed frozen bitmap at index " : "malformed portable bitmap at index ") + std::to_string(i);
             return nullptr;
         }
@@ -1257,11 +1051,14 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
         nc += size;
         raw_total += (lens[i] + 15) & ~(uint64_t)15;
         slab_total += ((lens[i] + 15) & ~(uint64_t)15) + 16ull * size;   // payload <= blob bytes, + 16-byte padding per container
+        const uint64_t hdr = frozen ? 4 + 5ull * size : portable_header_bytes(size, hasrun);
+        payload += lens[i] > hdr ? lens[i] - hdr : 0;
     }
     SetPtr s = set_new((uint32_t)n, nc, slab_total + 16);
     if (!s) return nullptr;
     s->n_containers = nc;
     s->slab_used = slab_total;
+    s->portable_bytes = payload;
     // per-bitmap tables: [roff | rlen | slab_base] for the kernels, bm_beg / bm_cnt into the directory
     PinBlock<uint64_t> tab(3 * n);
     PinBlock<uint32_t> bc(2 * n);
@@ -1283,10 +1080,6 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
             s->h_cnt[i] = cnt[i];
             s->h_bytes[i] = lens[i] + 16ull * cnt[i];
             s->h_ebytes[i] = (uint64_t)cnt[i] * BITSET_BYTES + lens[i];   // replaced by the device's figures (ensure_mirrors)
-            const uint64_t hdr = ((cnt[i] && (((uint8_t)bufs[i][0] | ((uint8_t)bufs[i][1] << 8)) == SERIAL_COOKIE))
-                                     ? 4 + (cnt[i] + 7) / 8 + (cnt[i] < (uint32_t)NO_OFFSET_THRESHOLD ? 4ull : 8ull) * cnt[i]
-                                     : 8 + 8ull * cnt[i]);
-            s->portable_bytes += frozen ? lens[i] - 4 - 5ull * cnt[i] + 0 : (lens[i] > hdr ? lens[i] - hdr : 0);
             ro += (lens[i] + 15) & ~(uint64_t)15;
             so += ((lens[i] + 15) & ~(uint64_t)15) + 16ull * cnt[i];
             cb += cnt[i];
@@ -3103,34 +2896,21 @@ static int pair_fused(int op, const roaring_bitmap_t *r1, const roaring_bitmap_t
     uint32_t ci = 0;
     for (int side = 0; side < 2; side++) {
         for (int32_t i = 0; i < ra[side]->size; i++, ci++) {
-            uint8_t t = ra[side]->typecodes[i];
-            const bool was_shared = t == T_SHARED;
-            const void *c = unwrap_shared(ra[side]->containers[i], t);
-            uint32_t card = host_container_card(c, t), len;
-            const uint8_t *p;
-            if (t == T_BITSET) {
-                len = 1024;
-                p = (const uint8_t *)((const bitset_container_t *)c)->words;
-                if (((const bitset_container_t *)c)->cardinality < 0) return 0;   // lazy state: batched path
-            } else if (t == T_ARRAY) {
-                len = card;
-                p = (const uint8_t *)((const array_container_t *)c)->array;
-            } else {
-                len = (uint32_t)((const run_container_t *)c)->n_runs;
-                p = (const uint8_t *)((const run_container_t *)c)->runs;
-            }
-            const uint32_t sb = stored_bytes(t, len), sb16 = round16(sb);
+            bool was_shared;
+            const PortableEntry e = entry_of(ra[side], i, &was_shared);
+            if (e.card & CARD_UNKNOWN) return 0;   // lazy state: batched path
+            const uint32_t sb = stored_bytes(e.type, e.len), sb16 = round16(sb);
             if (o + sb16 > FUSED_IN_BYTES) return 0;
-            memcpy(h + o, p, sb);
+            memcpy(h + o, e.payload, sb);
             if (sb16 > sb) memset(h + o + sb, 0, sb16 - sb);
-            c_key[ci] = ra[side]->keys[i];
-            c_type[ci] = t;
+            c_key[ci] = e.key;
+            c_type[ci] = e.type;
             c_shared[ci] = was_shared ? 1 : 0;
-            c_card[ci] = card;
-            c_len[ci] = len;
+            c_card[ci] = e.card;
+            c_len[ci] = e.len;
             c_off[ci] = (uint32_t)o;
             o += sb16;
-            E[side] += effective_bytes(t, len, card);
+            E[side] += effective_bytes(e.type, e.len, e.card);
         }
     }
     // the result slots must fit the mapped block (same bound as PairBuf::build)
@@ -3359,38 +3139,23 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     if (idx == nullptr) n = S->n_bitmaps;
     std::vector<uint32_t> ia(n), ib(n, 0);
     for (size_t i = 0; i < n; i++) ia[i] = idx ? idx[i] : (uint32_t)i;
-    std::vector<uint8_t> blob;
     // roaring.c:2292 (open range empty / start past the 32-bit universe) and :2303 (the CLOSED
-    // range, after the reference's truncation of both ends to 32 bits, is empty): plain copy
+    // range, after the reference's truncation of both ends to 32 bits, is empty): plain copy, the
+    // symmetric difference with the empty bitmap
     const bool noop = range_start >= range_end || range_start > (uint64_t)UINT32_MAX + 1 ||
                       (uint32_t)range_start > (uint32_t)(range_end - 1);
-    if (noop) {  // copy: symmetric difference with the empty bitmap
-        const uint32_t hdr[2] = {SERIAL_COOKIE_NO_RUN, 0};
-        blob.assign((const uint8_t *)hdr, (const uint8_t *)hdr + 8);
-    } else {
-        const uint32_t first = (uint32_t)range_start, last = (uint32_t)(range_end - 1);
-        const uint32_t hb0 = first >> 16, hb1 = last >> 16, nk = hb1 - hb0 + 1;
-        const size_t nfb = (nk + 7) / 8, hdr = 4 + nfb + 4 * (size_t)nk + (nk >= (uint32_t)NO_OFFSET_THRESHOLD ? 4 * (size_t)nk : 0);
-        blob.assign(hdr + 6 * (size_t)nk, 0);
-        const uint32_t cookie = SERIAL_COOKIE | ((nk - 1) << 16);
-        memcpy(blob.data(), &cookie, 4);
-        memset(blob.data() + 4, 0xFF, nfb);  // every container is a run
-        if (nk & 7) blob[4 + nfb - 1] = (uint8_t)((1u << (nk & 7)) - 1);
-        uint8_t *kc = blob.data() + 4 + nfb, *offs = kc + 4 * (size_t)nk, *pay = blob.data() + hdr;
-        for (uint32_t k = 0; k < nk; k++) {
-            const uint32_t hb = hb0 + k, lo = hb == hb0 ? (first & 0xFFFF) : 0, hi = hb == hb1 ? (last & 0xFFFF) : 0xFFFF;
-            const uint16_t key = (uint16_t)hb, cm1 = (uint16_t)(hi - lo), one = 1, v0 = (uint16_t)lo;
-            memcpy(kc + 4 * (size_t)k, &key, 2);
-            memcpy(kc + 4 * (size_t)k + 2, &cm1, 2);
-            if (nk >= (uint32_t)NO_OFFSET_THRESHOLD) {
-                const uint32_t o = (uint32_t)(hdr + 6 * (size_t)k);
-                memcpy(offs + 4 * (size_t)k, &o, 4);
-            }
-            memcpy(pay + 6 * (size_t)k, &one, 2);
-            memcpy(pay + 6 * (size_t)k + 2, &v0, 2);
-            memcpy(pay + 6 * (size_t)k + 4, &cm1, 2);
-        }
+    const uint32_t first = (uint32_t)range_start, last = (uint32_t)(range_end - 1);
+    const uint32_t hb0 = first >> 16, hb1 = last >> 16, nk = noop ? 0 : hb1 - hb0 + 1;
+    std::vector<rle16_t> runs(nk);   // one run {lo, hi - lo} per key
+    for (uint32_t k = 0; k < nk; k++) {
+        const uint32_t hb = hb0 + k, lo = hb == hb0 ? (first & 0xFFFF) : 0, hi = hb == hb1 ? (last & 0xFFFF) : 0xFFFF;
+        runs[k] = rle16_t{(uint16_t)lo, (uint16_t)(hi - lo)};
     }
+    const auto range = [&](uint32_t k) {
+        return PortableEntry{(uint16_t)(hb0 + k), T_RUN, runs[k].length + 1u, 1, (const uint8_t *)&runs[k]};
+    };
+    std::vector<uint8_t> blob(portable_size(nk, range));
+    write_portable(blob.data(), nk, range);
     const char *bp = (const char *)blob.data();
     const size_t bl = blob.size();
     SetPtr Rg(upload_blobs_impl(&bp, &bl, 1, false));
@@ -3442,44 +3207,6 @@ struct rb200_set64 {
 extern "C" {
 namespace {
 struct R64Bucket { uint32_t high; const char *ptr; size_t len; };
-// length of the 32-bit portable bitmap starting at buf (0 = malformed); header walk only
-size_t portable_length(const uint8_t *buf, size_t maxlen) {
-    if (maxlen < 4) return 0;
-    uint32_t cookie;
-    memcpy(&cookie, buf, 4);
-    size_t pos = 4, size;
-    const uint8_t *runflags = nullptr;
-    if ((cookie & 0xFFFF) == SERIAL_COOKIE) {
-        size = (cookie >> 16) + 1;
-        runflags = buf + 4;
-        pos += (size + 7) / 8;
-    } else if (cookie == SERIAL_COOKIE_NO_RUN && maxlen >= 8) {
-        uint32_t sz;
-        memcpy(&sz, buf + 4, 4);
-        size = sz;
-        pos = 8;
-    } else {
-        return 0;
-    }
-    if (size > 65536 || pos + 4 * size > maxlen) return 0;
-    const uint8_t *kc = buf + pos;
-    pos += 4 * size;
-    if (!runflags || size >= (size_t)NO_OFFSET_THRESHOLD) pos += 4 * size;
-    for (size_t i = 0; i < size; i++) {
-        uint16_t cm1;
-        memcpy(&cm1, kc + 4 * i + 2, 2);
-        if (runflags && ((runflags[i / 8] >> (i % 8)) & 1)) {
-            if (pos + 2 > maxlen) return 0;
-            uint16_t nr;
-            memcpy(&nr, buf + pos, 2);
-            pos += 2 + 4 * (size_t)nr;
-        } else {
-            pos += (uint32_t)cm1 + 1 > (uint32_t)MAX_ARRAY ? (size_t)BITSET_BYTES : 2 * ((size_t)cm1 + 1);
-        }
-        if (pos > maxlen) return 0;
-    }
-    return pos;
-}
 // The bucket headers of one 64-bit portable blob (roaring64.c:2440-2531); nullptr when they are
 // well formed, else what is wrong.  The buckets' contents are checked by the device parse.
 const char *parse_r64(const char *buf, size_t len, std::vector<R64Bucket> &out) {
@@ -3496,7 +3223,7 @@ const char *parse_r64(const char *buf, size_t len, std::vector<R64Bucket> &out) 
         pos += 4;
         if (i && b.high <= out.back().high) return "the high 32 bits of the buckets are not strictly increasing";
         b.ptr = buf + pos;
-        b.len = portable_length((const uint8_t *)buf + pos, len - pos);
+        b.len = walk_portable((const uint8_t *)buf + pos, len - pos, [](const PortableEntry &) {});
         if (!b.len) return "a bucket runs past the end of the blob or is not a 32-bit portable bitmap";
         pos += b.len;
         out.push_back(b);
@@ -3551,9 +3278,9 @@ rb200_set64 *set64_upload_impl(const char *const *bufs, const size_t *lens, size
         }
         if (ptrs.size() >= 0xffffffffull) { t_err = "set64: more than 2^32 - 2 buckets"; return nullptr; }
     }
-    static const uint32_t empty_blob[2] = {SERIAL_COOKIE_NO_RUN, 0};
+    uint8_t empty_blob[8];
+    blens.push_back(write_portable(empty_blob, 0, [](uint32_t) { return PortableEntry{}; }));
     ptrs.push_back((const char *)empty_blob);
-    blens.push_back(8);
     highs.push_back(0);
     if (!ctx_init()) return nullptr;
     Set64Ptr s = set64_new((uint32_t)n, (uint32_t)ptrs.size());

@@ -325,12 +325,6 @@ k_card_items(SetView A, SetView B, Items it, uint64_t W, OpStats *st) {
 }
 
 // ------------------------------------------------------------------------------ finalize
-// header bytes of the portable format (roaring_array.c:469-500)
-__device__ __forceinline__ uint32_t portable_header_bytes(uint32_t n, bool hasrun) {
-    if (!hasrun) return 8u + 8u * n;
-    return 4u + ((n + 7u) >> 3) + (n < 4u ? 4u * n : 8u * n);
-}
-
 #ifndef RB200_FIN_BLOCKS
 #define RB200_FIN_BLOCKS 16
 #endif
@@ -721,11 +715,6 @@ void launch_pack_copy(const SetView &S, uint32_t n, int elide, const uint64_t *o
 // so results can leave the device as bytes — one D2H, no per-container host allocation.
 namespace rb200 {
 
-__device__ __forceinline__ uint32_t ser_header_bytes(uint32_t n, bool hasrun) {
-    if (!hasrun) return 8u + 8u * n;
-    return 4u + ((n + 7u) >> 3) + (n < 4u ? 4u * n : 8u * n);
-}
-
 __global__ void __launch_bounds__(128)
 k_ser_measure(SetView S, uint32_t n, uint64_t *__restrict__ sizes16, uint32_t *__restrict__ exact,
               uint32_t *__restrict__ hasrun_out) {
@@ -743,7 +732,7 @@ k_ser_measure(SetView S, uint32_t n, uint64_t *__restrict__ sizes16, uint32_t *_
         bytes = __reduce_add_sync(FULLMASK, bytes);
         anyrun = __reduce_or_sync(FULLMASK, anyrun);
         if (lane == 0) {
-            const uint32_t tot = ser_header_bytes(nc, anyrun != 0) + bytes;
+            const uint32_t tot = portable_header_bytes(nc, anyrun != 0) + bytes;
             exact[b] = tot;
             sizes16[b] = (uint64_t)round16(tot);
             hasrun_out[b] = anyrun;
@@ -792,10 +781,10 @@ k_ser_write(SetView S, uint32_t n, const uint64_t *__restrict__ off, const uint3
         const uint32_t c0 = S.bm_beg[b], nc = S.bm_cnt[b];
         const bool hasrun = hasrun_in[b] != 0;
         uint8_t *o = dst + off[b];
-        const uint32_t hdr = ser_header_bytes(nc, hasrun);
+        const uint32_t hdr = portable_header_bytes(nc, hasrun);
         uint8_t *kc, *offs = nullptr;
         if (hasrun) {
-            if (lane == 0) store_u32(o, 12347u | ((nc - 1) << 16));  // SERIAL_COOKIE, roaring_array.h:35-40
+            if (lane == 0) store_u32(o, SERIAL_COOKIE | ((nc - 1) << 16));
             const uint32_t nfb = (nc + 7) >> 3;
             for (uint32_t j = lane; j < nfb; j += 32) {
                 uint32_t byte = 0;
@@ -804,9 +793,9 @@ k_ser_write(SetView S, uint32_t n, const uint64_t *__restrict__ off, const uint3
                 o[4 + j] = (uint8_t)byte;
             }
             kc = o + 4 + nfb;
-            if (nc >= 4) offs = kc + 4 * nc;  // NO_OFFSET_THRESHOLD
+            if (nc >= NO_OFFSET_THRESHOLD) offs = kc + 4 * nc;
         } else {
-            if (lane == 0) { store_u32(o, 12346u); store_u32(o + 4, nc); }
+            if (lane == 0) { store_u32(o, SERIAL_COOKIE_NO_RUN); store_u32(o + 4, nc); }
             kc = o + 8;
             offs = kc + 4 * nc;
         }
@@ -971,12 +960,12 @@ k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
         const uint8_t *runflags = nullptr;
         if (!bad) {
             const uint32_t cookie = ld_u32(buf);
-            if ((cookie & 0xFFFFu) == 12347u) {          // SERIAL_COOKIE, roaring_array.h:35-40
+            if ((cookie & 0xFFFFu) == SERIAL_COOKIE) {
                 size = (cookie >> 16) + 1;
                 hasrun = true;
                 runflags = buf + 4;
                 pos = 4 + ((size + 7) >> 3);
-            } else if (cookie == 12346u && len >= 8) {   // SERIAL_COOKIE_NO_RUN
+            } else if (cookie == SERIAL_COOKIE_NO_RUN && len >= 8) {
                 size = ld_u32(buf + 4);
                 pos = 8;
             } else {
@@ -987,7 +976,7 @@ k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
         const uint8_t *kc = buf + pos;
         if (!bad) {
             pos += 4ull * size;
-            if (!hasrun || size >= 4u) pos += 4ull * size;   // offset header (NO_OFFSET_THRESHOLD), not trusted
+            if (!hasrun || size >= NO_OFFSET_THRESHOLD) pos += 4ull * size;   // offset header, not trusted
         }
         uint64_t off = slab_base[b];
         int prev_key = -1;
@@ -1112,9 +1101,8 @@ __global__ void k_deser_bitmap_cards(SetOut out, uint32_t nb, const OpStats *st)
 // ------------------------------------------------------------------------------ frozen format
 // roaring_bitmap_frozen_serialize / roaring_bitmap_frozen_view (src/roaring.c:3180-3456): zones
 // [bitset words | runs | array values | keys u16 | counts u16 | typecodes u8 | header u32], the
-// header LAST: (n_containers << 15) | FROZEN_COOKIE (13766).  counts = cardinality-1 (bitset,
-// array) or n_runs (run).  Blob starts are 32-byte aligned so frozen_view accepts them in place.
-constexpr uint32_t FROZEN_COOKIE = 13766u;
+// header LAST: (n_containers << 15) | FROZEN_COOKIE.  counts = cardinality-1 (bitset, array) or
+// n_runs (run).  Blob starts are 32-byte aligned so frozen_view accepts them in place.
 
 __global__ void __launch_bounds__(128)
 k_frozen_measure(SetView S, uint32_t n, uint64_t *__restrict__ sizes32, uint32_t *__restrict__ exact,

@@ -23,6 +23,7 @@
 #include "../../include/roaring_b200.h"
 #include "rb200_common.h"
 #include "rb200_internal.h"
+#include "rb200_portable.h"
 
 #define RB_API extern "C" __attribute__((visibility("default")))
 
@@ -150,109 +151,15 @@ RB_API void rb200_comm_destroy(rb200_comm_t *c) {
 // =================================================================== host-side blob algebra
 namespace {
 
-constexpr uint32_t COOKIE_NO_RUN = 12346, COOKIE_RUN = 12347;   // roaring_array.h:35-40
-constexpr int NO_OFFSET_THRESHOLD_ = 4;
+using rb200::PortableEntry;
 
-// header-level view: keys, cardinalities, run flags, payload spans (run sizes are read from the
-// payload: the walk is sequential).  false = malformed.
-struct BlobIndex {
-    uint32_t n = 0;
-    bool hasrun = false;
-    std::vector<uint16_t> key, cm1;
-    std::vector<uint8_t> isrun;
-    std::vector<uint64_t> start;
-    std::vector<uint32_t> size;
-};
-
-bool index_blob(const uint8_t *buf, size_t len, BlobIndex &ix) {
-    if (len < 4) return false;
-    uint32_t cookie;
-    memcpy(&cookie, buf, 4);
-    size_t pos = 4;
-    const uint8_t *flags = nullptr;
-    if ((cookie & 0xFFFF) == COOKIE_RUN) {
-        ix.n = (cookie >> 16) + 1;
-        ix.hasrun = true;
-        flags = buf + 4;
-        pos = 4 + (ix.n + 7) / 8;
-    } else if (cookie == COOKIE_NO_RUN && len >= 8) {
-        memcpy(&ix.n, buf + 4, 4);
-        pos = 8;
-    } else {
-        return false;
-    }
-    const uint32_t n = ix.n;
-    if (n > 65536 || pos + 4ull * n > len) return false;
-    const uint8_t *kc = buf + pos;
-    pos += 4ull * n;
-    if (!ix.hasrun || n >= (uint32_t)NO_OFFSET_THRESHOLD_) pos += 4ull * n;
-    ix.key.resize(n); ix.cm1.resize(n); ix.isrun.resize(n); ix.start.resize(n); ix.size.resize(n);
-    for (uint32_t i = 0; i < n; i++) {
-        memcpy(&ix.key[i], kc + 4 * i, 2);
-        memcpy(&ix.cm1[i], kc + 4 * i + 2, 2);
-        if (i && ix.key[i] <= ix.key[i - 1]) return false;
-        const bool r = ix.hasrun && ((flags[i >> 3] >> (i & 7)) & 1);
-        ix.isrun[i] = r;
-        uint32_t sz;
-        if (r) {
-            if (pos + 2 > len) return false;
-            uint16_t nr;
-            memcpy(&nr, buf + pos, 2);
-            sz = 2u + 4u * nr;
-        } else {
-            const uint32_t card = (uint32_t)ix.cm1[i] + 1;
-            sz = card > 4096u ? 8192u : 2u * card;
-        }
-        if (pos + sz > len) return false;
-        ix.start[i] = pos;
-        ix.size[i] = sz;
-        pos += sz;
-    }
-    return true;
-}
-
-// serialize containers [i0, i1) of several indexed blobs (in order) as ONE portable bitmap
-struct Piece { const uint8_t *buf; const BlobIndex *ix; uint32_t i0, i1; };
-
-bool build_blob(const std::vector<Piece> &pieces, char **out, size_t *outlen) {
-    uint32_t n = 0;
-    bool hasrun = false;
-    uint64_t payload = 0;
-    for (const Piece &p : pieces)
-        for (uint32_t i = p.i0; i < p.i1; i++) {
-            n++;
-            hasrun |= p.ix->isrun[i] != 0;
-            payload += p.ix->size[i];
-        }
-    const size_t hdr = hasrun ? 4 + (n + 7) / 8 + (n < (uint32_t)NO_OFFSET_THRESHOLD_ ? 4ull : 8ull) * n : 8 + 8ull * n;
-    uint8_t *o = (uint8_t *)malloc(hdr + payload + 16);
+// the containers as ONE malloc'd portable bitmap
+bool write_blob(const std::vector<PortableEntry> &c, char **out, size_t *outlen) {
+    const auto at = [&c](uint32_t i) { return c[i]; };
+    uint8_t *o = (uint8_t *)malloc(rb200::portable_size((uint32_t)c.size(), at));
     if (!o) return false;
-    memset(o, 0, hdr);
-    uint8_t *kc, *offs = nullptr;
-    if (hasrun) {
-        const uint32_t cookie = COOKIE_RUN | ((n - 1) << 16);
-        memcpy(o, &cookie, 4);
-        kc = o + 4 + (n + 7) / 8;
-        if (n >= (uint32_t)NO_OFFSET_THRESHOLD_) offs = kc + 4ull * n;
-    } else {
-        memcpy(o, &COOKIE_NO_RUN, 4);
-        memcpy(o + 4, &n, 4);
-        kc = o + 8;
-        offs = kc + 4ull * n;
-    }
-    uint64_t pos = hdr;
-    uint32_t k = 0;
-    for (const Piece &p : pieces)
-        for (uint32_t i = p.i0; i < p.i1; i++, k++) {
-            memcpy(kc + 4ull * k, &p.ix->key[i], 2);
-            memcpy(kc + 4ull * k + 2, &p.ix->cm1[i], 2);
-            if (p.ix->isrun[i]) o[4 + (k >> 3)] |= (uint8_t)(1u << (k & 7));
-            if (offs) { const uint32_t o32 = (uint32_t)pos; memcpy(offs + 4ull * k, &o32, 4); }
-            memcpy(o + pos, p.buf + p.ix->start[i], p.ix->size[i]);
-            pos += p.ix->size[i];
-        }
+    *outlen = rb200::write_portable(o, (uint32_t)c.size(), at);
     *out = (char *)o;
-    *outlen = (size_t)pos;
     return true;
 }
 
@@ -269,18 +176,17 @@ RB_API int rb200_plan_key_ranges(const char *const *bufs, const size_t *lens, si
     uint32_t first = 65536, last = 0;
     bool any = false;
     for (size_t b = 0; b < n; b++) {
-        BlobIndex ix;
-        if (!index_blob((const uint8_t *)bufs[b], lens[b], ix)) {
-            rb200::set_error("plan_key_ranges: malformed portable bitmap at index " + std::to_string(b));
-            return -1;
-        }
         // weight of a container = its bytes + a fixed per-container cost (k_or_many2 on config 3: a
         // container costs about as much as 0.5 KiB of payload)
-        for (uint32_t i = 0; i < ix.n; i++) hist[ix.key[i]] += (uint64_t)ix.size[i] + 512;
-        if (ix.n) {
+        const auto weigh = [&](const PortableEntry &e) {
+            hist[e.key] += (uint64_t)rb200::portable_bytes(e.type, e.len) + 512;
             any = true;
-            if (ix.key[0] < first) first = ix.key[0];
-            if (ix.key[ix.n - 1] > last) last = ix.key[ix.n - 1];
+            if (e.key < first) first = e.key;
+            if (e.key > last) last = e.key;
+        };
+        if (!rb200::walk_portable((const uint8_t *)bufs[b], lens[b], weigh)) {
+            rb200::set_error("plan_key_ranges: malformed portable bitmap at index " + std::to_string(b));
+            return -1;
         }
     }
     uint64_t total = 0;
@@ -315,33 +221,28 @@ RB_API int rb200_plan_key_ranges(const char *const *bufs, const size_t *lens, si
 // blob; release with rb200_blob_free).
 RB_API int rb200_blob_slice_keys(const char *buf, size_t len, uint32_t key_lo, uint32_t key_hi, char **out,
                                  size_t *outlen) {
-    BlobIndex ix;
-    if (!index_blob((const uint8_t *)buf, len, ix)) { rb200::set_error("blob_slice_keys: malformed portable bitmap"); return -1; }
-    uint32_t i0 = 0, i1 = ix.n;
-    while (i0 < ix.n && ix.key[i0] < key_lo) i0++;
-    while (i1 > i0 && ix.key[i1 - 1] > key_hi) i1--;
-    std::vector<Piece> p{Piece{(const uint8_t *)buf, &ix, i0, i1}};
-    if (!build_blob(p, out, outlen)) { rb200::set_error("blob_slice_keys: out of memory"); return -1; }
+    std::vector<PortableEntry> c;
+    const auto keep = [&](const PortableEntry &e) { if (e.key >= key_lo && e.key <= key_hi) c.push_back(e); };
+    if (!rb200::walk_portable((const uint8_t *)buf, len, keep)) { rb200::set_error("blob_slice_keys: malformed portable bitmap"); return -1; }
+    if (!write_blob(c, out, outlen)) { rb200::set_error("blob_slice_keys: out of memory"); return -1; }
     return 0;
 }
 
 // Concatenation of bitmaps living on disjoint, increasing key ranges (per-rank results in rank order).
 RB_API int rb200_blobs_concat(const char *const *bufs, const size_t *lens, size_t n, char **out, size_t *outlen) {
-    std::vector<BlobIndex> ix(n);
-    std::vector<Piece> pieces;
-    int last = -1;
+    std::vector<PortableEntry> c;
     for (size_t b = 0; b < n; b++) {
-        if (!index_blob((const uint8_t *)bufs[b], lens[b], ix[b])) {
+        const size_t c0 = c.size();
+        if (!rb200::walk_portable((const uint8_t *)bufs[b], lens[b], [&c](const PortableEntry &e) { c.push_back(e); })) {
             rb200::set_error("blobs_concat: malformed portable bitmap at index " + std::to_string(b));
             return -1;
         }
-        if (ix[b].n) {
-            if ((int)ix[b].key[0] <= last) { rb200::set_error("blobs_concat: shards are not on increasing disjoint key ranges"); return -1; }
-            last = ix[b].key[ix[b].n - 1];
+        if (c0 && c.size() > c0 && c[c0].key <= c[c0 - 1].key) {
+            rb200::set_error("blobs_concat: shards are not on increasing disjoint key ranges");
+            return -1;
         }
-        pieces.push_back(Piece{(const uint8_t *)bufs[b], &ix[b], 0, ix[b].n});
     }
-    if (!build_blob(pieces, out, outlen)) { rb200::set_error("blobs_concat: out of memory"); return -1; }
+    if (!write_blob(c, out, outlen)) { rb200::set_error("blobs_concat: out of memory"); return -1; }
     return 0;
 }
 

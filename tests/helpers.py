@@ -1,9 +1,14 @@
 """Shared helpers for the parity tests."""
 import hashlib
+import os
+import subprocess
+import tempfile
 
 import numpy as np
 
 import synth
+
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "croaring_b200", "csrc")
 
 DATASETS = ["census1881", "weather_sept_85", "wikileaks-noquotes",
             "census1881_srt", "wikileaks-noquotes_srt", "uscensus2000"]
@@ -21,6 +26,19 @@ def synth_blobs(R, seed, n, key_space=10, max_keys=9, profiles=None):
         blobs.append(R.serialize(r))
         R.free(r)
     return blobs
+
+
+def run_probe(src, *args):
+    """Compile a host-side probe against the library's headers with nvcc and run it with args.
+    nvcc runs without LD_PRELOAD (it crashes with a preloaded sanitizer runtime); the probe keeps it."""
+    with tempfile.TemporaryDirectory() as td:
+        cu = os.path.join(td, "probe.cu")
+        open(cu, "w").write(src)
+        exe = os.path.join(td, "probe")
+        env = {k: v for k, v in os.environ.items() if k != "LD_PRELOAD"}
+        subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-std=c++17", "--expt-relaxed-constexpr",
+                               "-gencode", "arch=compute_90a,code=sm_90a", "-I", CSRC, cu, "-o", exe], env=env)
+        return subprocess.run([exe, *args], capture_output=True, text=True)
 
 
 def no_run_twins(R, blobs):

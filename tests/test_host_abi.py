@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import croaring_b200 as rb
-from helpers import synth_blobs
+from helpers import run_probe, synth_blobs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -97,21 +97,8 @@ int main() {
     return bad;
 }
 '''
-    out = _run_probe(src)
+    out = run_probe(src)
     assert out.returncode == 0, out.stdout
-
-
-def _run_probe(src):
-    """Compile a host-side probe against the library's headers with nvcc and run it."""
-    import tempfile
-    with tempfile.TemporaryDirectory() as td:
-        cu = os.path.join(td, "probe.cu")
-        open(cu, "w").write(src)
-        exe = os.path.join(td, "probe")
-        subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-std=c++17", "--expt-relaxed-constexpr",
-                               "-gencode", "arch=compute_90a,code=sm_90a",
-                               "-I", os.path.join(ROOT, "croaring_b200", "csrc"), cu, "-o", exe])
-        return subprocess.run([exe], capture_output=True, text=True)
 
 
 def test_many2_index_formats_round_trip():
@@ -182,7 +169,7 @@ int main() {
     return bad;
 }
 '''
-    out = _run_probe(src)
+    out = run_probe(src)
     assert out.returncode == 0, out.stdout
 
 
@@ -199,10 +186,10 @@ def test_compute_fails_loudly_without_gpu():
 
 
 def test_mutated_blobs_never_crash_the_host_parsers(R):
-    """Seeded mutation fuzz of the two host-side portable-format readers (rb200_host.cu parse_portable
-    behind rb200_bitmap_portable_deserialize_safe; rb200_shard.cu index_blob behind the blob algebra):
+    """Seeded mutation fuzz of the host-side portable-format entry points (walk_portable behind
+    rb200_bitmap_portable_deserialize_safe and behind the blob algebra of rb200_shard.cu):
     byte flips, truncations, garbage tails and splices must be either refused or handled
-    consistently — what one reader accepts the other slices, and accepted bytes re-serialize stably."""
+    consistently — what one entry point accepts the other slices, and accepted bytes re-serialize stably."""
     import random
     from croaring_b200 import sharding as sh
     rng = random.Random(20260923)

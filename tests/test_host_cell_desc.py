@@ -2,7 +2,7 @@
 is a host+device helper; every field survives packing and unpacking at its limits, compiled for the
 host with nvcc."""
 
-from test_host_abi import _run_probe
+from helpers import run_probe
 
 
 def test_cell_descriptor_round_trip():
@@ -61,5 +61,5 @@ int main() {
     return bad;
 }
 '''
-    out = _run_probe(src)
+    out = run_probe(src)
     assert out.returncode == 0, out.stdout

@@ -14,6 +14,13 @@ def _blob32(vals16, key=0):
     return struct.pack("<IIHHI", 12346, 1, key, n - 1, 16) + struct.pack(f"<{n}H", *vals16)
 
 
+def _blob32_keys(keys):
+    """A 32-bit portable blob (no run containers) of one-value array containers, keys as given."""
+    n = len(keys)
+    return (struct.pack("<II", 12346, n) + b"".join(struct.pack("<HH", k, 0) for k in keys)
+            + b"".join(struct.pack("<I", 8 + 8 * n + 2 * i) for i in range(n)) + struct.pack(f"<{n}H", *range(n)))
+
+
 def _blob64(buckets, count=None):
     """A 64-bit portable blob: u64 bucket count, then per bucket u32 high32 + 32-bit blob."""
     body = b"".join(struct.pack("<I", h) + b for h, b in buckets)
@@ -31,6 +38,8 @@ def test_malformed_blobs_refused_before_any_cuda_call():
         (good[:-1], "runs past the end of the blob"),
         (good[:14], "runs past the end of the blob"),
         (_blob64([(1, b"\x00" * 12)]), "not a 32-bit portable bitmap"),
+        (_blob64([(1, _blob32_keys([4, 4]))]), "not a 32-bit portable bitmap"),
+        (_blob64([(1, _blob32_keys([2, 6, 5]))]), "not a 32-bit portable bitmap"),
     ]
     for blob, why in cases:
         with pytest.raises(rb.RB200Error, match=why):
