@@ -33,17 +33,6 @@ constexpr int BUILD_THREADS = 256, BUILD_ITEMS = 8;
 constexpr uint64_t BUILD_TILE = (uint64_t)BUILD_THREADS * BUILD_ITEMS;
 constexpr int BUILD_WARPS = BUILD_THREADS / 32;
 
-static inline int build_sm_count() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
-
 // largest b in [lo, hi] with off[b] <= p (off[lo] <= p): the bitmap holding position p
 __device__ __forceinline__ uint32_t find_bitmap(const uint64_t *__restrict__ off, uint32_t lo, uint32_t hi,
                                                 uint64_t p) {
@@ -317,52 +306,43 @@ uint64_t build_tile_count(uint64_t N) { return build_tiles(N); }
 void launch_build_measure(const uint32_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
                           uint32_t *unsorted, cudaStream_t s) {
     if (!N) return;
-    k_build_measure<uint32_t><<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_cnt, unsorted);
-    g_launches++;
+    launch_kernel(k_build_measure<uint32_t>, build_tiles(N), BUILD_THREADS, 0, s, v, off, n, N, tile_cnt, unsorted);
 }
 
 void launch_build64_measure(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, uint64_t *tile_cnt,
                             uint32_t *unsorted, cudaStream_t s) {
     if (!N) return;
-    k_build_measure<uint64_t><<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_cnt, unsorted);
-    g_launches++;
+    launch_kernel(k_build_measure<uint64_t>, build_tiles(N), BUILD_THREADS, 0, s, v, off, n, N, tile_cnt, unsorted);
 }
 
 void launch_build64_split(const uint64_t *v, const uint64_t *off, uint32_t n, uint64_t N, const uint64_t *tile_base,
                           uint32_t *lo, uint64_t *b_pos, uint32_t *b_high, cudaStream_t s) {
     if (!N) return;
-    k_build64_split<<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_base, lo, b_pos, b_high);
-    g_launches++;
+    launch_kernel(k_build64_split, build_tiles(N), BUILD_THREADS, 0, s, v, off, n, N, tile_base, lo, b_pos, b_high);
 }
 
 void launch_build_emit(const uint32_t *v, const uint64_t *off, uint32_t n, uint64_t N, const uint64_t *tile_base,
                        uint16_t *c_key, uint64_t *c_pos, cudaStream_t s) {
     if (!N) return;
-    k_build_emit<<<build_tiles(N), BUILD_THREADS, 0, s>>>(v, off, n, N, tile_base, c_key, c_pos);
-    g_launches++;
+    launch_kernel(k_build_emit, build_tiles(N), BUILD_THREADS, 0, s, v, off, n, N, tile_base, c_key, c_pos);
 }
 
 void launch_build_slots(const uint64_t *c_pos, uint64_t nc, uint64_t N, uint64_t *slot, cudaStream_t s) {
     if (!nc) return;
-    k_build_slots<<<(uint32_t)((nc + 255) / 256), 256, 0, s>>>(c_pos, nc, N, slot);
-    g_launches++;
+    launch_kernel(k_build_slots, (uint32_t)((nc + 255) / 256), 256, 0, s, c_pos, nc, N, slot);
 }
 
 void launch_build_bitmaps(const uint64_t *off, uint32_t n, const uint64_t *c_pos, uint64_t nc, uint32_t *bm_beg,
                           uint32_t *bm_cnt, cudaStream_t s) {
     if (!n) return;
-    k_build_bitmaps<<<(n + 255) / 256, 256, 0, s>>>(off, n, c_pos, nc, bm_beg, bm_cnt);
-    g_launches++;
+    launch_kernel(k_build_bitmaps, (n + 255) / 256, 256, 0, s, off, n, c_pos, nc, bm_beg, bm_cnt);
 }
 
 void launch_build_write(const uint32_t *v, const uint64_t *c_pos, uint64_t nc, uint64_t N, SetOut out,
                         uint64_t slab_cap, OpStats *st, cudaStream_t s) {
     if (!nc) return;
-    uint64_t blocks = (nc + 3) / 4;
-    const uint64_t cap = (uint64_t)build_sm_count() * 6;   // 6 x 32 KiB of accumulators per SM
-    if (blocks > cap) blocks = cap;
-    k_build_write<<<(uint32_t)blocks, 128, 0, s>>>(v, c_pos, nc, N, out, slab_cap, st);
-    g_launches++;
+    // 6 x 32 KiB of accumulators per SM
+    launch_kernel(k_build_write, grid_for(nc, 4, 6), 128, 0, s, v, c_pos, nc, N, out, slab_cap, st);
 }
 
 // Exclusive sum of n u64 (n < 2^31).  temp == nullptr: *temp_bytes receives the scratch size.
@@ -378,10 +358,7 @@ bool build_scan(void *temp, size_t *temp_bytes, const uint64_t *in, uint64_t *ou
 template <typename T>
 static bool sort_chunk(void *temp, size_t *temp_bytes, const T *in, T *out, const uint64_t *off, uint64_t first,
                        uint64_t items, uint32_t nseg, int *rel, cudaStream_t s) {
-    if (temp) {
-        k_build_rel_offsets<<<(nseg + 256) / 256, 256, 0, s>>>(off, nseg, rel);
-        g_launches++;
-    }
+    if (temp) launch_kernel(k_build_rel_offsets, (nseg + 256) / 256, 256, 0, s, off, nseg, rel);
     const cudaError_t e = cub::DeviceSegmentedSort::SortKeys(temp, *temp_bytes, in + first, out + first, (int)items,
                                                              (int)nseg, rel, rel + 1, s);
     if (temp) g_launches++;

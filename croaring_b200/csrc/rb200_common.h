@@ -269,8 +269,28 @@ bool launch_pair_fused(int op, const uint8_t *d_in, uint8_t *out_mapped, uint32_
                        cudaStream_t s);
 
 
-// --- launch wrappers (rb200_kernels.cu); every wrapper bumps g_launches -----------------
+// --- launch wrappers ------------------------------------------------------------------------
+// g_launches: kernels launched so far (rb200_kernel_launches); launch_kernel counts each of its
+// launches, the cub calls of rb200_build.cu count their own.
+// g_sm_count: multiprocessor count of the library's device (rb200_init).
 extern unsigned long long g_launches;
+extern int g_sm_count;
+
+// Blocks for `units` work units at `per_block` units per block: at least one, at most
+// `blocks_per_sm` per multiprocessor.
+inline uint32_t grid_for(uint64_t units, uint64_t per_block, uint32_t blocks_per_sm) {
+    const uint64_t b = (units + per_block - 1) / per_block, cap = (uint64_t)g_sm_count * blocks_per_sm;
+    return (uint32_t)(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
+#ifdef __CUDACC__
+template <typename... Params, typename... Args>
+inline void launch_kernel(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                          Args... args) {
+    kernel<<<grid, block, smem, s>>>(args...);
+    g_launches++;
+}
+#endif
 
 void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, const uint32_t *ib,
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
@@ -304,10 +324,12 @@ void launch_many_compact(const uint32_t *flags, uint16_t *keys_out, OpStats *st,
 // or_many: key-major index, then one pass over the payloads (rb200_many2.cu)
 void launch_or_many2(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t key_lo, uint32_t key_hi,
                      const Many2Index &ix, uint32_t max_units, uint32_t *scratch, uint32_t *tickets,
-                     uint32_t scratch_slots, SetOut out, uint32_t *card_per_key, OpStats *st, int sms,
-                     cudaStream_t s, cudaEvent_t ev_kernel_start, bool use_tma, bool window_index, uint32_t *cnt_tab);
+                     uint32_t scratch_slots, SetOut out, uint32_t *card_per_key, OpStats *st, cudaStream_t s,
+                     cudaEvent_t ev_kernel_start, bool use_tma, bool window_index, uint32_t *cnt_tab);
 constexpr uint32_t M2W_MAX_CHUNKS = 64;   // key-window index build: chunks of 256 input bitmaps per window
 
+// exclusive scan of bytes[0, n) into off (n + 1 entries: the last is the total), and of cnts into
+// beg the same way when cnts is not null
 void launch_pack_scan(const uint64_t *bytes, const uint32_t *cnts, uint32_t n, uint64_t *off,
                       uint64_t *beg, cudaStream_t s);
 void launch_serialize_measure(const SetView &S, uint32_t n, uint64_t *sizes16, uint32_t *exact,
@@ -328,8 +350,8 @@ void launch_frozen_write(const SetView &S, uint32_t n, uint64_t nc, const uint64
                          uint64_t *c_dst, cudaStream_t s);
 void launch_run_optimize(const SetView &S, uint32_t nb, uint64_t nc, int mode, SetOut out, OpStats *st,
                          cudaStream_t s);
-void launch_values_measure(const SetView &S, uint32_t nb, uint64_t *bm_vals, uint32_t *dummy,
-                           uint64_t *c_start, uint32_t *c_bitmap, cudaStream_t s);
+void launch_values_measure(const SetView &S, uint32_t nb, uint64_t *bm_vals, uint64_t *c_start,
+                           uint32_t *c_bitmap, cudaStream_t s);
 void launch_values_write(const SetView &S, uint32_t nb, const uint64_t *bm_off, const uint64_t *c_start,
                          const uint32_t *c_bitmap, uint64_t nc, uint32_t *out, cudaStream_t s);
 // per bitmap of a produced set: bm_card, bm_bytes, bm_ebytes from its container directory
@@ -370,6 +392,6 @@ void launch_r64_ser_layout(const uint32_t *b_beg, const uint32_t *b_cnt, const u
 
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
                      uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
-                     int sms, cudaStream_t s);
+                     cudaStream_t s);
 
 }  // namespace rb200

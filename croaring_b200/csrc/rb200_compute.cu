@@ -12,19 +12,6 @@
 
 namespace rb200 {
 
-extern unsigned long long g_launches;
-
-static inline int sm_count() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
-
 #ifndef RB200_CI_MINBLOCKS
 #define RB200_CI_MINBLOCKS 6   // resident CTAs per SM the register allocation is held to (6 = what the 36 KiB of shared memory allow)
 #endif
@@ -242,21 +229,13 @@ void launch_compute_items(const SetView &A, const SetView &B, Items it, uint64_t
                           uint8_t *slab, uint64_t slab_cap, OpStats *st, int rules, int copy_ticket,
                           cudaStream_t s) {
     if (!W) return;
-    const uint64_t b = (W + 3) / 4;   // a warp per unit, 4 per block, at most 6 resident blocks per SM
-    const uint32_t g = (uint32_t)(b < (uint64_t)sm_count() * 6 ? b : (uint64_t)sm_count() * 6);
-    switch (op) {
-        case OP_AND: k_compute_items<OP_AND, false><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket); break;
-        case OP_OR:
-            if (rules & RULES_LAZY) k_compute_items<OP_OR, true><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
-            else k_compute_items<OP_OR, false><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
-            break;
-        case OP_XOR:
-            if (rules & RULES_LAZY) k_compute_items<OP_XOR, true><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
-            else k_compute_items<OP_XOR, false><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
-            break;
-        default: k_compute_items<OP_ANDNOT, false><<<g, 128, 0, s>>>(A, B, it, W, slab, slab_cap, st, rules, copy_ticket); break;
-    }
-    g_launches++;
+    const bool lazy = (rules & RULES_LAZY) != 0;
+    auto *k = op == OP_AND  ? k_compute_items<OP_AND, false>
+            : op == OP_OR   ? (lazy ? k_compute_items<OP_OR, true> : k_compute_items<OP_OR, false>)
+            : op == OP_XOR  ? (lazy ? k_compute_items<OP_XOR, true> : k_compute_items<OP_XOR, false>)
+                            : k_compute_items<OP_ANDNOT, false>;
+    // a warp per unit, 4 per block, at most 6 resident blocks per SM
+    launch_kernel(k, grid_for(W, 4, 6), 128, 0, s, A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
 }
 
 }  // namespace rb200

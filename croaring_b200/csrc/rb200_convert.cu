@@ -11,17 +11,6 @@
 
 namespace rb200 {
 
-static inline int conv_sm_count() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
-
 // number of maximal runs of a bitset container held in global memory
 __device__ __forceinline__ int bitset_nruns_global(const uint8_t *p, int lane) {
     const uint32_t *w = reinterpret_cast<const uint32_t *>(p);
@@ -113,25 +102,15 @@ __global__ void k_copy_bitmap_dir(SetView S, uint32_t nb, SetOut out) {
 
 void launch_run_optimize(const SetView &S, uint32_t nb, uint64_t nc, int mode, SetOut out, OpStats *st,
                          cudaStream_t s) {
-    if (nb) {
-        k_copy_bitmap_dir<<<(nb + 127) / 128, 128, 0, s>>>(S, nb, out);
-        g_launches++;
-    }
-    if (nc) {
-        uint64_t blocks = (nc + 3) / 4;
-        const uint64_t cap = (uint64_t)conv_sm_count() * 6;
-        if (blocks > cap) blocks = cap;
-        k_run_optimize<<<(uint32_t)blocks, 128, 0, s>>>(S, nc, mode, out, st);
-        g_launches++;
-    }
+    if (nb) launch_kernel(k_copy_bitmap_dir, (nb + 127) / 128, 128, 0, s, S, nb, out);
+    if (nc) launch_kernel(k_run_optimize, grid_for(nc, 4, 6), 128, 0, s, S, nc, mode, out, st);
 }
 
 // ------------------------------------------------------------------------------ to_uint32_array
 // per bitmap: cardinality (for the caller's exclusive scan) ; per container: start index of its
 // values inside the bitmap's output range
 __global__ void __launch_bounds__(128)
-k_values_measure(SetView S, uint32_t nb, uint64_t *__restrict__ bm_vals, uint32_t *__restrict__ dummy,
-                 uint64_t *__restrict__ c_start) {
+k_values_measure(SetView S, uint32_t nb, uint64_t *__restrict__ bm_vals, uint64_t *__restrict__ c_start) {
     const int lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -141,18 +120,11 @@ k_values_measure(SetView S, uint32_t nb, uint64_t *__restrict__ bm_vals, uint32_
         for (uint32_t i0 = 0; i0 < n; i0 += 32) {
             const uint32_t i = i0 + lane;
             const uint32_t cd = i < n ? S.c_card[c0 + i] : 0u;
-            unsigned long long incl = cd;
-            for (int d = 1; d < 32; d <<= 1) {
-                const unsigned long long tv = __shfl_up_sync(FULLMASK, incl, d);
-                if (lane >= d) incl += tv;
-            }
-            if (i < n) c_start[c0 + i] = run + incl - cd;
+            const unsigned long long incl = warp_incl_scan((unsigned long long)cd, lane);
+            if (i < n) c_start[(uint64_t)c0 + i] = run + incl - cd;
             run += __shfl_sync(FULLMASK, incl, 31);
         }
-        if (lane == 0) {
-            bm_vals[b] = run;
-            dummy[b] = 0;
-        }
+        if (lane == 0) bm_vals[b] = run;
     }
 }
 
@@ -228,25 +200,18 @@ __global__ void k_container_bitmap(SetView S, uint32_t nb, uint32_t *__restrict_
     }
 }
 
-void launch_values_measure(const SetView &S, uint32_t nb, uint64_t *bm_vals, uint32_t *dummy,
-                           uint64_t *c_start, uint32_t *c_bitmap, cudaStream_t s) {
+void launch_values_measure(const SetView &S, uint32_t nb, uint64_t *bm_vals, uint64_t *c_start,
+                           uint32_t *c_bitmap, cudaStream_t s) {
     if (!nb) return;
-    uint32_t g = (nb + 3) / 4;
-    const uint32_t cap = (uint32_t)conv_sm_count() * 16;
-    if (g > cap) g = cap;
-    k_values_measure<<<g, 128, 0, s>>>(S, nb, bm_vals, dummy, c_start);
-    k_container_bitmap<<<g, 128, 0, s>>>(S, nb, c_bitmap);
-    g_launches += 2;
+    const uint32_t g = grid_for(nb, 4, 16);
+    launch_kernel(k_values_measure, g, 128, 0, s, S, nb, bm_vals, c_start);
+    launch_kernel(k_container_bitmap, g, 128, 0, s, S, nb, c_bitmap);
 }
 
 void launch_values_write(const SetView &S, uint32_t nb, const uint64_t *bm_off, const uint64_t *c_start,
                          const uint32_t *c_bitmap, uint64_t nc, uint32_t *out, cudaStream_t s) {
     if (!nc) return;
-    uint64_t blocks = (nc + 3) / 4;
-    const uint64_t cap = (uint64_t)conv_sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    k_values_write<<<(uint32_t)blocks, 128, 0, s>>>(S, nb, bm_off, c_start, c_bitmap, nc, out);
-    g_launches++;
+    launch_kernel(k_values_write, grid_for(nc, 4, 16), 128, 0, s, S, nb, bm_off, c_start, c_bitmap, nc, out);
 }
 
 }  // namespace rb200

@@ -41,6 +41,61 @@ __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, int lane) {
     }
     return v;
 }
+__device__ __forceinline__ unsigned long long warp_incl_scan(unsigned long long v, int lane) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const unsigned long long t = __shfl_up_sync(FULLMASK, v, d);
+        if (lane >= d) v += t;
+    }
+    return v;
+}
+
+// sum over the warp, in every lane (__reduce_add_sync covers 32-bit values only)
+__device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(FULLMASK, v, d);
+    return v;
+}
+
+// Exclusive scan of v over a block of NT threads; *total receives the block's sum in every thread.
+// s: NT / 32 words of shared memory.  Every thread of the block must call it; it synchronises the
+// block, also before it returns, so s can be reused right away.
+template <int NT, typename T>
+__device__ __forceinline__ T block_excl_scan(T v, T *s, T *total) {
+    constexpr int NW = NT / 32;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const T incl = warp_incl_scan(v, lane);
+    if (lane == 31) s[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+        const T x = warp_incl_scan(lane < NW ? s[lane] : (T)0, lane);
+        if (lane < NW) s[lane] = x;   // inclusive over the warps
+    }
+    __syncthreads();
+    const T r = (wid ? s[wid - 1] : (T)0) + incl - v;
+    *total = s[NW - 1];
+    __syncthreads();
+    return r;
+}
+
+// first position in the sorted a[0, n) whose value is >= key (lower) / > key (upper)
+__device__ __forceinline__ uint32_t lower_bound_u16(const uint16_t *a, uint32_t n, uint32_t key) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (a[mid] < key) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ uint32_t upper_bound_u16(const uint16_t *a, uint32_t n, uint32_t key) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (a[mid] <= key) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
 
 // ---------------------------------------------------------------- type rules
 __host__ __device__ __forceinline__ int rule_ab(int card) {

@@ -15,16 +15,6 @@
 
 namespace rb200 {
 
-__device__ __forceinline__ uint32_t lb_u16(const uint16_t *a, uint32_t n, uint32_t key) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (a[mid] < key) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
-}
-
 struct FusedSmem {
     uint32_t acc[FUSED_WARPS][WARP_SMEM_WORDS];   // accumulator + merge window (rb200_device.cuh)
     uint16_t keys[FUSED_MAX_ITEMS];          // keys of A then B
@@ -61,7 +51,7 @@ k_pair_fused(const uint8_t *__restrict__ in, uint8_t *out, uint32_t out_bytes, i
         if (t < na) {
             ca = t;
             key = sm.keys[t];
-            const uint32_t lb = lb_u16(sm.keys + na, nb, key);
+            const uint32_t lb = lower_bound_u16(sm.keys + na, nb, key);
             const bool matched = lb < nb && sm.keys[na + lb] == key;
             pos = t + lb;
             if (matched) {
@@ -76,13 +66,7 @@ k_pair_fused(const uint8_t *__restrict__ in, uint8_t *out, uint32_t out_bytes, i
             const uint32_t j = t - na;
             cb = t;
             key = sm.keys[t];
-            // upper bound of key in A
-            uint32_t lo = 0, hi = na;
-            while (lo < hi) {
-                const uint32_t mid = (lo + hi) >> 1;
-                if (sm.keys[mid] <= key) lo = mid + 1;
-                else hi = mid;
-            }
+            const uint32_t lo = upper_bound_u16(sm.keys, na, key);
             const bool matched = lo > 0 && sm.keys[lo - 1] == key;
             pos = j + lo;
             if (!matched && (OP == OP_OR || OP == OP_XOR)) {
@@ -185,14 +169,9 @@ bool launch_pair_fused(int op, const uint8_t *d_in, uint8_t *out_mapped, uint32_
         cudaFuncSetAttribute(k_pair_fused<OP_ANDNOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FusedSmem));
         attr = true;
     }
-    const size_t smem = sizeof(FusedSmem);
-    switch (op) {
-        case OP_AND: k_pair_fused<OP_AND><<<1, FUSED_WARPS * 32, smem, s>>>(d_in, out_mapped, out_bytes, rules, seq); break;
-        case OP_OR: k_pair_fused<OP_OR><<<1, FUSED_WARPS * 32, smem, s>>>(d_in, out_mapped, out_bytes, rules, seq); break;
-        case OP_XOR: k_pair_fused<OP_XOR><<<1, FUSED_WARPS * 32, smem, s>>>(d_in, out_mapped, out_bytes, rules, seq); break;
-        default: k_pair_fused<OP_ANDNOT><<<1, FUSED_WARPS * 32, smem, s>>>(d_in, out_mapped, out_bytes, rules, seq); break;
-    }
-    g_launches++;
+    auto *k = op == OP_AND ? k_pair_fused<OP_AND> : op == OP_OR ? k_pair_fused<OP_OR>
+            : op == OP_XOR ? k_pair_fused<OP_XOR> : k_pair_fused<OP_ANDNOT>;
+    launch_kernel(k, 1, FUSED_WARPS * 32, sizeof(FusedSmem), s, d_in, out_mapped, out_bytes, rules, seq);
     return cudaGetLastError() == cudaSuccess;
 }
 

@@ -115,7 +115,6 @@ struct Ctx {
     // single-pair fused path (rb200_fused.cu): packed operands (pinned + device), mapped result block
     uint8_t *h_fused_in = nullptr, *d_fused_in = nullptr, *h_fused_out = nullptr, *d_fused_out = nullptr;
     uint32_t fused_seq = 0;
-    int sms = 132;
     std::multimap<size_t, void *> dpool, hpool;
     std::mutex alloc_mu;  // dpool / hpool are also used by the background downloader thread
     uint64_t dev_in_use = 0;  // bytes of device blocks handed out by dev_alloc and not returned (under alloc_mu)
@@ -181,7 +180,7 @@ bool ctx_init(int device = -1) {
     CK(cudaHostAlloc(&g.h_fused_out, FUSED_OUT_BYTES, cudaHostAllocMapped));
     CK(cudaHostGetDevicePointer(&g.d_fused_out, g.h_fused_out, 0));
     memset(g.h_fused_out, 0, 64);
-    CK(cudaDeviceGetAttribute(&g.sms, cudaDevAttrMultiProcessorCount, g.device));
+    CK(cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, g.device));
     g_halloc.look();  // resolve the host allocator once, before any worker thread exists
     g.inited = true;
     return true;
@@ -1570,7 +1569,7 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         if (want_ck) cudaMemsetAsync(g.d_cardkey, 0, 65536 * 4, g.stream);
         launch_or_many2(vs, d_idx.get(), (uint32_t)n, key_lo, key_hi, ix, (uint32_t)max_units,
                         g.d_m2_scratch, g.d_m2_tickets, M2_SCRATCH_SLOTS, R->out(), want_ck ? g.d_cardkey : nullptr,
-                        g.d_stats, g.sms, g.stream, g.evk0, use_tma, window_index,
+                        g.d_stats, g.stream, g.evk0, use_tma, window_index,
                         (uint32_t *)(d_index.get() + al256(16 * tot) + al256(4 * max_units)));
     }
     if (ok) {
@@ -1698,7 +1697,7 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
         launch_many_compact(g.d_flags, g.d_keys, g.d_stats, g.stream);
         call.kernels_begin();
         launch_xor_many(vs, d_idx.get(), (uint32_t)n, g.d_keys, t_type.get(), t_card.get(), t_len.get(), R->out(),
-                        g.d_stats, g.sms, g.stream);
+                        g.d_stats, g.stream);
         call.kernels_end();
         call.end();
         ok = call.finish(ok);
@@ -2477,15 +2476,15 @@ int rb200_set_to_uint32(const rb200_set_t *S, uint32_t **vals, uint64_t **off_ou
     HostArrays out;
     if (!out.alloc(nb, false)) return -1;
     if (nb == 0) return out.hand_out(vals, off_out, nullptr);
-    DevBlock<uint64_t> d_bv(nb), d_off(nb + 1), d_dummy(nb + 1), d_cstart(nc);
-    DevBlock<uint32_t> d_zero(nb), d_cbm(nc), d_vals;
+    DevBlock<uint64_t> d_bv(nb), d_off(nb + 1), d_cstart(nc);
+    DevBlock<uint32_t> d_cbm(nc), d_vals;
     PinBlock<uint64_t> h_off(nb + 1);
     SyncCall call;
     uint64_t total = 0;
-    bool ok = d_bv && d_off && d_dummy && d_cstart && d_zero && d_cbm && h_off;
+    bool ok = d_bv && d_off && d_cstart && d_cbm && h_off;
     if (ok) {
-        launch_values_measure(S->view(), (uint32_t)nb, d_bv.get(), d_zero.get(), d_cstart.get(), d_cbm.get(), g.stream);
-        launch_pack_scan(d_bv.get(), d_zero.get(), (uint32_t)nb, d_off.get(), d_dummy.get(), g.stream);
+        launch_values_measure(S->view(), (uint32_t)nb, d_bv.get(), d_cstart.get(), d_cbm.get(), g.stream);
+        launch_pack_scan(d_bv.get(), nullptr, (uint32_t)nb, d_off.get(), nullptr, g.stream);
         ok = cudaMemcpyAsync(h_off.get(), d_off.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;
     }
@@ -2778,18 +2777,18 @@ static int serialize_impl(const rb200_set *s, char **buf, uint64_t **off_out, ui
     HostArrays out;
     if (!out.alloc(nb, true)) return -1;
     if (nb == 0) return out.hand_out(buf, off_out, len_out);
-    DevBlock<uint64_t> d_sz(nb), d_off(nb + 1), d_dummy(nb + 1);
+    DevBlock<uint64_t> d_sz(nb), d_off(nb + 1);
     DevBlock<uint32_t> d_exact(nb), d_hasrun(nb);
     DevBlock<uint8_t> d_blob;
     PinBlock<uint8_t> h_meta(8 * (nb + 1) + 4 * nb);
     SyncCall call;
     uint64_t total = 0;
-    bool ok = d_sz && d_off && d_dummy && d_exact && d_hasrun && h_meta;
+    bool ok = d_sz && d_off && d_exact && d_hasrun && h_meta;
     if (ok) {
         const SetView v = s->view();
         if (frozen) launch_frozen_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
         else launch_serialize_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
-        launch_pack_scan(d_sz.get(), d_hasrun.get(), (uint32_t)nb, d_off.get(), d_dummy.get(), g.stream);
+        launch_pack_scan(d_sz.get(), nullptr, (uint32_t)nb, d_off.get(), nullptr, g.stream);
         ok = cudaMemcpyAsync(h_meta.get(), d_off.get(), 8 * (nb + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaMemcpyAsync(h_meta.get() + 8 * (nb + 1), d_exact.get(), 4 * nb, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;
@@ -3394,19 +3393,19 @@ int serialize64_impl(const rb200_set64 *s, char **buf, uint64_t **off_out, uint6
     }
     if (n == 0) return out.hand_out(buf, off_out, len_out);
     const uint32_t *d_beg = s->d_dir.get(), *d_cnt = d_beg + n, *d_high = d_beg + 2 * n;
-    DevBlock<uint64_t> d_sz(nb), d_boff(nb), d_s16(n), d_e64(n), d_off(n + 1), d_dummy(n + 1);
+    DevBlock<uint64_t> d_sz(nb), d_boff(nb), d_s16(n), d_e64(n), d_off(n + 1);
     DevBlock<uint32_t> d_exact(nb), d_hasrun(nb);
     DevBlock<uint8_t> d_blob;
     PinBlock<uint64_t> h_meta(2 * n + 1);
     SyncCall call;
     uint64_t total = 0;
     const SetView v = s->inner->view();
-    bool ok = d_sz && d_boff && d_exact && d_hasrun && d_s16 && d_e64 && d_off && d_dummy && h_meta &&
+    bool ok = d_sz && d_boff && d_exact && d_hasrun && d_s16 && d_e64 && d_off && h_meta &&
               set64_dir_on_device(s);
     if (ok) {
         launch_serialize_measure(v, (uint32_t)nb, d_sz.get(), d_exact.get(), d_hasrun.get(), g.stream);
         launch_r64_ser_sizes(d_beg, d_cnt, (uint32_t)n, v.bm_cnt, d_exact.get(), d_s16.get(), d_e64.get(), g.stream);
-        launch_pack_scan(d_s16.get(), d_cnt, (uint32_t)n, d_off.get(), d_dummy.get(), g.stream);
+        launch_pack_scan(d_s16.get(), nullptr, (uint32_t)n, d_off.get(), nullptr, g.stream);
         ok = cudaMemcpyAsync(h_meta.get(), d_off.get(), 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaMemcpyAsync(h_meta.get() + n + 1, d_e64.get(), 8 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
              cudaStreamSynchronize(g.stream) == cudaSuccess;

@@ -15,36 +15,7 @@
 namespace rb200 {
 
 unsigned long long g_launches = 0;
-
-static inline int sm_count() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
-
-__device__ __forceinline__ uint32_t lower_bound_u16(const uint16_t *a, uint32_t n, uint32_t key) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (a[mid] < key) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
-}
-__device__ __forceinline__ uint32_t upper_bound_u16(const uint16_t *a, uint32_t n, uint32_t key) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (a[mid] <= key) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
-}
+int g_sm_count = 132;   // until rb200_init reads the device's
 
 // code-path class of a matched cell (see rb200_common.h CLS_*); mirrors the branches of cell_compute
 __device__ __forceinline__ int cell_class(int op, int rules, int tA, int tB, uint32_t cA, uint32_t cB, uint32_t lA,
@@ -434,7 +405,7 @@ k_finalize_cards(Items it, const uint64_t *__restrict__ item_off, uint32_t npair
         unsigned long long card = 0;
         for (uint64_t i = i0 + lane; i < i1; i += 32)
             if (it.kind[i] == K_COMPUTE) card += it.ocard[i];
-        for (int d = 16; d > 0; d >>= 1) card += __shfl_xor_sync(FULLMASK, card, d);
+        card = warp_sum(card);
         if (lane == 0) out[p] = card;
     }
 }
@@ -447,7 +418,7 @@ __global__ void k_set_cardinalities(SetView S, uint32_t n, uint64_t *__restrict_
         const uint32_t c0 = S.bm_beg[b], nc = S.bm_cnt[b];
         unsigned long long card = 0;
         for (uint32_t i = lane; i < nc; i += 32) card += S.c_card[c0 + i] & CARD_MASK;
-        for (int d = 16; d > 0; d >>= 1) card += __shfl_xor_sync(FULLMASK, card, d);
+        card = warp_sum(card);
         if (lane == 0) out[b] = card;
     }
 }
@@ -456,7 +427,7 @@ __global__ void k_set_cardinalities(SetView S, uint32_t n, uint64_t *__restrict_
 __global__ void k_sum_cards(const uint64_t *__restrict__ bm_card, uint32_t n, unsigned long long *acc) {
     unsigned long long v = 0;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) v += bm_card[i];
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(FULLMASK, v, d);
+    v = warp_sum(v);
     if ((threadIdx.x & 31) == 0 && v) atomicAdd(acc, v);
 }
 
@@ -477,20 +448,11 @@ __global__ void k_many_mark(SetView S, const uint32_t *__restrict__ idx, uint32_
 __global__ void __launch_bounds__(1024)
 k_many_compact(const uint32_t *__restrict__ flags, uint16_t *__restrict__ keys, OpStats *st) {
     __shared__ uint32_t s_warp[32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    uint32_t cnt = 0;
+    const int tid = threadIdx.x;
+    uint32_t cnt = 0, nk;
     for (int k = 0; k < 64; k++) cnt += flags[tid * 64 + k] ? 1u : 0u;
-    const uint32_t incl = warp_incl_scan(cnt, lane);
-    if (lane == 31) s_warp[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        const uint32_t v = s_warp[lane];
-        const uint32_t s = warp_incl_scan(v, lane);
-        s_warp[lane] = s - v;
-        if (lane == 31) st->nk = s;
-    }
-    __syncthreads();
-    uint32_t o = s_warp[wid] + incl - cnt;
+    uint32_t o = block_excl_scan<1024>(cnt, s_warp, &nk);
+    if (tid == 0) st->nk = nk;
     for (int k = 0; k < 64; k++)
         if (flags[tid * 64 + k]) keys[o++] = (uint16_t)(tid * 64 + k);
 }
@@ -512,7 +474,7 @@ k_pack_measure(SetView S, uint32_t n, int elide, uint64_t *__restrict__ bytes, u
             const bool skip = src != SRC_NONE && ((src & SRC_B) ? (elide & 2) : (elide & 1));
             if (!skip) v += round16(stored_bytes(S.c_type[c0 + i], S.c_len[c0 + i]));
         }
-        for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(FULLMASK, v, d);
+        v = warp_sum(v);
         if (lane == 0) {
             bytes[b] = v;
             cnts[b] = nc;
@@ -520,43 +482,29 @@ k_pack_measure(SetView S, uint32_t n, int elide, uint64_t *__restrict__ bytes, u
     }
 }
 
-// single CTA: exclusive scans of per-bitmap container counts and payload bytes
+// single CTA: exclusive scan of per-bitmap payload bytes, and of container counts when cnts is given
 // (n+1 outputs each: the last entry is the total)
 __global__ void __launch_bounds__(1024)
 k_pack_scan(const uint64_t *__restrict__ bytes, const uint32_t *__restrict__ cnts, uint32_t n,
             uint64_t *__restrict__ off_out, uint64_t *__restrict__ beg_out) {
-    __shared__ unsigned long long s_b[32], s_c[32];
-    __shared__ unsigned long long carry_b, carry_c;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid == 0) carry_b = carry_c = 0;
-    __syncthreads();
+    __shared__ unsigned long long s_w[32];
+    unsigned long long carry_b = 0, carry_c = 0;
     for (uint32_t base = 0; base < n; base += 1024) {
-        const uint32_t i = base + tid;
-        unsigned long long vb = i < n ? bytes[i] : 0ull, vc = i < n ? cnts[i] : 0ull;
-        unsigned long long ib = vb, ic = vc;
-        for (int d = 1; d < 32; d <<= 1) {
-            unsigned long long tb = __shfl_up_sync(FULLMASK, ib, d), tc = __shfl_up_sync(FULLMASK, ic, d);
-            if (lane >= d) { ib += tb; ic += tc; }
+        const uint32_t i = base + threadIdx.x;
+        unsigned long long tot;
+        const unsigned long long eb = carry_b + block_excl_scan<1024>(i < n ? bytes[i] : 0ull, s_w, &tot);
+        if (i < n) off_out[i] = eb;
+        carry_b += tot;
+        if (cnts) {
+            const unsigned long long ec = carry_c + block_excl_scan<1024>(i < n ? (unsigned long long)cnts[i] : 0ull, s_w, &tot);
+            if (i < n) beg_out[i] = ec;
+            carry_c += tot;
         }
-        if (lane == 31) { s_b[wid] = ib; s_c[wid] = ic; }
-        __syncthreads();
-        if (wid == 0) {
-            unsigned long long wb = s_b[lane], wc = s_c[lane], xb = wb, xc = wc;
-            for (int d = 1; d < 32; d <<= 1) {
-                unsigned long long tb = __shfl_up_sync(FULLMASK, xb, d), tc = __shfl_up_sync(FULLMASK, xc, d);
-                if (lane >= d) { xb += tb; xc += tc; }
-            }
-            s_b[lane] = xb - wb;
-            s_c[lane] = xc - wc;
-        }
-        __syncthreads();
-        const unsigned long long eb = carry_b + s_b[wid] + ib - vb, ec = carry_c + s_c[wid] + ic - vc;
-        if (i < n) { off_out[i] = eb; beg_out[i] = ec; }
-        __syncthreads();
-        if (tid == 1023) { carry_b = eb + vb; carry_c = ec + vc; }
-        __syncthreads();
     }
-    if (tid == 0) { off_out[n] = carry_b; beg_out[n] = carry_c; }
+    if (threadIdx.x == 0) {
+        off_out[n] = carry_b;
+        if (cnts) beg_out[n] = carry_c;
+    }
 }
 
 __global__ void __launch_bounds__(128)
@@ -604,7 +552,7 @@ k_pack_copy(SetView S, uint32_t n, int elide, const uint64_t *__restrict__ off_i
             }
             run += __shfl_sync(FULLMASK, incl, 31);
         }
-        for (int d = 16; d > 0; d >>= 1) card += __shfl_xor_sync(FULLMASK, card, d);
+        card = warp_sum(card);
         if (lane == 0) {
             out.bm_beg[b] = (uint32_t)nb;
             out.bm_cnt[b] = nc;
@@ -614,98 +562,74 @@ k_pack_copy(SetView S, uint32_t n, int elide, const uint64_t *__restrict__ off_i
 }
 
 // ------------------------------------------------------------------------------ launchers
-static inline uint32_t blocks_for_warps(uint64_t warps, int warps_per_block, int max_blocks) {
-    uint64_t b = (warps + warps_per_block - 1) / warps_per_block;
-    if (b < 1) b = 1;
-    if (b > (uint64_t)max_blocks) b = max_blocks;
-    return (uint32_t)b;
-}
-
 void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, const uint32_t *ib,
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
                        const PassShare &sh, Items it, OpStats *st, cudaStream_t s) {
     if (!npairs) return;
-    const uint32_t g = blocks_for_warps(npairs, 4, sm_count() * 16);
-    k_plan_pairs<<<g, 128, 0, s>>>(A, B, ia, ib, item_off, npairs, op, card_only, rules, sh, it, st);
-    g_launches++;
+    launch_kernel(k_plan_pairs, grid_for(npairs, 4, 16), 128, 0, s, A, B, ia, ib, item_off, npairs, op, card_only,
+                  rules, sh, it, st);
 }
 
 void launch_order_items(Items it, uint64_t W, OpStats *st, cudaStream_t s) {
     if (!W || !it.desc_cls) return;
-    const uint64_t chunks = (W + 2047) / 2048;
-    const uint32_t g = (uint32_t)(chunks < (uint64_t)sm_count() * 8 ? chunks : (uint64_t)sm_count() * 8);
-    k_order_items<<<g, 256, 0, s>>>(it, W, st);
-    g_launches++;
+    launch_kernel(k_order_items, grid_for(W, 2048, 8), 256, 0, s, it, W, st);
 }
 
 void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W, OpStats *st,
                        cudaStream_t s) {
     if (!W) return;
-    const uint32_t g = blocks_for_warps((W + 7) / 8, 4, sm_count() * 5);
-    k_card_items<<<g, 128, 0, s>>>(A, B, it, W, st);
-    g_launches++;
+    // tickets of 8 items, 4 warps per block
+    launch_kernel(k_card_items, grid_for(W, 32, 5), 128, 0, s, A, B, it, W, st);
 }
 
 void launch_finalize_pairs(const SetView &A, const SetView &B, Items it, const uint64_t *item_off,
                            uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, cudaStream_t s) {
     if (!npairs) return;
     // a warp per pair, full residency (16 CTAs of 4 warps per SM); counters: one atomic per block
-    const uint32_t g = blocks_for_warps(npairs, 4, sm_count() * RB200_FIN_BLOCKS);
-    k_finalize_pairs<<<g, 128, 0, s>>>(A, B, it, item_off, npairs, sh.onA ? 0u : 2u, sh.onB ? 0u : 2u, out, st);
-    g_launches++;
+    launch_kernel(k_finalize_pairs, grid_for(npairs, 4, RB200_FIN_BLOCKS), 128, 0, s, A, B, it, item_off, npairs,
+                  sh.onA ? 0u : 2u, sh.onB ? 0u : 2u, out, st);
 }
 
 void launch_finalize_cards(Items it, const uint64_t *item_off, uint32_t npairs, uint64_t *out,
                            cudaStream_t s) {
     if (!npairs) return;
-    const uint32_t g = blocks_for_warps(npairs, 4, sm_count() * 16);
-    k_finalize_cards<<<g, 128, 0, s>>>(it, item_off, npairs, out);
-    g_launches++;
+    launch_kernel(k_finalize_cards, grid_for(npairs, 4, 16), 128, 0, s, it, item_off, npairs, out);
 }
 
 void launch_sum_cardinalities(const uint64_t *bm_card, uint32_t n, uint64_t *d_acc, cudaStream_t s) {
     if (!n) return;
     const uint32_t blocks = (n + 255) / 256 < 592u ? (n + 255) / 256 : 592u;
-    k_sum_cards<<<blocks, 256, 0, s>>>(bm_card, n, (unsigned long long *)d_acc);
-    g_launches++;
+    launch_kernel(k_sum_cards, blocks, 256, 0, s, bm_card, n, (unsigned long long *)d_acc);
 }
 void launch_set_cardinalities(const SetView &S, uint32_t n, uint64_t *out, cudaStream_t s) {
     if (!n) return;
-    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
-    k_set_cardinalities<<<g, 128, 0, s>>>(S, n, out);
-    g_launches++;
+    launch_kernel(k_set_cardinalities, grid_for(n, 4, 16), 128, 0, s, S, n, out);
 }
 
 void launch_many_mark(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t key_lo,
                       uint32_t key_hi, uint32_t *flags, cudaStream_t s) {
     cudaMemsetAsync(flags, 0, 65536 * sizeof(uint32_t), s);
     if (!n) return;
-    const uint32_t g = n < (uint32_t)sm_count() * 8 ? n : (uint32_t)sm_count() * 8;
-    k_many_mark<<<g, 128, 0, s>>>(S, idx, n, key_lo, key_hi, flags);
-    g_launches++;
+    launch_kernel(k_many_mark, grid_for(n, 1, 8), 128, 0, s, S, idx, n, key_lo, key_hi, flags);
 }
 
 void launch_many_compact(const uint32_t *flags, uint16_t *keys_out, OpStats *st, cudaStream_t s) {
-    k_many_compact<<<1, 1024, 0, s>>>(flags, keys_out, st);
-    g_launches++;
+    launch_kernel(k_many_compact, 1, 1024, 0, s, flags, keys_out, st);
 }
 
-}  // namespace rb200
-
-namespace rb200 {
 void launch_pack(const SetView &S, uint32_t n, int elide, uint64_t *bytes, uint32_t *cnts, uint64_t *off,
                  uint64_t *beg, cudaStream_t s) {
-    const uint32_t g = blocks_for_warps(n ? n : 1, 4, sm_count() * 16);
-    k_pack_measure<<<g, 128, 0, s>>>(S, n, elide, bytes, cnts);
-    k_pack_scan<<<1, 1024, 0, s>>>(bytes, cnts, n, off, beg);
-    g_launches += 2;
+    launch_kernel(k_pack_measure, grid_for(n, 4, 16), 128, 0, s, S, n, elide, bytes, cnts);
+    launch_pack_scan(bytes, cnts, n, off, beg, s);
 }
 void launch_pack_copy(const SetView &S, uint32_t n, int elide, const uint64_t *off, const uint64_t *beg,
                       SetOut out, cudaStream_t s) {
     if (!n) return;
-    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
-    k_pack_copy<<<g, 128, 0, s>>>(S, n, elide, off, beg, out);
-    g_launches++;
+    launch_kernel(k_pack_copy, grid_for(n, 4, 16), 128, 0, s, S, n, elide, off, beg, out);
+}
+void launch_pack_scan(const uint64_t *bytes, const uint32_t *cnts, uint32_t n, uint64_t *off,
+                      uint64_t *beg, cudaStream_t s) {
+    launch_kernel(k_pack_scan, 1, 1024, 0, s, bytes, cnts, n, off, beg);
 }
 }  // namespace rb200
 
@@ -837,15 +761,6 @@ k_ser_write(SetView S, uint32_t n, const uint64_t *__restrict__ off, const uint3
 // u32 high 32 bits and the 32-bit portable blob of its low halves.  The buckets are the bitmaps of an
 // inner set (k_ser_measure gives their exact sizes, k_ser_write writes them at boff); empty buckets
 // are not emitted, as the reference never holds one.  Warp per 64-bit bitmap.
-__device__ __forceinline__ unsigned long long warp_incl_scan64(unsigned long long v, int lane) {
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const unsigned long long t = __shfl_up_sync(FULLMASK, v, d);
-        if (lane >= d) v += t;
-    }
-    return v;
-}
-
 __global__ void __launch_bounds__(128)
 k_r64_ser_sizes(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict__ b_cnt, uint32_t n,
                 const uint32_t *__restrict__ bm_cnt, const uint32_t *__restrict__ exact,
@@ -858,7 +773,7 @@ k_r64_ser_sizes(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict__
         unsigned long long sum = 0;
         for (uint32_t k = lane; k < c; k += 32)
             if (bm_cnt[j0 + k]) sum += 4ull + exact[j0 + k];
-        for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(FULLMASK, sum, d);
+        sum = warp_sum(sum);
         if (lane == 0) {
             exact64[i] = 8 + sum;
             sizes16[i] = (8 + sum + 15) & ~15ull;
@@ -886,7 +801,7 @@ k_r64_ser_layout(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict_
             const uint32_t j = j0 + k0 + lane;
             const bool in = k0 + lane < c, live = in && bm_cnt[j] != 0;
             const unsigned long long sz = live ? 4ull + exact[j] : 0ull;
-            const unsigned long long incl = warp_incl_scan64(sz, lane);
+            const unsigned long long incl = warp_incl_scan(sz, lane);
             const uint64_t pos = run + incl - sz;
             if (live) {
                 store_u32(dst + pos, high[j]);
@@ -904,31 +819,24 @@ k_r64_ser_layout(const uint32_t *__restrict__ b_beg, const uint32_t *__restrict_
 void launch_r64_ser_sizes(const uint32_t *b_beg, const uint32_t *b_cnt, uint32_t n, const uint32_t *bm_cnt,
                           const uint32_t *exact, uint64_t *sizes16, uint64_t *exact64, cudaStream_t s) {
     if (!n) return;
-    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
-    k_r64_ser_sizes<<<g, 128, 0, s>>>(b_beg, b_cnt, n, bm_cnt, exact, sizes16, exact64);
-    g_launches++;
+    launch_kernel(k_r64_ser_sizes, grid_for(n, 4, 16), 128, 0, s, b_beg, b_cnt, n, bm_cnt, exact, sizes16, exact64);
 }
 void launch_r64_ser_layout(const uint32_t *b_beg, const uint32_t *b_cnt, const uint32_t *high, uint32_t n,
                            uint32_t nbuckets, const uint32_t *bm_cnt, const uint32_t *exact, const uint64_t *off,
                            uint64_t *boff, uint8_t *dst, cudaStream_t s) {
-    const uint32_t g = blocks_for_warps(n ? n : 1, 4, sm_count() * 16);
-    k_r64_ser_layout<<<g, 128, 0, s>>>(b_beg, b_cnt, high, n, nbuckets, bm_cnt, exact, off, boff, dst);
-    g_launches++;
+    launch_kernel(k_r64_ser_layout, grid_for(n, 4, 16), 128, 0, s, b_beg, b_cnt, high, n, nbuckets, bm_cnt, exact, off,
+                  boff, dst);
 }
 
 void launch_serialize_measure(const SetView &S, uint32_t n, uint64_t *sizes16, uint32_t *exact,
                               uint32_t *hasrun, cudaStream_t s) {
     if (!n) return;
-    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
-    k_ser_measure<<<g, 128, 0, s>>>(S, n, sizes16, exact, hasrun);
-    g_launches++;
+    launch_kernel(k_ser_measure, grid_for(n, 4, 16), 128, 0, s, S, n, sizes16, exact, hasrun);
 }
 void launch_serialize_write(const SetView &S, uint32_t n, const uint64_t *off, const uint32_t *hasrun,
                             uint8_t *dst, cudaStream_t s) {
     if (!n) return;
-    const uint32_t g = blocks_for_warps(n, 4, sm_count() * 16);
-    k_ser_write<<<g, 128, 0, s>>>(S, n, off, hasrun, dst);
-    g_launches++;
+    launch_kernel(k_ser_write, grid_for(n, 4, 16), 128, 0, s, S, n, off, hasrun, dst);
 }
 }  // namespace rb200
 
@@ -941,6 +849,23 @@ namespace rb200 {
 
 __device__ __forceinline__ uint32_t ld_u16(const uint8_t *p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
 __device__ __forceinline__ uint32_t ld_u32(const uint8_t *p) { return ld_u16(p) | (ld_u16(p + 2) << 16); }
+
+// Do the keys of this chunk of (up to) 32 containers, one per lane, strictly increase, also from
+// prev_key, the last key of the previous chunk (-1 before the first)?  (roaring.c:496-503)
+// Advances prev_key to the chunk's last key.
+__device__ __forceinline__ bool keys_increase(uint32_t key, bool valid, int &prev_key, int lane) {
+    int left = __shfl_up_sync(FULLMASK, (int)key, 1);
+    if (lane == 0) left = prev_key;
+    if (__any_sync(FULLMASK, valid && (int)key <= left)) return false;
+    prev_key = __shfl_sync(FULLMASK, (int)key, 31);
+    return true;
+}
+
+// blob b of nb is malformed: error 3; the host names the first such blob, nb - st->nk
+__device__ __forceinline__ void report_malformed(OpStats *st, uint32_t nb, uint32_t b) {
+    atomicExch(&st->error, 3u);
+    atomicMax(&st->nk, nb - b);
+}
 
 __global__ void __launch_bounds__(128)
 k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
@@ -991,11 +916,7 @@ k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
                 isrun = hasrun && ((runflags[i >> 3] >> (i & 7)) & 1);
                 known = isrun ? 0u : (card > (uint32_t)MAX_ARRAY ? (uint32_t)BITSET_BYTES : 2u * card);
             }
-            // keys strictly increasing (roaring.c:496-503)
-            int left = __shfl_up_sync(FULLMASK, (int)key, 1);
-            if (lane == 0) left = prev_key;
-            if (__any_sync(FULLMASK, valid && (int)key <= left)) { bad = true; break; }
-            prev_key = __shfl_sync(FULLMASK, (int)key, 31);
+            if (!keys_increase(key, valid, prev_key, lane)) { bad = true; break; }
             // sequential walk over the chunk: a run container's size is in its first two bytes
             uint64_t mypos = 0;
             uint32_t mylen = 0, mystored = 0;
@@ -1029,10 +950,7 @@ k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
             }
             off += __shfl_sync(FULLMASK, incl, 31);
         }
-        if (bad && lane == 0) {
-            atomicExch(&st->error, 3u);
-            atomicMax(&st->nk, nb - b);  // host: first malformed blob = nb - nk
-        }
+        if (bad && lane == 0) report_malformed(st, nb, b);
     }
 }
 
@@ -1089,11 +1007,9 @@ __global__ void k_deser_bitmap_cards(SetOut out, uint32_t nb, const OpStats *st)
             sbytes += round16(stored_bytes(out.c_type[c0 + i], out.c_len[c0 + i]));
             ebytes += effective_bytes(out.c_type[c0 + i], out.c_len[c0 + i], out.c_card[c0 + i]);
         }
-        for (int d = 16; d > 0; d >>= 1) {
-            card += __shfl_xor_sync(FULLMASK, card, d);
-            sbytes += __shfl_xor_sync(FULLMASK, sbytes, d);
-            ebytes += __shfl_xor_sync(FULLMASK, ebytes, d);
-        }
+        card = warp_sum(card);
+        sbytes = warp_sum(sbytes);
+        ebytes = warp_sum(ebytes);
         if (lane == 0) { out.bm_card[b] = card; out.bm_bytes[b] = sbytes; out.bm_ebytes[b] = ebytes; }
     }
 }
@@ -1103,6 +1019,23 @@ __global__ void k_deser_bitmap_cards(SetOut out, uint32_t nb, const OpStats *st)
 // [bitset words | runs | array values | keys u16 | counts u16 | typecodes u8 | header u32], the
 // header LAST: (n_containers << 15) | FROZEN_COOKIE.  counts = cardinality-1 (bitset, array) or
 // n_runs (run).  Blob starts are 32-byte aligned so frozen_view accepts them in place.
+
+// Write cursors of the three payload zones of one blob, zb bytes of bitset words then zr bytes of
+// runs then the array values, advanced by a warp over its containers a chunk of 32 at a time.
+struct FrozenZones {
+    unsigned long long pb, pr, pa;
+    __device__ FrozenZones(unsigned long long zb, unsigned long long zr) : pb(0), pr(zb), pa(zb + zr) {}
+    // offset of this lane's container (type t, sz payload bytes; sz = 0 past the end) in the zones
+    __device__ __forceinline__ unsigned long long next(int t, uint32_t sz, int lane) {
+        const uint32_t sb = t == T_BITSET ? sz : 0u, sr = t == T_RUN ? sz : 0u, sa = t == T_ARRAY ? sz : 0u;
+        const uint32_t ib = warp_incl_scan(sb, lane), ir = warp_incl_scan(sr, lane), ia = warp_incl_scan(sa, lane);
+        const unsigned long long d = t == T_BITSET ? pb + ib - sb : (t == T_RUN ? pr + ir - sr : pa + ia - sa);
+        pb += __shfl_sync(FULLMASK, ib, 31);
+        pr += __shfl_sync(FULLMASK, ir, 31);
+        pa += __shfl_sync(FULLMASK, ia, 31);
+        return d;
+    }
+};
 
 __global__ void __launch_bounds__(128)
 k_frozen_measure(SetView S, uint32_t n, uint64_t *__restrict__ sizes32, uint32_t *__restrict__ exact,
@@ -1114,7 +1047,7 @@ k_frozen_measure(SetView S, uint32_t n, uint64_t *__restrict__ sizes32, uint32_t
         const uint32_t c0 = S.bm_beg[b], nc = S.bm_cnt[b];
         unsigned long long bytes = 0;
         for (uint32_t i = lane; i < nc; i += 32) bytes += stored_bytes(S.c_type[c0 + i], S.c_len[c0 + i]);
-        for (int d = 16; d > 0; d >>= 1) bytes += __shfl_xor_sync(FULLMASK, bytes, d);
+        bytes = warp_sum(bytes);
         if (lane == 0) {
             const unsigned long long tot = bytes + 5ull * nc + 4ull;
             exact[b] = (uint32_t)tot;
@@ -1138,14 +1071,12 @@ k_frozen_dir(SetView S, uint32_t n, const uint64_t *__restrict__ off, uint8_t *_
             const uint32_t sz = stored_bytes(t, S.c_len[c0 + i]);
             if (t == T_BITSET) zb += sz; else if (t == T_RUN) zr += sz; else za += sz;
         }
-        for (int d = 16; d > 0; d >>= 1) {
-            zb += __shfl_xor_sync(FULLMASK, zb, d);
-            zr += __shfl_xor_sync(FULLMASK, zr, d);
-            za += __shfl_xor_sync(FULLMASK, za, d);
-        }
+        zb = warp_sum(zb);
+        zr = warp_sum(zr);
+        za = warp_sum(za);
         uint8_t *base = dst + off[b];
         const unsigned long long k0 = zb + zr + za, n0 = k0 + 2ull * nc, t0 = n0 + 2ull * nc, h0 = t0 + nc;
-        unsigned long long pb = 0, pr = zb, pa = zb + zr;  // running write cursors of the three zones
+        FrozenZones z(zb, zr);
         for (uint32_t chunk = 0; chunk < nc; chunk += 32) {
             const uint32_t i = chunk + lane;
             const bool valid = i < nc;
@@ -1157,18 +1088,13 @@ k_frozen_dir(SetView S, uint32_t n, const uint64_t *__restrict__ off, uint8_t *_
                 card = S.c_card[c0 + i] & CARD_MASK;
                 sz = stored_bytes(t, len);
             }
-            const uint32_t sb = t == T_BITSET ? sz : 0u, sr = t == T_RUN ? sz : 0u, sa = t == T_ARRAY ? sz : 0u;
-            const uint32_t ib = warp_incl_scan(sb, lane), ir = warp_incl_scan(sr, lane), ia = warp_incl_scan(sa, lane);
+            const unsigned long long d = z.next(t, sz, lane);
             if (valid) {
-                const unsigned long long d = t == T_BITSET ? pb + ib - sb : (t == T_RUN ? pr + ir - sr : pa + ia - sa);
                 c_dst[c0 + i] = off[b] + d;
                 store_u16(base + k0 + 2ull * i, S.c_key[c0 + i]);
                 store_u16(base + n0 + 2ull * i, t == T_RUN ? len : card - 1u);
                 base[t0 + i] = (uint8_t)t;
             }
-            pb += __shfl_sync(FULLMASK, ib, 31);
-            pr += __shfl_sync(FULLMASK, ir, 31);
-            pa += __shfl_sync(FULLMASK, ia, 31);
         }
         if (lane == 0) store_u32(base + h0, (nc << 15) | FROZEN_COOKIE);
     }
@@ -1186,18 +1112,13 @@ k_frozen_copy(SetView S, uint64_t nc, const uint64_t *__restrict__ c_dst, uint8_
 void launch_frozen_measure(const SetView &S, uint32_t n, uint64_t *sizes32, uint32_t *exact, uint32_t *cnt,
                            cudaStream_t s) {
     if (!n) return;
-    k_frozen_measure<<<blocks_for_warps(n, 4, sm_count() * 16), 128, 0, s>>>(S, n, sizes32, exact, cnt);
-    g_launches++;
+    launch_kernel(k_frozen_measure, grid_for(n, 4, 16), 128, 0, s, S, n, sizes32, exact, cnt);
 }
 void launch_frozen_write(const SetView &S, uint32_t n, uint64_t nc, const uint64_t *off, uint8_t *dst,
                          uint64_t *c_dst, cudaStream_t s) {
     if (!n) return;
-    k_frozen_dir<<<blocks_for_warps(n, 4, sm_count() * 16), 128, 0, s>>>(S, n, off, dst, c_dst);
-    g_launches++;
-    if (nc) {
-        k_frozen_copy<<<blocks_for_warps(nc, 4, sm_count() * 16), 128, 0, s>>>(S, nc, c_dst, dst);
-        g_launches++;
-    }
+    launch_kernel(k_frozen_dir, grid_for(n, 4, 16), 128, 0, s, S, n, off, dst, c_dst);
+    if (nc) launch_kernel(k_frozen_copy, grid_for(nc, 4, 16), 128, 0, s, S, nc, c_dst, dst);
 }
 
 // frozen blobs -> directory (the zones make every payload offset a prefix sum: no sequential walk)
@@ -1231,14 +1152,13 @@ k_frozen_parse_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__
                 else bad = true;
             }
             bad = __any_sync(FULLMASK, bad);
-            for (int d = 16; d > 0; d >>= 1) {
-                zb += __shfl_xor_sync(FULLMASK, zb, d);
-                zr += __shfl_xor_sync(FULLMASK, zr, d);
-                za += __shfl_xor_sync(FULLMASK, za, d);
-            }
+            zb = warp_sum(zb);
+            zr = warp_sum(zr);
+            za = warp_sum(za);
             if (zb + zr + za + 5ull * nc + 4ull != len) bad = true;   // roaring.c:3425-3429 exact length
         }
-        unsigned long long pb = 0, pr = zb, pa = zb + zr, off = slab_base[b];
+        FrozenZones z(zb, zr);
+        unsigned long long off = slab_base[b];
         int prev_key = -1;
         for (uint32_t chunk = 0; chunk < nc && !bad; chunk += 32) {
             const uint32_t i = chunk + lane;
@@ -1251,17 +1171,12 @@ k_frozen_parse_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__
                 cnt = ld_u16(nz + 2ull * i);
                 sz = t == T_BITSET ? (uint32_t)BITSET_BYTES : (t == T_RUN ? 4u * cnt : 2u * (cnt + 1u));
             }
-            int left = __shfl_up_sync(FULLMASK, (int)key, 1);
-            if (lane == 0) left = prev_key;
-            if (__any_sync(FULLMASK, valid && (int)key <= left)) { bad = true; break; }
-            prev_key = __shfl_sync(FULLMASK, (int)key, 31);
-            const uint32_t sb = t == T_BITSET ? sz : 0u, sr = t == T_RUN ? sz : 0u, sa = t == T_ARRAY ? sz : 0u;
-            const uint32_t ib = warp_incl_scan(sb, lane), ir = warp_incl_scan(sr, lane), ia = warp_incl_scan(sa, lane);
+            if (!keys_increase(key, valid, prev_key, lane)) { bad = true; break; }
+            const unsigned long long d = z.next(t, sz, lane);
             const uint32_t r16 = valid ? round16(sz) : 0u;
             const uint32_t incl = warp_incl_scan(r16, lane);
             if (valid) {
                 const uint64_t c = (uint64_t)c0 + i;
-                const unsigned long long d = t == T_BITSET ? pb + ib - sb : (t == T_RUN ? pr + ir - sr : pa + ia - sa);
                 out.c_key[c] = (uint16_t)key;
                 out.c_type[c] = (uint8_t)t;
                 out.c_card[c] = cnt + 1u;                    // runs: recounted by k_deser_copy
@@ -1270,56 +1185,37 @@ k_frozen_parse_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__
                 out.c_src[c] = SRC_NONE;
                 src_pos[c] = roff[b] + d;
             }
-            pb += __shfl_sync(FULLMASK, ib, 31);
-            pr += __shfl_sync(FULLMASK, ir, 31);
-            pa += __shfl_sync(FULLMASK, ia, 31);
             off += __shfl_sync(FULLMASK, incl, 31);
         }
-        if (bad && lane == 0) {
-            atomicExch(&st->error, 3u);
-            atomicMax(&st->nk, nb - b);
-        }
+        if (bad && lane == 0) report_malformed(st, nb, b);
     }
+}
+
+// the directory parse (k_deser_dir / k_frozen_parse_dir), then the payload moves and the bitmap figures
+static void deserialize_tail(const uint8_t *raw, uint32_t nb, uint64_t nc, SetOut out, uint64_t *src_pos, OpStats *st,
+                             cudaStream_t s) {
+    if (nc) launch_kernel(k_deser_copy, grid_for(nc, 4, 16), 128, 0, s, raw, src_pos, nc, out, st);
+    launch_kernel(k_deser_bitmap_cards, grid_for(nb, 4, 16), 128, 0, s, out, nb, st);
 }
 
 void launch_deserialize_frozen(const uint8_t *raw, const uint64_t *roff, const uint64_t *rlen,
                                const uint64_t *slab_base, uint32_t nb, uint64_t nc, SetOut out,
                                uint64_t *src_pos, OpStats *st, cudaStream_t s) {
     if (!nb) return;
-    k_frozen_parse_dir<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(raw, roff, rlen, slab_base, nb, out, src_pos, st);
-    g_launches++;
-    if (nc) {
-        k_deser_copy<<<blocks_for_warps(nc, 4, sm_count() * 16), 128, 0, s>>>(raw, src_pos, nc, out, st);
-        g_launches++;
-    }
-    k_deser_bitmap_cards<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(out, nb, st);
-    g_launches++;
+    launch_kernel(k_frozen_parse_dir, grid_for(nb, 4, 16), 128, 0, s, raw, roff, rlen, slab_base, nb, out, src_pos, st);
+    deserialize_tail(raw, nb, nc, out, src_pos, st, s);
 }
 
 void launch_deserialize(const uint8_t *raw, const uint64_t *roff, const uint64_t *rlen,
                         const uint64_t *slab_base, uint32_t nb, uint64_t nc, SetOut out,
                         uint64_t *src_pos, OpStats *st, cudaStream_t s) {
     if (!nb) return;
-    k_deser_dir<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(raw, roff, rlen, slab_base, nb, out, src_pos, st);
-    g_launches++;
-    if (nc) {
-        k_deser_copy<<<blocks_for_warps(nc, 4, sm_count() * 16), 128, 0, s>>>(raw, src_pos, nc, out, st);
-        g_launches++;
-    }
-    k_deser_bitmap_cards<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(out, nb, st);
-    g_launches++;
+    launch_kernel(k_deser_dir, grid_for(nb, 4, 16), 128, 0, s, raw, roff, rlen, slab_base, nb, out, src_pos, st);
+    deserialize_tail(raw, nb, nc, out, src_pos, st, s);
 }
-}  // namespace rb200
 
-namespace rb200 {
 void launch_bitmap_figures(SetOut out, uint32_t nb, const OpStats *st, cudaStream_t s) {
     if (!nb) return;
-    k_deser_bitmap_cards<<<blocks_for_warps(nb, 4, sm_count() * 16), 128, 0, s>>>(out, nb, st);
-    g_launches++;
-}
-void launch_pack_scan(const uint64_t *bytes, const uint32_t *cnts, uint32_t n, uint64_t *off,
-                      uint64_t *beg, cudaStream_t s) {
-    k_pack_scan<<<1, 1024, 0, s>>>(bytes, cnts, n, off, beg);
-    g_launches++;
+    launch_kernel(k_deser_bitmap_cards, grid_for(nb, 4, 16), 128, 0, s, out, nb, st);
 }
 }  // namespace rb200

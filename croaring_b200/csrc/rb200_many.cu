@@ -21,14 +21,14 @@ struct ManySmem {
     uint32_t pcard[OM_CHUNK];
     uint32_t warp_a[OM_THREADS / 32];
     int red[OM_THREADS / 32][2];
-    uint32_t np, ki;
+    uint32_t ki;
 };
 
 // Gather the participants of `key` among bitmaps [c0, c0+OM_CHUNK) ∩ [0,n) in input order.
 __device__ __forceinline__ uint32_t many_gather(ManySmem &sm, const SetView &S,
                                                 const uint32_t *__restrict__ idx, uint32_t n,
                                                 uint32_t key, uint32_t c0, uint32_t c1) {
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int tid = threadIdx.x;
     uint32_t cnt = 0;
     // two lower_bound searches per thread, advanced in lockstep so their loads overlap
     uint32_t b0[2], nb[2], lo[2], hi[2];
@@ -71,17 +71,8 @@ __device__ __forceinline__ uint32_t many_gather(ManySmem &sm, const SetView &S,
         off[k] = hit[k] ? S.c_off[c] : 0ull;
         cnt += hit[k] ? 1u : 0u;
     }
-    const uint32_t incl = warp_incl_scan(cnt, lane);
-    if (lane == 31) sm.warp_a[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        const uint32_t va = lane < OM_THREADS / 32 ? sm.warp_a[lane] : 0u;
-        const uint32_t sa = warp_incl_scan(va, lane);
-        if (lane < OM_THREADS / 32) sm.warp_a[lane] = sa - va;
-        if (lane == 31) sm.np = sa;
-    }
-    __syncthreads();
-    uint32_t o = sm.warp_a[wid] + incl - cnt;
+    uint32_t np;
+    uint32_t o = block_excl_scan<OM_THREADS>(cnt, sm.warp_a, &np);
 #pragma unroll
     for (int k = 0; k < 2; k++)
         if (hit[k]) {
@@ -93,7 +84,7 @@ __device__ __forceinline__ uint32_t many_gather(ManySmem &sm, const SetView &S,
             o++;
         }
     __syncthreads();
-    return sm.np;
+    return np;
 }
 
 // ------------------------------------------------------------------------------ xor_many
@@ -252,28 +243,16 @@ k_compact_dir(const uint16_t *__restrict__ keys, const uint8_t *__restrict__ t_t
               SetOut out, OpStats *st) {
     __shared__ uint32_t s_w[32];
     __shared__ unsigned long long s_c[32];
-    __shared__ uint32_t s_carry, s_total;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint32_t nk = st->nk;
-    if (tid == 0) s_carry = 0;
+    uint32_t carry = 0;
     unsigned long long csum = 0;
-    __syncthreads();
     for (uint32_t base = 0; base < nk; base += 1024) {
         const uint32_t i = base + tid;
         const bool live = i < nk && t_type[i] != 0;
-        const uint32_t v = live ? 1u : 0u;
-        const uint32_t incl = warp_incl_scan(v, lane);
-        if (lane == 31) s_w[wid] = incl;
-        __syncthreads();
-        if (wid == 0) {
-            const uint32_t x = s_w[lane];
-            const uint32_t sx = warp_incl_scan(x, lane);
-            s_w[lane] = sx - x;
-            if (lane == 31) s_total = sx;
-        }
-        __syncthreads();
+        uint32_t total;
+        const uint32_t o = carry + block_excl_scan<1024>(live ? 1u : 0u, s_w, &total);
         if (live) {
-            const uint32_t o = s_carry + s_w[wid] + incl - v;
             out.c_key[o] = keys[i];
             out.c_type[o] = t_type[i];
             out.c_card[o] = t_card[i];
@@ -282,30 +261,26 @@ k_compact_dir(const uint16_t *__restrict__ keys, const uint8_t *__restrict__ t_t
             out.c_src[o] = SRC_NONE;
             csum += t_card[i];
         }
-        __syncthreads();
-        if (tid == 0) s_carry += s_total;
-        __syncthreads();
+        carry += total;
     }
-    for (int d = 16; d > 0; d >>= 1) csum += __shfl_xor_sync(FULLMASK, csum, d);
+    csum = warp_sum(csum);
     if (lane == 0) s_c[wid] = csum;
     __syncthreads();
     if (tid == 0) {
         unsigned long long t = 0;
         for (int w = 0; w < 32; w++) t += s_c[w];
         out.bm_beg[0] = 0;
-        out.bm_cnt[0] = s_carry;
+        out.bm_cnt[0] = carry;
         out.bm_card[0] = t;
-        st->dir_cursor = s_carry;
+        st->dir_cursor = carry;
     }
 }
 
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
                      uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
-                     int sms, cudaStream_t s) {
-    k_xor_many<<<sms * 2, OM_THREADS, 0, s>>>(S, idx, n, keys, t_type, t_card, t_len, out.payload, st);
-    g_launches++;
-    k_compact_dir<<<1, 1024, 0, s>>>(keys, t_type, t_card, t_len, out, st);
-    g_launches++;
+                     cudaStream_t s) {
+    launch_kernel(k_xor_many, g_sm_count * 2, OM_THREADS, 0, s, S, idx, n, keys, t_type, t_card, t_len, out.payload, st);
+    launch_kernel(k_compact_dir, 1, 1024, 0, s, keys, t_type, t_card, t_len, out, st);
 }
 
 }  // namespace rb200

@@ -32,8 +32,6 @@
 //         makes that test a popcount instead of a second pass over the payloads.
 #include <stdlib.h>
 
-#include <algorithm>
-
 #include "rb200_device.cuh"
 
 namespace rb200 {
@@ -813,7 +811,7 @@ __global__ void k_many2_sum_cards(const uint32_t *__restrict__ c_card, const OpS
     const uint32_t n = st->nk;
     unsigned long long v = 0;
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) v += c_card[i];
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(FULLMASK, v, d);
+    v = warp_sum(v);
     if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = v;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -825,24 +823,24 @@ __global__ void k_many2_sum_cards(const uint32_t *__restrict__ c_card, const OpS
 
 void launch_or_many2(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t key_lo, uint32_t key_hi,
                      const Many2Index &ix, uint32_t max_units, uint32_t *scratch, uint32_t *tickets,
-                     uint32_t scratch_slots, SetOut out, uint32_t *card_per_key, OpStats *st, int sms,
-                     cudaStream_t s, cudaEvent_t ev_kernel_start, bool use_tma, bool window_index, uint32_t *cnt_tab) {
-    const uint32_t gw = (uint32_t)sms * 8;
+                     uint32_t scratch_slots, SetOut out, uint32_t *card_per_key, OpStats *st, cudaStream_t s,
+                     cudaEvent_t ev_kernel_start, bool use_tma, bool window_index, uint32_t *cnt_tab) {
+    const uint32_t gw = (uint32_t)g_sm_count * 8;
     if (window_index) {
         // long directories: key-window index build, shared-memory counting, no global atomics
-        const uint32_t gs = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, (uint64_t)sms * 4));
-        k_many2_span<<<gs, 256, 0, s>>>(S, idx, n, ix.key_fill);
+        launch_kernel(k_many2_span, grid_for(n, 256, 4), 256, 0, s, S, idx, n, ix.key_fill);
         const uint32_t nchunks = (n + M2W_THREADS - 1) / M2W_THREADS;
-        k_many2_window<false><<<sms * 6, M2W_THREADS, 0, s>>>(S, idx, n, key_lo, key_hi, ix, nchunks, cnt_tab);
-        k_many2_scan<<<1, 1024, 0, s>>>(ix, scratch_slots, max_units, (uint32_t)sms * 8, out, st, 1);
-        k_many2_window<true><<<sms * 6, M2W_THREADS, 0, s>>>(S, idx, n, key_lo, key_hi, ix, nchunks, cnt_tab);
-        g_launches += 1;
+        launch_kernel(k_many2_window<false>, g_sm_count * 6, M2W_THREADS, 0, s, S, idx, n, key_lo, key_hi, ix, nchunks,
+                      cnt_tab);
+        launch_kernel(k_many2_scan, 1, 1024, 0, s, ix, scratch_slots, max_units, gw, out, st, 1);
+        launch_kernel(k_many2_window<true>, g_sm_count * 6, M2W_THREADS, 0, s, S, idx, n, key_lo, key_hi, ix, nchunks,
+                      cnt_tab);
     } else {
-        k_many2_count<<<gw, 128, 0, s>>>(S, idx, n, key_lo, key_hi, ix);
-        k_many2_scan<<<1, 1024, 0, s>>>(ix, scratch_slots, max_units, (uint32_t)sms * 8, out, st, 0);
-        k_many2_fill<<<gw, 128, 0, s>>>(S, idx, n, key_lo, key_hi, ix);
+        launch_kernel(k_many2_count, gw, 128, 0, s, S, idx, n, key_lo, key_hi, ix);
+        launch_kernel(k_many2_scan, 1, 1024, 0, s, ix, scratch_slots, max_units, gw, out, st, 0);
+        launch_kernel(k_many2_fill, gw, 128, 0, s, S, idx, n, key_lo, key_hi, ix);
     }
-    k_many2_fold<<<gw, 128, 0, s>>>(ix, st);
+    launch_kernel(k_many2_fold, gw, 128, 0, s, ix, st);
     if (ev_kernel_start) cudaEventRecord(ev_kernel_start, s);
     const size_t smem_direct = (sizeof(Many2Smem) + 127) & ~(size_t)127, smem_tma = smem_direct + 2 * M2_HALF;
     static bool attr = false;
@@ -852,11 +850,12 @@ void launch_or_many2(const SetView &S, const uint32_t *idx, uint32_t n, uint32_t
         attr = true;
     }
     if (use_tma)
-        k_or_many2<true><<<sms * 2, M2_THREADS, smem_tma, s>>>(S, ix, n, scratch, tickets, out, card_per_key, st);
+        launch_kernel(k_or_many2<true>, g_sm_count * 2, M2_THREADS, smem_tma, s, S, ix, n, scratch, tickets, out,
+                      card_per_key, st);
     else
-        k_or_many2<false><<<sms * RB200_M2_MINB, M2_THREADS, smem_direct, s>>>(S, ix, n, scratch, tickets, out, card_per_key, st);
-    k_many2_sum_cards<<<1, 1024, 0, s>>>(out.c_card, st, out.bm_card);
-    g_launches += 6;
+        launch_kernel(k_or_many2<false>, g_sm_count * RB200_M2_MINB, M2_THREADS, smem_direct, s, S, ix, n, scratch,
+                      tickets, out, card_per_key, st);
+    launch_kernel(k_many2_sum_cards, 1, 1024, 0, s, out.c_card, st, out.bm_card);
 }
 
 }  // namespace rb200
