@@ -90,6 +90,7 @@ def lib():
     sig("rb200_batch_relations", C.c_int, _P, _P, _P, _P, C.c_size_t, _P)
     sig("rb200_set_op_stats", C.c_int, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64))
     sig("rb200_batch_flip", _P, _P, _P, C.c_size_t, C.c_uint64, C.c_uint64)
+    sig("rb200_batch_add_offset", _P, _P, _P, C.c_size_t, _P)
     sig("rb200_r64_batch_op_serialized", C.c_int, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
         C.c_size_t, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t, _P, _P, C.c_size_t,
         C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)), C.POINTER(C.POINTER(C.c_uint64)))
@@ -515,6 +516,27 @@ def _values_u32(a):
     return np.ascontiguousarray(a, dtype=np.uint32)
 
 
+def _offsets_i64(offsets, n):
+    """add_offset's offsets as n contiguous int64 values: a scalar is broadcast; values outside the
+    int64 range, non-integers and a length other than n are refused (never wrapped or rounded)."""
+    if isinstance(offsets, (int, np.integer)):
+        offsets = [int(offsets)] * n
+    a = np.asarray(offsets)
+    if a.dtype == object:   # Python ints beyond what numpy holds natively
+        if not all(isinstance(x, (int, np.integer)) for x in a.reshape(-1)):
+            raise RB200Error("offsets must be integers")
+        if any(not -(1 << 63) <= int(x) < (1 << 63) for x in a.reshape(-1)):
+            raise RB200Error("offsets must lie in the int64 range [-2^63, 2^63)")
+        a = a.astype(np.int64)
+    if a.ndim != 1 or (a.size and a.dtype.kind not in "iu"):
+        raise RB200Error(f"offsets must be a 1-D integer array, got {a.dtype} with shape {a.shape}")
+    if a.dtype.kind == "u" and a.size and int(a.max()) >= (1 << 63):
+        raise RB200Error("offsets must lie in the int64 range [-2^63, 2^63)")
+    if a.size != n:
+        raise RB200Error(f"offsets has {a.size} entries for {n} items")
+    return np.ascontiguousarray(a, dtype=np.int64)
+
+
 class DeviceSet:
     """An ordered collection of bitmaps resident in HBM (rb200_set_t*)."""
 
@@ -655,6 +677,17 @@ class DeviceSet:
             idx = _u32(idx)
             ip, n = idx.ctypes.data, idx.size
         return DeviceSet(lib().rb200_batch_flip(self.ptr, ip, n, int(range_start), int(range_end)))
+
+    def add_offset(self, offsets, idx=None):
+        """roaring_bitmap_add_offset of every (or the selected) bitmap: result[k] = self[idx[k]] +
+        offsets[k].  offsets: one integer for every item, or one per item (int64 range)."""
+        if idx is None:
+            ip, n = None, len(self)
+        else:
+            idx = _u32(idx)
+            ip, n = idx.ctypes.data, idx.size
+        offs = _offsets_i64(offsets, n)   # held until the call returns
+        return DeviceSet(lib().rb200_batch_add_offset(self.ptr, ip, n, offs.ctypes.data))
 
     def op_stats(self):
         """(device_ms, compute_kernel_ms, algorithmic_bytes) of the batch op that produced this set."""

@@ -390,6 +390,15 @@ void launch_r64_ser_layout(const uint32_t *b_beg, const uint32_t *b_cnt, const u
                            uint32_t nbuckets, const uint32_t *bm_cnt, const uint32_t *exact, const uint64_t *off,
                            uint64_t *boff, uint8_t *dst, cudaStream_t s);
 
+// roaring_bitmap_add_offset over a batch (rb200_offset.cu): item p is bitmap idx[p] (idx null: p) of S
+// shifted by offsets[p]; its 2 x (containers) item slots start at item_off[p].  cell: one uint4 per
+// item slot for the cells kernel.  The result directory is then built by launch_finalize_pairs(S, S, ...).
+void launch_offset_plan(const SetView &S, const uint32_t *idx, const int64_t *offsets, const uint64_t *item_off,
+                        uint32_t n, const PassShare &sh, Items it, uint4 *cell, uint64_t slab_cap, OpStats *st,
+                        cudaStream_t s);
+void launch_offset_cells(const SetView &S, Items it, const uint4 *cell, uint64_t W, uint64_t bias, uint8_t *slab,
+                         OpStats *st, cudaStream_t s);
+
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
                      uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
                      cudaStream_t s);

@@ -171,6 +171,23 @@ __host__ __device__ inline int decide_type(int op, int tA, int tB, uint32_t cA, 
     }
 }
 
+// Final type of one output key of roaring_bitmap_add_offset (src/roaring.c:2470-2505) with a shift
+// that is not a multiple of 65536.  The key holds one or two parts, each of its source container's
+// type (container_add_offset, containers.h:1536); tB = 0 when there is one part.  Two parts were
+// merged by container_ior (containers.h:1226-1319), and every container was then repaired
+// (container_repair_after_lazy, containers.h:344-371).  The parts are disjoint and neither is
+// full, so container_ior's full-run branches never fire.  card / nruns: of the key's union.
+__host__ __device__ inline int offset_type(int tA, int tB, int card, int nruns) {
+    if (tB == 0) {   // one part: repair alone
+        if (tA == T_ARRAY) return T_ARRAY;
+        return tA == T_BITSET ? rule_ab(card) : rule_eff(card, nruns);
+    }
+    if (tA == T_BITSET && tB == T_BITSET)   // bitset_container_or + OR_BITSET_CONVERSION_TO_FULL
+        return card == 65536 ? T_RUN : rule_ab(card);
+    if (tA == T_BITSET || tB == T_BITSET || (tA == T_ARRAY && tB == T_ARRAY)) return rule_ab(card);
+    return rule_eff(card, nruns);           // a run with a run or an array: the efficient container
+}
+
 __host__ __device__ __forceinline__ uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
 
 // payload bytes as stored in a slab (runs without the 2-byte n_runs prefix)

@@ -3126,6 +3126,99 @@ bool roaring_bitmap_is_strict_subset(const roaring_bitmap_t *r1, const roaring_b
     return r > 0 && (r & 4);
 }
 
+// ---- shift: roaring_bitmap_add_offset (src/roaring.c:2426-2507) ----------------------------------
+// result[k] = S[idx[k]] with offsets[k] added to every value.  Every source container owns two item
+// slots, its lo and its hi part (rb200_offset.cu); k_finalize_pairs compacts them into the result
+// directory.  Key-aligned shifts (offset % 65536 == 0) share the operand's containers, or copy them
+// when S shares containers itself (holds never chain, see rb200_set::held); one batch may mix both.
+rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, size_t n, const int64_t *offsets) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    if (!offsets) { t_err = "add_offset: offsets is NULL"; return nullptr; }
+    if (!S) { t_err = "add_offset: S is NULL"; return nullptr; }
+    if (idx == nullptr) n = S->n_bitmaps;
+    if (n > 0xffffffffull) { t_err = "add_offset: n must be below 2^32"; return nullptr; }
+    for (size_t k = 0; idx && k < n; k++) {
+        if (idx[k] >= S->n_bitmaps) {
+            t_err = "add_offset: idx[" + std::to_string(k) + "] = " + std::to_string(idx[k]) +
+                    " is out of range (the set holds " + std::to_string(S->n_bitmaps) + " bitmaps)";
+            return nullptr;
+        }
+    }
+    if (reject_lazy(S, "add_offset")) return nullptr;
+    if (!ctx_init() || !ensure_mirrors(S)) return nullptr;
+    // item slots and the result slab, sized from the host mirrors before the launch.  A computed
+    // container holds at most min(8192, 2 x its cardinality) bytes (offset_type: a run is kept only
+    // when it is no larger, a bitset only above 4096 values), and its parts come from at most two
+    // sources, each feeding at most two containers: 2 x the effective bytes of the operand, plus the
+    // 16-byte rounding of every slot.  Copied key-aligned containers take their stored bytes.
+    const size_t o_off = 0, o_idx = al256(8 * (n + 1)), o_ofs = o_idx + al256(4 * n), bytes = o_ofs + al256(8 * n);
+    PinBlock<uint8_t> h(bytes);
+    DevBlock<uint8_t> d(bytes);
+    if (!h || !d) return nullptr;
+    uint64_t *off = (uint64_t *)(h.get() + o_off);
+    uint32_t *hidx = (uint32_t *)(h.get() + o_idx);
+    int64_t *hofs = (int64_t *)(h.get() + o_ofs);
+    uint64_t w = 0, sb = 64, sb_copy = 0;
+    bool any_aligned = false;
+    for (size_t p = 0; p < n; p++) {
+        const uint32_t b = idx ? idx[p] : (uint32_t)p;
+        hidx[p] = b;
+        hofs[p] = offsets[p];
+        off[p] = w;
+        w += 2 * (uint64_t)S->h_cnt[b];
+        if ((offsets[p] & 0xffff) == 0) {
+            any_aligned = true;
+            sb_copy += S->h_bytes[b];
+        } else {
+            sb += 2 * S->h_ebytes[b] + 32 * (uint64_t)S->h_cnt[b];
+        }
+    }
+    off[n] = w;
+    if (w > 0xffffffffull) { t_err = "add_offset: batch too large: more than 2^32 - 1 container slots, split it"; return nullptr; }
+    const bool share = any_aligned && !S->sharing();
+    SetPtr R = set_new((uint32_t)n, w, share ? sb : sb + sb_copy);
+    PassShare sh = {false, false, 0, 0, 0};
+    if (R && share && !share_operands(R.get(), S, S, true, false, sh)) {
+        R.reset();   // out of the offsets' reach: copy everything into a slab sized for it
+        R = set_new((uint32_t)n, w, sb + sb_copy);
+    }
+    ItemsBuf ib_;
+    DevBlock<uint4> cell;
+    bool ok = R && ib_.alloc(w, false, false) && cell.reset(w);
+    if (ok) {
+        for (int k = 0; k < 4; k++) R->ev[k] = ev_get();
+        ok = R->pstats.reset(1) && R->ev[0] && R->ev[1] && R->ev[2] && R->ev[3];
+    }
+    if (ok) {
+        cudaEventRecord(R->ev[0], g.stream);
+        ok = stats_reset() && cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+        const SetView vs = S->view();
+        const uint64_t *d_off = (const uint64_t *)(d.get() + o_off);
+        launch_offset_plan(vs, (const uint32_t *)(d.get() + o_idx), (const int64_t *)(d.get() + o_ofs), d_off,
+                           (uint32_t)n, sh, ib_.it, cell.get(), R->slab_cap, g.d_stats, g.stream);
+        cudaEventRecord(R->ev[1], g.stream);
+        launch_offset_cells(vs, ib_.it, cell.get(), w, sh.bias, R->d_slab, g.d_stats, g.stream);
+        cudaEventRecord(R->ev[2], g.stream);
+        launch_finalize_pairs(vs, vs, ib_.it, d_off, (uint32_t)n, sh, R->out(), g.d_stats, g.stream);
+        ok = ok && cudaMemcpyAsync(R->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+        cudaEventRecord(R->ev[3], g.stream);
+        // no synchronisation here: the counters are taken over by resolve() on first use
+        R->pending = true;
+        R->staging = std::move(h);   // the pinned item layout must outlive its H2D copy
+        R->parentA = S->h_ptr;
+        R->portable_bytes = 0;
+        R->mirrors_pending = n > 0;
+        for (size_t p = 0; p < n; p++) R->h_flags[p] = S->h_flags[hidx[p]] & FLAG_COW;   // roaring.c:2449-2450
+        g.last_op = R.get();
+    }
+    if (!ok) {
+        if (t_err.empty()) t_err = "add_offset: enqueue failed";
+        cudaStreamSynchronize(g.stream);   // the H2D copy of the layout may still read it
+        return nullptr;
+    }
+    return R.release();
+}
+
 // ---- negation: roaring_bitmap_flip (src/roaring.c:2289-2349) ------------------------------------
 // result[k] = S[idx[k]] with [range_start, range_end) negated.  The range is materialised as ONE
 // tiny bitmap of run containers (one {lo, hi-lo} run per key it touches) and every flip is a

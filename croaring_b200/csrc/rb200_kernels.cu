@@ -326,10 +326,10 @@ k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ it
                 ebytes += effective_bytes(ot, it.olen[i], it.ocard[i] & CARD_MASK);
             }
             anyrun |= (ot == T_RUN) ? 1u : 0u;
-            if (kind == K_COMPUTE) {
+            if (kind == K_COMPUTE) {   // (add_offset's cells name a source on one side or none, SRC_NONE)
                 const uint32_t ca = it.ca[i], cb = it.cb[i];
-                bytes += portable_bytes(A.c_type[ca], A.c_len[ca]) +
-                         portable_bytes(B.c_type[cb], B.c_len[cb]) + osz;
+                bytes += (ca != SRC_NONE ? portable_bytes(A.c_type[ca], A.c_len[ca]) : 0u) +
+                         (cb != SRC_NONE ? portable_bytes(B.c_type[cb], B.c_len[cb]) : 0u) + osz;
             } else {   // a copied pass-through container is read and written, a shared one moves nothing
                 bytes += (unsigned long long)(kind == K_COPY_A ? rw_a : rw_b) * osz;
             }

@@ -206,6 +206,12 @@ int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint
 rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t n, uint64_t range_start,
                               uint64_t range_end);
 
+/* result[k] = S[idx[k]] + offsets[k], as roaring_bitmap_add_offset computes it (src/roaring.c:2431), k < n; idx == NULL:
+ * every bitmap in order (n = rb200_set_count(S)).  Any int64 offset; values pushed out of [0, 2^32) are
+ * dropped.  Key-aligned shifts (offset % 65536 == 0) share the operand's containers instead of copying them.
+ * Returns a new resident set, NULL on error (rb200_last_error). */
+rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, size_t n, const int64_t *offsets);
+
 /* 64-bit bitmaps (src/roaring64.c) through their portable format: result[k] =
  * roaring64_bitmap_{and,or,xor,andnot}(a[ia[k]], b[ib[k]]) — the same container grid per
  * high-32 bucket.  *out (pinned, owned by the library; blob k at *out + (*off)[k], (*len)[k]
