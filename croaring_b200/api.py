@@ -201,6 +201,15 @@ def _u32(a):
     return np.ascontiguousarray(a, dtype=np.uint32)
 
 
+def _selection(idx, n_all):
+    """(array, pointer, count) of a selection of bitmaps; idx None selects all n_all of them.  The
+    array is what the pointer points into: keep it alive until the call returns."""
+    if idx is None:
+        return None, None, n_all
+    idx = _u32(idx)
+    return idx, idx.ctypes.data, idx.size
+
+
 class Bitmap:
     """A host roaring_bitmap_t* (reference memory layout) owned by this object."""
 
@@ -653,11 +662,7 @@ class DeviceSet:
         return DeviceSet(lib().rb200_set_repair_after_lazy(self.ptr))
 
     def or_many_heap(self, idx=None):
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         return DeviceSet(lib().rb200_or_many_heap(self.ptr, ip, n))
 
     def and_cardinality(self, other, ia, ib):
@@ -671,21 +676,13 @@ class DeviceSet:
 
     def flip(self, range_start, range_end, idx=None):
         """roaring_bitmap_flip of every (or the selected) bitmap over [range_start, range_end)."""
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         return DeviceSet(lib().rb200_batch_flip(self.ptr, ip, n, int(range_start), int(range_end)))
 
     def add_offset(self, offsets, idx=None):
         """roaring_bitmap_add_offset of every (or the selected) bitmap: result[k] = self[idx[k]] +
         offsets[k].  offsets: one integer for every item, or one per item (int64 range)."""
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         offs = _offsets_i64(offsets, n)   # held until the call returns
         return DeviceSet(lib().rb200_batch_add_offset(self.ptr, ip, n, offs.ctypes.data))
 
@@ -706,11 +703,7 @@ class DeviceSet:
         return out
 
     def or_many(self, idx=None, key_lo=0, key_hi=65535, card_per_key=None):
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         cp = card_per_key.ctypes.data if card_per_key is not None else None
         if card_per_key is not None:
             assert card_per_key.dtype == np.uint32 and card_per_key.size == 65536
@@ -720,11 +713,7 @@ class DeviceSet:
     def or_many_sharded(self, comm, key_lo, key_hi, span, idx=None):
         """rb200_or_many_sharded: (this rank's part as a DeviceSet, uint32 per-key cardinalities of
         the span summed over the ranks, cardinality of the whole union)."""
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         cards = np.zeros(max(0, span[1] - span[0] + 1), dtype=np.uint32)
         tot = C.c_uint64(0)
         p = lib().rb200_or_many_sharded(self.ptr, ip, n, key_lo, key_hi, span[0], span[1], comm.ptr,
@@ -737,11 +726,7 @@ class DeviceSet:
             raise RB200Error(last_error())
 
     def xor_many(self, idx=None):
-        if idx is None:
-            ip, n = None, len(self)
-        else:
-            idx = _u32(idx)
-            ip, n = idx.ctypes.data, idx.size
+        idx, ip, n = _selection(idx, len(self))
         return DeviceSet(lib().rb200_xor_many(self.ptr, ip, n))
 
     def cardinalities(self):

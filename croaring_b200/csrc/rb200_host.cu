@@ -585,6 +585,48 @@ class SyncCall {
     bool timed_, finished_ = false;
 };
 
+// The ending of a batch op that returns as soon as its work is queued: its counters are taken over
+// by resolve() on first use, so consecutive ops pipeline on the stream without a host round trip.
+// begin() gives the result R four events and pinned counters, records the op's start and resets
+// the stats; kernels_begin() / kernels_end() bracket the compute kernel; finish(ok) queues the copy
+// of the counters and the op's end and hands R over, pending, with the staging block its H2D copies
+// read.  A failed call returns NULL (R is freed by its owner) after waiting for the stream while it
+// holds a staging block.  `what` heads the default t_err.
+class DeferredCall {
+   public:
+    DeferredCall(const char *what, SetPtr &R, PinBlock<uint8_t> &staging) : what_(what), R_(R), staging_(staging) {}
+    DeferredCall(const DeferredCall &) = delete;
+    bool begin() {
+        for (int k = 0; k < 4; k++) R_->ev[k] = ev_get();
+        if (!R_->pstats.reset(1) || !R_->ev[0] || !R_->ev[1] || !R_->ev[2] || !R_->ev[3]) return false;
+        cudaEventRecord(R_->ev[0], g.stream);
+        return stats_reset();
+    }
+    void kernels_begin() { cudaEventRecord(R_->ev[1], g.stream); }
+    void kernels_end() { cudaEventRecord(R_->ev[2], g.stream); }
+    rb200_set *finish(bool ok) {
+        if (ok) {
+            ok = cudaMemcpyAsync(R_->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+            cudaEventRecord(R_->ev[3], g.stream);
+        }
+        if (!ok) {
+            if (t_err.empty()) t_err = std::string(what_) + ": enqueue failed";
+            if (staging_) cudaStreamSynchronize(g.stream);
+            return nullptr;
+        }
+        R_->pending = true;
+        R_->staging = std::move(staging_);
+        R_->mirrors_pending = R_->n_bitmaps > 0;  // h_cnt / h_bytes / h_card: see ensure_mirrors()
+        g.last_op = R_.get();
+        return R_.release();
+    }
+
+   private:
+    const char *what_;
+    SetPtr &R_;
+    PinBlock<uint8_t> &staging_;
+};
+
 // The batch op that produced s has run (or was never enqueued): its events, counters and pair list
 // go back to the pools.
 void retire_op(rb200_set *s) {
@@ -1316,6 +1358,60 @@ bool reject_lazy(const rb200_set *s, const char *what) {
     return true;
 }
 
+// The bitmaps S[idx[0..n)] an entry point works on; idx == NULL selects every bitmap of S in order.
+struct Selection {
+    const rb200_set *S;
+    const uint32_t *idx;
+    size_t n;
+    // Refuse a selection the device must never see, before any device call; `what` heads t_err.
+    // n is checked before idx is read, and becomes the set's size when idx is NULL.
+    bool check(const char *what) {
+        if (!S) { t_err = std::string(what) + ": S is NULL"; return false; }
+        if (reject_lazy(S, what)) return false;
+        if (!idx) { n = S->n_bitmaps; return true; }
+        if (n > 0xffffffffull) { t_err = std::string(what) + ": more than 2^32 - 1 bitmaps selected"; return false; }
+        for (size_t k = 0; k < n; k++) {
+            if (idx[k] >= S->n_bitmaps) {
+                t_err = std::string(what) + ": index out of range: idx[" + std::to_string(k) + "] = " +
+                        std::to_string(idx[k]) + ", the set holds " + std::to_string(S->n_bitmaps) + " bitmaps";
+                return false;
+            }
+        }
+        return true;
+    }
+    uint32_t operator[](size_t k) const { return idx ? idx[k] : (uint32_t)k; }
+    bool all() const { return idx == nullptr; }
+    // containers of the selected bitmaps and the OR of their COW flags (S's mirrors must be current)
+    uint64_t containers() const {
+        uint64_t t = 0;
+        for (size_t k = 0; k < n; k++) t += S->h_cnt[(*this)[k]];
+        return t;
+    }
+    uint8_t cow() const {
+        uint8_t f = 0;
+        for (size_t k = 0; k < n; k++) f |= S->h_flags[(*this)[k]];
+        return f & FLAG_COW;
+    }
+    // idx on the device through the pinned block h, which must outlive the copy; d stays NULL for
+    // all(), which the kernels read as the identity
+    bool to_device(DevBlock<uint32_t> &d, PinBlock<uint32_t> &h) const {
+        if (!idx || !n) return true;
+        if (!d.reset(n) || !h.reset(n)) return false;
+        memcpy(h.get(), idx, 4 * n);
+        return cudaMemcpyAsync(d.get(), h.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    }
+};
+
+// Host fields of a one-bitmap result of `containers` bitset slots (or_many, xor_many): the COW flag
+// is propagated from the inputs (roaring_bitmap_lazy_or, roaring.c:2523).
+void fill_single_result(rb200_set *R, uint32_t containers, uint64_t slab_used, const Selection &sel) {
+    R->n_containers = containers;
+    R->slab_used = slab_used;
+    R->h_cnt[0] = containers;
+    R->h_bytes[0] = R->h_ebytes[0] = (uint64_t)containers * BITSET_BYTES;
+    R->h_flags[0] = sel.cow();
+}
+
 // Let R point into A's payload (onA) and / or B's (onB): R holds their slabs and its payload base
 // moves to the lowest of its own slab and their bases.  false (nothing changed) when the span from
 // that base to the end of the highest slab would not fit the 44 bits of a cell descriptor's offsets.
@@ -1384,18 +1480,14 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         }
         ok = R != nullptr;
     }
+    DeferredCall call("batch op", R, pb.h);
+    if (ok) ok = call.begin();
     if (ok) {
-        for (int k = 0; k < 4; k++) R->ev[k] = ev_get();
-        ok = R->pstats.reset(1) && R->ev[0] && R->ev[1] && R->ev[2] && R->ev[3];
-    }
-    if (ok) {
-        cudaEventRecord(R->ev[0], g.stream);
-        ok = stats_reset();
         const SetView va = A->view(), vb = B->view();
         launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, op, false, rules, sh, ib_.it,
                           g.d_stats, g.stream);
         launch_order_items(ib_.it, pb.W, g.d_stats, g.stream);
-        cudaEventRecord(R->ev[1], g.stream);
+        call.kernels_begin();
         // pass-through tickets: one item per lane, fewer lanes when the operands' containers are big
         // (32 x 8 KiB on one warp would be the tail of the launch)
         const uint64_t n_cont = A->n_containers + B->n_containers;
@@ -1405,28 +1497,15 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         static const int ct_env = []() { const char *e = getenv("RB200_COPY_TICKET"); return e ? std::min(32, std::max(1, atoi(e))) : 0; }();
         const int copy_ticket = ct_env ? ct_env : avg_b <= 256 ? 32 : avg_b <= 2048 ? 16 : 8;
         launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_stats, rules, copy_ticket, g.stream);
-        cudaEventRecord(R->ev[2], g.stream);
+        call.kernels_end();
         launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, sh, R->out(), g.d_stats, g.stream);
-        ok = ok && cudaMemcpyAsync(R->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        cudaEventRecord(R->ev[3], g.stream);
-        // no synchronisation here: the counters are taken over by resolve() on first use
-        R->pending = true;
-        R->staging = std::move(pb.h);   // the pinned pair list must outlive its H2D copy
         R->parentA = A->h_ptr;
         R->parentB = B->h_ptr;
-        R->portable_bytes = 0;
-        R->mirrors_pending = np > 0;  // h_cnt / h_bytes / h_card: see ensure_mirrors()
         R->lazy = (rules & RULES_LAZY) != 0 && !(rules & RULES_FLIP);
         for (size_t p = 0; p < np; p++) R->h_flags[p] = (A->h_flags[ia[p]] | B->h_flags[ib[p]]) & FLAG_COW;
-        g.last_op = R.get();
     }
     // the device buffers go back when pb / ib_ leave scope: stream-ordered reuse
-    if (!ok) {
-        if (t_err.empty()) t_err = "batch op: enqueue failed";
-        if (pb.h) cudaStreamSynchronize(g.stream);   // the pair list's H2D copy may still read it
-        return nullptr;
-    }
-    return R.release();
+    return call.finish(ok);
 }
 
 }  // namespace
@@ -1488,7 +1567,9 @@ static float g_last_collective_ms = 0.f;
 static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t n, uint32_t key_lo,
                                uint32_t key_hi, uint32_t *card_per_key, const ShardArgs *sh) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!ctx_init()) return nullptr;
+    Selection sel{S, idx, n};
+    if (!sel.check("or_many") || !ctx_init()) return nullptr;
+    n = sel.n;
     if (key_hi > 65535) key_hi = 65535;
     uint32_t span_n = 0;
     if (sh) {
@@ -1496,19 +1577,11 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         span_n = sh->span_hi - sh->span_lo + 1;
     }
     const bool want_ck = card_per_key != nullptr || sh != nullptr;
-    if (reject_lazy(S, "or_many")) return nullptr;
     if (!ensure_mirrors(S)) return nullptr;
-    if (idx == nullptr) n = S->n_bitmaps;
     // the index (rb200_many2.cu) holds input positions, per-key segments and counts in 32 bits; its
     // entry buffer is sized for every container of the inputs (the host has no per-bitmap keys to
     // count only those of [key_lo, key_hi]), so the container limit covers them all
-    if (n > 0xffffffffu) { t_err = "or_many: more than 2^32 - 1 inputs"; return nullptr; }
-    uint64_t tot = 0;
-    for (size_t i = 0; i < n; i++) {
-        const uint32_t b = idx ? idx[i] : (uint32_t)i;
-        if (b >= S->n_bitmaps) { t_err = "or_many: index out of range"; return nullptr; }
-        tot += S->h_cnt[b];
-    }
+    const uint64_t tot = sel.containers();
     if (tot > 0xffffffffu) { t_err = "or_many: the inputs carry more than 2^32 - 1 containers (every key counts, whatever the key range)"; return nullptr; }
     uint64_t maxk = key_lo <= key_hi ? (uint64_t)key_hi - key_lo + 1 : 0;
     if (tot < maxk) maxk = tot;
@@ -1518,20 +1591,13 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     PinBlock<uint32_t> h_idx, ck;
     DevBlock<uint8_t> d_index;
     SyncCall call("or_many", "or_many launch", true);
-    bool ok = true;
-    if (idx && n) {
-        ok = d_idx.reset(n) && h_idx.reset(n);
-        if (ok) {
-            memcpy(h_idx.get(), idx, 4 * n);
-            ok = cudaMemcpyAsync(d_idx.get(), h_idx.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
-        }
-    }
+    bool ok = sel.to_device(d_idx, h_idx);
     cudaEvent_t evc0 = nullptr, evc1 = nullptr;
     if (ok && want_ck) ok = ck.reset(65536);
     if (ok && sh) { evc0 = ev_get(); evc1 = ev_get(); ok = evc0 && evc1; }
     // index: entries + work-unit table from the device pool
     uint64_t tot_kib = 0;
-    for (size_t i = 0; i < n; i++) tot_kib += (S->h_bytes[idx ? idx[i] : i] >> 10) + 1;
+    for (size_t i = 0; i < n; i++) tot_kib += (S->h_bytes[sel[i]] >> 10) + 1;
     const uint64_t max_units = std::max<uint64_t>(1, std::min<uint64_t>(tot, std::min<uint64_t>(65536, tot) + tot_kib / 32 + 1));
     // key-window index build: per-(window, chunk of 256 bitmaps) key counts when there are several chunks
     const uint64_t m2_chunks = (n + 255) / 256;
@@ -1589,15 +1655,7 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     if (ok) {
         const uint32_t *h_ck = ck.get();
         const uint32_t nk = g.h_stats->nk;
-        R->n_containers = nk;
-        R->slab_used = (uint64_t)nk * BITSET_BYTES;
-        R->h_cnt[0] = nk;
-        R->h_bytes[0] = (uint64_t)nk * BITSET_BYTES;
-        R->h_ebytes[0] = (uint64_t)nk * BITSET_BYTES;
-        uint8_t fl = 0;
-        // roaring_bitmap_lazy_or propagates COW from the inputs (roaring.c:2523)
-        for (size_t i = 0; i < n; i++) fl |= S->h_flags[idx ? idx[i] : i];
-        R->h_flags[0] = fl & FLAG_COW;
+        fill_single_result(R.get(), nk, (uint64_t)nk * BITSET_BYTES, sel);
         if (card_per_key)
             for (int k = 0; k < 65536; k++) card_per_key[k] += h_ck[k];
         if (sh) {
@@ -1612,7 +1670,7 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         // output term is added by the caller-visible stat only when the set is downloaded,
         // here we account inputs exactly from the host mirrors when the whole key space is used.
         uint64_t inb = 0;
-        if (key_lo == 0 && key_hi == 65535 && idx == nullptr) inb = S->portable_bytes;
+        if (key_lo == 0 && key_hi == 65535 && sel.all()) inb = S->portable_bytes;
         g.last_algo_bytes = inb;
     }
     ev_put(evc0);
@@ -1664,17 +1722,9 @@ int rb200_comm_allreduce_u64(rb200_comm_t *comm, uint64_t *d_buf, size_t count) 
 // roaring_bitmap_xor_many (src/roaring.c:795-809) over S[idx[0..n)] (idx == NULL: all, in order).
 rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!ctx_init()) return nullptr;
-    if (reject_lazy(S, "xor_many")) return nullptr;
-    if (!ensure_mirrors(S)) return nullptr;
-    if (idx == nullptr) n = S->n_bitmaps;
-    uint64_t tot = 0;
-    for (size_t i = 0; i < n; i++) {
-        const uint32_t b = idx ? idx[i] : (uint32_t)i;
-        if (b >= S->n_bitmaps) { t_err = "xor_many: index out of range"; return nullptr; }
-        tot += S->h_cnt[b];
-    }
-    const uint64_t maxk = std::min<uint64_t>(65536, tot);
+    Selection sel{S, idx, n};
+    if (!sel.check("xor_many") || !ctx_init() || !ensure_mirrors(S)) return nullptr;
+    const uint64_t maxk = std::min<uint64_t>(65536, sel.containers());
     SetPtr R = set_new(1, maxk, maxk * BITSET_BYTES);
     if (!R) return nullptr;
     DevBlock<uint32_t> d_idx;
@@ -1682,37 +1732,22 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
     DevBlock<uint8_t> t_type(maxk);
     DevBlock<uint32_t> t_card(maxk), t_len(maxk);
     SyncCall call("xor_many", "xor_many launch", true);
-    bool ok = t_type && t_card && t_len;
-    if (ok && idx && n) {
-        ok = d_idx.reset(n) && h_idx.reset(n);
-        if (ok) {
-            memcpy(h_idx.get(), idx, 4 * n);
-            ok = cudaMemcpyAsync(d_idx.get(), h_idx.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
-        }
-    }
+    bool ok = t_type && t_card && t_len && sel.to_device(d_idx, h_idx);
     if (ok) {
         ok = call.begin();
         const SetView vs = S->view();
-        launch_many_mark(vs, d_idx.get(), (uint32_t)n, 0, 65535, g.d_flags, g.stream);
+        launch_many_mark(vs, d_idx.get(), (uint32_t)sel.n, 0, 65535, g.d_flags, g.stream);
         launch_many_compact(g.d_flags, g.d_keys, g.d_stats, g.stream);
         call.kernels_begin();
-        launch_xor_many(vs, d_idx.get(), (uint32_t)n, g.d_keys, t_type.get(), t_card.get(), t_len.get(), R->out(),
+        launch_xor_many(vs, d_idx.get(), (uint32_t)sel.n, g.d_keys, t_type.get(), t_card.get(), t_len.get(), R->out(),
                         g.d_stats, g.stream);
         call.kernels_end();
         call.end();
         ok = call.finish(ok);
     }
     if (ok) {
-        const uint32_t live = (uint32_t)g.h_stats->dir_cursor;
-        R->n_containers = live;
-        R->slab_used = (uint64_t)g.h_stats->nk * BITSET_BYTES;
-        R->h_cnt[0] = live;
-        R->h_bytes[0] = (uint64_t)live * BITSET_BYTES;
-        R->h_ebytes[0] = (uint64_t)live * BITSET_BYTES;
-        uint8_t fl = 0;
-        for (size_t i = 0; i < n; i++) fl |= S->h_flags[idx ? idx[i] : i];
-        R->h_flags[0] = fl & FLAG_COW;
-        g.last_algo_bytes = (idx == nullptr) ? S->portable_bytes : 0;
+        fill_single_result(R.get(), (uint32_t)g.h_stats->dir_cursor, (uint64_t)g.h_stats->nk * BITSET_BYTES, sel);
+        g.last_algo_bytes = sel.all() ? S->portable_bytes : 0;
     }
     return ok ? R.release() : nullptr;
 }
@@ -2832,6 +2867,30 @@ void rb200_bitmaps_free(roaring_bitmap_t **bms, size_t n) {
     pool_for(n, n < 64 ? 1 : host_workers(), 8, [&](size_t i) { bitmap_free_host(bms[i]); });
 }
 
+}  // extern "C"
+
+namespace {
+// Host bitmaps as a temporary set bound to them (rb200_set_bind_host): the callers below keep their
+// inputs alive for the whole call, so a result's pass-through containers are rebuilt from the
+// caller's memory instead of crossing PCIe again.
+SetPtr upload_bound(const roaring_bitmap_t *const *bms, size_t n) {
+    SetPtr S(rb200_set_upload(bms, n));
+    if (S) rb200_set_bind_host(S.get(), 1);
+    return S;
+}
+SetPtr upload_bound(std::initializer_list<const roaring_bitmap_t *> bms) { return upload_bound(bms.begin(), bms.size()); }
+
+// r1 op r2 under `rules` on the batched path: the resident result, NULL on failure (t_err).
+SetPtr pair_result(int op, const roaring_bitmap_t *r1, const roaring_bitmap_t *r2, int rules) {
+    const SetPtr S = upload_bound({r1, r2});
+    if (!S) return nullptr;
+    const uint32_t ia = 0, ib = 1;
+    return SetPtr(batch_op_impl(op, S.get(), S.get(), &ia, &ib, 1, rules));
+}
+}  // namespace
+
+extern "C" {
+
 int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_bitmap_t *const *b,
                         size_t np, roaring_bitmap_t **out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
@@ -2844,9 +2903,8 @@ int rb200_batch_op_host(int op, const roaring_bitmap_t *const *a, const roaring_
         ia[p] = (uint32_t)p;
         ib[p] = (uint32_t)(np + p);
     }
-    SetPtr S(rb200_set_upload(all.data(), all.size()));
+    const SetPtr S = upload_bound(all.data(), all.size());
     if (!S) return -1;
-    rb200_set_bind_host(S.get(), 1);  // the inputs outlive this call
     SetPtr R(batch_op_impl(op, S.get(), S.get(), ia.data(), ib.data(), np));
     return R ? rb200_set_download_all(R.get(), out) : -1;
 }
@@ -2989,36 +3047,17 @@ roaring_bitmap_t *roaring_bitmap_andnot(const roaring_bitmap_t *r1, const roarin
 
 roaring_bitmap_t *roaring_bitmap_or_many(size_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    SetPtr S(rb200_set_upload(rs, number));
+    const SetPtr S = upload_bound(rs, number);
     if (!S) return nullptr;
     SetPtr R(rb200_or_many(S.get(), nullptr, number));
     return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 
-// In-place twins (src/roaring.c:812 and_inplace, :1063 or_inplace, :1200 xor_inplace, :1342
-// andnot_inplace): the result is computed on the device with the in-place type rules and then
-// swapped into x1 (its old containers and directory are released, its flags kept).
-// replace x1's directory and containers by those of `out` (consumed); x1 keeps its flags
-static void swap_into(roaring_bitmap_t *x1, roaring_bitmap_t *out);
-static void dropin_inplace(int op, roaring_bitmap_t *x1, const roaring_bitmap_t *x2, int rules = RULES_INPLACE) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (rules == RULES_INPLACE) {   // (the lazy in-place twins take the batched path)
-        roaring_bitmap_t *fo = nullptr;
-        const int f = pair_fused(op, x1, x2, RULES_INPLACE, &fo);
-        if (f == 1) { swap_into(x1, fo); return; }
-        if (f < 0) { dropin_failed("roaring_bitmap_*_inplace"); return; }
-    }
-    const roaring_bitmap_t *both[2] = {x1, x2};
-    SetPtr S(rb200_set_upload(both, 2));
-    if (!S) { dropin_failed("roaring_bitmap_*_inplace"); return; }
-    rb200_set_bind_host(S.get(), 1);
-    const uint32_t ia = 0, ib = 1;
-    roaring_bitmap_t *out = nullptr;
-    if (SetPtr R{batch_op_impl(op, S.get(), S.get(), &ia, &ib, 1, rules)}) out = rb200_set_download(R.get(), 0);
-    if (!out) { dropin_failed("roaring_bitmap_*_inplace"); return; }  // x1 is left untouched
-    swap_into(x1, out);
-}
-static void swap_into(roaring_bitmap_t *x1, roaring_bitmap_t *out) {
+// The end of an in-place call: the result `out` (consumed) replaces x1's directory and containers
+// (the old ones are released, x1's flags kept); without a result x1 is left untouched and the
+// failure of `fn` is reported.
+static void finish_inplace(roaring_bitmap_t *x1, roaring_bitmap_t *out, const char *fn) {
+    if (!out) { dropin_failed(fn); return; }
     roaring_array_t *ra = &x1->high_low_container, *rn = &out->high_low_container;
     const uint8_t flags = ra->flags;
     if (!(flags & FLAG_FROZEN)) {
@@ -3028,6 +3067,20 @@ static void swap_into(roaring_bitmap_t *x1, roaring_bitmap_t *out) {
     *ra = *rn;
     ra->flags = flags;
     h_free(out);
+}
+// In-place twins (src/roaring.c:812 and_inplace, :1063 or_inplace, :1200 xor_inplace, :1342
+// andnot_inplace): the result is computed on the device with the in-place type rules and then
+// swapped into x1.
+static void dropin_inplace(int op, roaring_bitmap_t *x1, const roaring_bitmap_t *x2, int rules = RULES_INPLACE) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    roaring_bitmap_t *out = nullptr;
+    // (the lazy in-place twins take the batched path)
+    const int f = rules == RULES_INPLACE ? pair_fused(op, x1, x2, RULES_INPLACE, &out) : 0;
+    if (f == 0) {
+        const SetPtr R = pair_result(op, x1, x2, rules);
+        out = R ? rb200_set_download(R.get(), 0) : nullptr;
+    }
+    finish_inplace(x1, out, "roaring_bitmap_*_inplace");
 }
 void roaring_bitmap_and_inplace(roaring_bitmap_t *x1, const roaring_bitmap_t *x2) {
     if (x1 == x2) return;  // roaring.c:814
@@ -3039,7 +3092,7 @@ void roaring_bitmap_andnot_inplace(roaring_bitmap_t *x1, const roaring_bitmap_t 
 
 roaring_bitmap_t *roaring_bitmap_xor_many(size_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    SetPtr S(rb200_set_upload(rs, number));
+    const SetPtr S = upload_bound(rs, number);
     if (!S) return nullptr;
     SetPtr R(rb200_xor_many(S.get(), nullptr, number));
     return R ? rb200_set_download(R.get(), 0) : nullptr;
@@ -3047,8 +3100,7 @@ roaring_bitmap_t *roaring_bitmap_xor_many(size_t number, const roaring_bitmap_t 
 
 uint64_t roaring_bitmap_and_cardinality(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const roaring_bitmap_t *both[2] = {r1, r2};
-    SetPtr S(rb200_set_upload(both, 2));
+    const SetPtr S = upload_bound({r1, r2});
     if (!S) return UINT64_MAX;
     const uint32_t ia = 0, ib = 1;
     uint64_t out = UINT64_MAX;
@@ -3104,8 +3156,7 @@ int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint
 }
 static int dropin_relation(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const roaring_bitmap_t *both[2] = {r1, r2};
-    SetPtr S(rb200_set_upload(both, 2));
+    const SetPtr S = upload_bound({r1, r2});
     if (!S) { dropin_failed("roaring_bitmap_equals / is_subset / is_strict_subset"); return -1; }
     const uint32_t ia = 0, ib = 1;
     uint8_t out = 0;
@@ -3134,18 +3185,9 @@ bool roaring_bitmap_is_strict_subset(const roaring_bitmap_t *r1, const roaring_b
 rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, size_t n, const int64_t *offsets) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     if (!offsets) { t_err = "add_offset: offsets is NULL"; return nullptr; }
-    if (!S) { t_err = "add_offset: S is NULL"; return nullptr; }
-    if (idx == nullptr) n = S->n_bitmaps;
-    if (n > 0xffffffffull) { t_err = "add_offset: n must be below 2^32"; return nullptr; }
-    for (size_t k = 0; idx && k < n; k++) {
-        if (idx[k] >= S->n_bitmaps) {
-            t_err = "add_offset: idx[" + std::to_string(k) + "] = " + std::to_string(idx[k]) +
-                    " is out of range (the set holds " + std::to_string(S->n_bitmaps) + " bitmaps)";
-            return nullptr;
-        }
-    }
-    if (reject_lazy(S, "add_offset")) return nullptr;
-    if (!ctx_init() || !ensure_mirrors(S)) return nullptr;
+    Selection sel{S, idx, n};
+    if (!sel.check("add_offset") || !ctx_init() || !ensure_mirrors(S)) return nullptr;
+    n = sel.n;
     // item slots and the result slab, sized from the host mirrors before the launch.  A computed
     // container holds at most min(8192, 2 x its cardinality) bytes (offset_type: a run is kept only
     // when it is no larger, a bitset only above 4096 values), and its parts come from at most two
@@ -3161,7 +3203,7 @@ rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, s
     uint64_t w = 0, sb = 64, sb_copy = 0;
     bool any_aligned = false;
     for (size_t p = 0; p < n; p++) {
-        const uint32_t b = idx ? idx[p] : (uint32_t)p;
+        const uint32_t b = sel[p];
         hidx[p] = b;
         hofs[p] = offsets[p];
         off[p] = w;
@@ -3184,39 +3226,22 @@ rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, s
     }
     ItemsBuf ib_;
     DevBlock<uint4> cell;
-    bool ok = R && ib_.alloc(w, false, false) && cell.reset(w);
+    DeferredCall call("add_offset", R, h);
+    const bool ok = R && ib_.alloc(w, false, false) && cell.reset(w) && call.begin() &&
+                    cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
     if (ok) {
-        for (int k = 0; k < 4; k++) R->ev[k] = ev_get();
-        ok = R->pstats.reset(1) && R->ev[0] && R->ev[1] && R->ev[2] && R->ev[3];
-    }
-    if (ok) {
-        cudaEventRecord(R->ev[0], g.stream);
-        ok = stats_reset() && cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
         const SetView vs = S->view();
         const uint64_t *d_off = (const uint64_t *)(d.get() + o_off);
         launch_offset_plan(vs, (const uint32_t *)(d.get() + o_idx), (const int64_t *)(d.get() + o_ofs), d_off,
                            (uint32_t)n, sh, ib_.it, cell.get(), R->slab_cap, g.d_stats, g.stream);
-        cudaEventRecord(R->ev[1], g.stream);
+        call.kernels_begin();
         launch_offset_cells(vs, ib_.it, cell.get(), w, sh.bias, R->d_slab, g.d_stats, g.stream);
-        cudaEventRecord(R->ev[2], g.stream);
+        call.kernels_end();
         launch_finalize_pairs(vs, vs, ib_.it, d_off, (uint32_t)n, sh, R->out(), g.d_stats, g.stream);
-        ok = ok && cudaMemcpyAsync(R->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-        cudaEventRecord(R->ev[3], g.stream);
-        // no synchronisation here: the counters are taken over by resolve() on first use
-        R->pending = true;
-        R->staging = std::move(h);   // the pinned item layout must outlive its H2D copy
         R->parentA = S->h_ptr;
-        R->portable_bytes = 0;
-        R->mirrors_pending = n > 0;
         for (size_t p = 0; p < n; p++) R->h_flags[p] = S->h_flags[hidx[p]] & FLAG_COW;   // roaring.c:2449-2450
-        g.last_op = R.get();
     }
-    if (!ok) {
-        if (t_err.empty()) t_err = "add_offset: enqueue failed";
-        cudaStreamSynchronize(g.stream);   // the H2D copy of the layout may still read it
-        return nullptr;
-    }
-    return R.release();
+    return call.finish(ok);
 }
 
 // ---- negation: roaring_bitmap_flip (src/roaring.c:2289-2349) ------------------------------------
@@ -3226,11 +3251,10 @@ rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, s
 rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t n, uint64_t range_start,
                               uint64_t range_end) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!ctx_init()) return nullptr;
-    if (reject_lazy(S, "flip")) return nullptr;
-    if (idx == nullptr) n = S->n_bitmaps;
-    std::vector<uint32_t> ia(n), ib(n, 0);
-    for (size_t i = 0; i < n; i++) ia[i] = idx ? idx[i] : (uint32_t)i;
+    Selection sel{S, idx, n};
+    if (!sel.check("flip") || !ctx_init()) return nullptr;
+    std::vector<uint32_t> ia(sel.n), ib(sel.n, 0);
+    for (size_t i = 0; i < sel.n; i++) ia[i] = sel[i];
     // roaring.c:2292 (open range empty / start past the 32-bit universe) and :2303 (the CLOSED
     // range, after the reference's truncation of both ends to 32 bits, is empty): plain copy, the
     // symmetric difference with the empty bitmap
@@ -3252,26 +3276,20 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     const size_t bl = blob.size();
     SetPtr Rg(upload_blobs_impl(&bp, &bl, 1, false));
     if (!Rg) return nullptr;
-    return batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
+    return batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), sel.n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
 }
 roaring_bitmap_t *roaring_bitmap_flip(const roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const roaring_bitmap_t *one[1] = {r1};
-    SetPtr S(rb200_set_upload(one, 1));
+    const SetPtr S = upload_bound({r1});
     if (!S) return nullptr;
-    rb200_set_bind_host(S.get(), 1);
     SetPtr R(rb200_batch_flip(S.get(), nullptr, 1, range_start, range_end));
     return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 void roaring_bitmap_flip_inplace(roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {
     if (range_start >= range_end || range_start > (uint64_t)UINT32_MAX + 1) return;  // roaring.c:2353
     if ((uint32_t)range_start > (uint32_t)(range_end - 1)) return;                    // roaring.c:2364
-    roaring_bitmap_t *out = roaring_bitmap_flip(r1, range_start, range_end);
-    if (!out) dropin_failed("roaring_bitmap_flip_inplace");
-    if (out) {
-        std::lock_guard<std::recursive_mutex> lk(g.mu);
-        swap_into(r1, out);
-    }
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    finish_inplace(r1, roaring_bitmap_flip(r1, range_start, range_end), "roaring_bitmap_flip_inplace");
 }
 
 // ---- 64-bit bitmaps resident on the device (src/roaring64.c) -------------------------------
@@ -3851,37 +3869,27 @@ bool roaring64_bitmap_intersect(const roaring64_bitmap_t *r1, const roaring64_bi
 // ---- public lazy API (include/roaring/roaring.h:932-977) ------------------------------------
 // The lazy state lives in ordinary host bitmaps exactly as the reference leaves it (bitsets with
 // cardinality -1, unconverted runs), so the reference's own functions accept what we return.
-static roaring_bitmap_t *dropin_lazy_pair(int op, const roaring_bitmap_t *r1, const roaring_bitmap_t *r2, int rules) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const roaring_bitmap_t *both[2] = {r1, r2};
-    SetPtr S(rb200_set_upload(both, 2));
-    if (!S) return nullptr;
-    rb200_set_bind_host(S.get(), 1);
-    const uint32_t ia = 0, ib = 1;
-    SetPtr R(batch_op_impl(op, S.get(), S.get(), &ia, &ib, 1, rules));
-    return R ? rb200_set_download(R.get(), 0) : nullptr;
-}
 roaring_bitmap_t *roaring_bitmap_lazy_or(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2, const bool bitsetconversion) {
-    return dropin_lazy_pair(OP_OR, r1, r2, RULES_LAZY | (bitsetconversion ? RULES_CONV : 0));
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    const SetPtr R = pair_result(OP_OR, r1, r2, RULES_LAZY | (bitsetconversion ? RULES_CONV : 0));
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 void roaring_bitmap_lazy_or_inplace(roaring_bitmap_t *r1, const roaring_bitmap_t *r2, const bool bitsetconversion) {
     dropin_inplace(OP_OR, r1, r2, RULES_LAZY | RULES_INPLACE | (bitsetconversion ? RULES_CONV : 0));
 }
 roaring_bitmap_t *roaring_bitmap_lazy_xor(const roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
-    return dropin_lazy_pair(OP_XOR, r1, r2, RULES_LAZY);
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    const SetPtr R = pair_result(OP_XOR, r1, r2, RULES_LAZY);
+    return R ? rb200_set_download(R.get(), 0) : nullptr;
 }
 void roaring_bitmap_lazy_xor_inplace(roaring_bitmap_t *r1, const roaring_bitmap_t *r2) {
     dropin_inplace(OP_XOR, r1, r2, RULES_LAZY | RULES_INPLACE);
 }
 void roaring_bitmap_repair_after_lazy(roaring_bitmap_t *r1) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    const roaring_bitmap_t *one[1] = {r1};
-    SetPtr S(rb200_set_upload(one, 1));
-    if (!S) { dropin_failed("roaring_bitmap_repair_after_lazy"); return; }
-    roaring_bitmap_t *out = nullptr;
-    if (SetPtr R{rb200_set_repair_after_lazy(S.get())}) out = rb200_set_download(R.get(), 0);
-    if (out) swap_into(r1, out);
-    else dropin_failed("roaring_bitmap_repair_after_lazy");
+    const SetPtr S = upload_bound({r1});
+    const SetPtr R(S ? rb200_set_repair_after_lazy(S.get()) : nullptr);
+    finish_inplace(r1, R ? rb200_set_download(R.get(), 0) : nullptr, "roaring_bitmap_repair_after_lazy");
 }
 
 // ---- roaring_bitmap_or_many_heap (src/roaring_priority_queue.c:200-250) ------------------------
@@ -3952,30 +3960,24 @@ bool portable_sizes(const rb200_set *S, std::vector<uint32_t> &out) {
 
 rb200_set_t *rb200_or_many_heap(const rb200_set_t *S, const uint32_t *idx, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!ctx_init()) return nullptr;
-    if (reject_lazy(S, "or_many_heap")) return nullptr;
-    if (idx == nullptr) n = S->n_bitmaps;
-    for (size_t i = 0; i < n; i++)
-        if (idx && idx[i] >= S->n_bitmaps) { t_err = "or_many_heap: index out of range"; return nullptr; }
-    if (n == 0) return rb200_or_many(S, idx, 0);
-    if (n == 1) {  // roaring_bitmap_copy: union with an empty bitmap = pass-through of every container
+    Selection sel{S, idx, n};
+    if (!sel.check("or_many_heap") || !ctx_init()) return nullptr;
+    if (sel.n == 0) return rb200_or_many(S, idx, 0);
+    if (sel.n == 1) {  // roaring_bitmap_copy: union with an empty bitmap = pass-through of every container
         roaring_bitmap_t *e = bitmap_alloc(0);
         if (!e) return nullptr;
         const roaring_bitmap_t *one[1] = {e};
         SetPtr E(rb200_set_upload(one, 1));
         bitmap_free_host(e);
         if (!E) return nullptr;
-        const uint32_t a = idx ? idx[0] : 0u, z = 0;
+        const uint32_t a = sel[0], z = 0;
         return batch_op_impl(OP_OR, S, E.get(), &a, &z, 1, 0);
     }
     std::vector<uint32_t> sz;
     if (!portable_sizes(S, sz)) return nullptr;
-    std::vector<HeapEl> e(n);
-    for (size_t i = 0; i < n; i++) {
-        const uint32_t b = idx ? idx[i] : (uint32_t)i;
-        e[i] = HeapEl{sz[b], false, const_cast<rb200_set *>(S), b};
-    }
-    uint32_t cnt = (uint32_t)n;
+    std::vector<HeapEl> e(sel.n);
+    for (size_t i = 0; i < sel.n; i++) e[i] = HeapEl{sz[sel[i]], false, const_cast<rb200_set *>(S), sel[i]};
+    uint32_t cnt = (uint32_t)sel.n;
     for (int32_t i = (int32_t)(cnt >> 1); i >= 0; i--) heap_down(e, cnt, (uint32_t)i);  // create_pq :68-82
     bool ok = true;
     while (cnt > 1 && ok) {
@@ -4003,7 +4005,7 @@ rb200_set_t *rb200_or_many_heap(const rb200_set_t *S, const uint32_t *idx, size_
 
 roaring_bitmap_t *roaring_bitmap_or_many_heap(uint32_t number, const roaring_bitmap_t **rs) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    SetPtr S(rb200_set_upload(rs, number));
+    const SetPtr S = upload_bound(rs, number);
     if (!S) return nullptr;
     SetPtr R(rb200_or_many_heap(S.get(), nullptr, number));
     return R ? rb200_set_download(R.get(), 0) : nullptr;

@@ -202,6 +202,11 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
 int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint32_t *ia,
                           const uint32_t *ib, size_t npairs, uint8_t *out);
 
+/* Selections.  rb200_batch_flip, rb200_batch_add_offset and the or_many / xor_many entry points work on
+ * S[idx[0..n)]; idx == NULL selects every bitmap of S in order (n is then ignored).  A NULL or lazy S, and
+ * with an idx, n >= 2^32 or an entry out of range, is refused before any device work; rb200_last_error()
+ * names the entry point. */
+
 /* result[k] = roaring_bitmap_flip(S[idx[k]], range_start, range_end) (idx == NULL: every bitmap). */
 rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t n, uint64_t range_start,
                               uint64_t range_end);

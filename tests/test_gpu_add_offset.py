@@ -132,7 +132,7 @@ def test_refusals(rb, R):
     lz = S.batch("or", S, one(0), one(1), lazy=True)
     with pytest.raises(rb.RB200Error, match="lazy"):
         lz.add_offset(5)
-    with pytest.raises(rb.RB200Error, match=r"idx\[1\] = 6 is out of range"):
+    with pytest.raises(rb.RB200Error, match=r"add_offset: index out of range: idx\[1\] = 6"):
         S.add_offset([1, 2], np.array([0, 6], np.uint32))
     L = rb.lib()
     assert not L.rb200_batch_add_offset(S.ptr, None, 0, None)

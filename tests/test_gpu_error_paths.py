@@ -46,6 +46,8 @@ def _cases(rb, R, blobs, S, lazy, S64):
     vals = torch.arange(10, dtype=torch.int32, device="cuda")
     offs = torch.tensor([0, 6, 3, 10], dtype=torch.int64, device="cuda")
     torch.cuda.synchronize()
+    lib = rb.api.lib()
+    two = np.array([0, 1], dtype=np.uint32)   # n = 2^32 with two entries: refused before idx is read
     return [
         ("batch_op", lambda: S.batch("or", S, [0, 1, 2], [1, 99, 3]), "pair index out of range"),
         ("batch_and_cardinality", lambda: S.and_cardinality(S, [0, 99], [1, 2]), "pair index out of range"),
@@ -53,6 +55,12 @@ def _cases(rb, R, blobs, S, lazy, S64):
         ("or_many", lambda: S.or_many(idx=[0, 99]), "or_many: index out of range"),
         ("xor_many", lambda: S.xor_many(idx=[0, 99]), "xor_many: index out of range"),
         ("or_many_heap", lambda: S.or_many_heap(idx=[0, 99]), "or_many_heap: index out of range"),
+        ("flip", lambda: S.flip(0, 1 << 20, idx=[0, 99]), "flip: index out of range: idx[1] = 99"),
+        ("add_offset", lambda: S.add_offset(5, idx=[0, 99]), "add_offset: index out of range: idx[1] = 99"),
+        ("xor_many n = 2^32", lambda: rb.DeviceSet(lib.rb200_xor_many(S.ptr, two.ctypes.data, 1 << 32)),
+         "xor_many: more than 2^32 - 1 bitmaps selected"),
+        ("or_many_heap n = 2^32", lambda: rb.DeviceSet(lib.rb200_or_many_heap(S.ptr, two.ctypes.data, 1 << 32)),
+         "or_many_heap: more than 2^32 - 1 bitmaps selected"),
         ("lazy batch_op", lambda: lazy.batch("and", lazy, [0], [1]), "batch op: the set is in a lazy state"),
         ("lazy serialize", lambda: lazy.serialize_all(), "serialize: the set is in a lazy state"),
         ("lazy flip", lambda: lazy.flip(0, 1 << 20), "flip: the set is in a lazy state"),

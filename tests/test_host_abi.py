@@ -185,6 +185,25 @@ def test_compute_fails_loudly_without_gpu():
         rb.DeviceSet.upload([a])
 
 
+def test_selection_entry_points_refuse_a_null_set_before_any_device():
+    """Every entry point that takes a selection of bitmaps (S, idx, n) refuses S == NULL with its
+    own name, before it touches the device (with or without one)."""
+    L = rb.lib()
+    offs = (ctypes.c_int64 * 1)(5)
+    calls = [
+        ("or_many", lambda: L.rb200_or_many(None, None, 1)),
+        ("or_many", lambda: L.rb200_or_many_keyrange(None, None, 1, 0, 65535, None)),
+        ("or_many", lambda: L.rb200_or_many_sharded(None, None, 1, 0, 65535, 0, 65535, None, None, None)),
+        ("xor_many", lambda: L.rb200_xor_many(None, None, 1)),
+        ("or_many_heap", lambda: L.rb200_or_many_heap(None, None, 1)),
+        ("add_offset", lambda: L.rb200_batch_add_offset(None, None, 1, ctypes.cast(offs, ctypes.c_void_p))),
+        ("flip", lambda: L.rb200_batch_flip(None, None, 1, 0, 10)),
+    ]
+    for what, call in calls:
+        assert not call(), what
+        assert rb.last_error() == f"{what}: S is NULL"
+
+
 def test_mutated_blobs_never_crash_the_host_parsers(R):
     """Seeded mutation fuzz of the host-side portable-format entry points (walk_portable behind
     rb200_bitmap_portable_deserialize_safe and behind the blob algebra of rb200_shard.cu):
