@@ -91,6 +91,10 @@ def lib():
     sig("rb200_set_op_stats", C.c_int, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64))
     sig("rb200_batch_flip", _P, _P, _P, C.c_size_t, C.c_uint64, C.c_uint64)
     sig("rb200_batch_add_offset", _P, _P, _P, C.c_size_t, _P)
+    for name in ("rb200_batch_add_many", "rb200_batch_remove_many", "rb200_set64_batch_add_many",
+                 "rb200_set64_batch_remove_many"):
+        sig(name, _P, _P, _P, C.c_size_t, _P, _P)
+        sig(name + "_device", _P, _P, _P, C.c_size_t, _P, _P)
     sig("rb200_r64_batch_op_serialized", C.c_int, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
         C.c_size_t, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t, _P, _P, C.c_size_t,
         C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)), C.POINTER(C.POINTER(C.c_uint64)))
@@ -546,6 +550,40 @@ def _offsets_i64(offsets, n):
     return np.ascontiguousarray(a, dtype=np.int64)
 
 
+def _device_offsets(values, offsets):
+    """Offsets of CUDA tensor values (n + 1 entries, as a CUDA or CPU tensor or an array) as a
+    contiguous tensor on the values' device, ready for the library stream."""
+    import torch
+    if offsets is None:
+        raise RB200Error("device values need offsets")
+    offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
+    if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
+        raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
+    last = int(offs[-1].item())
+    if last < 0 or last > values.numel():
+        raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
+    offs = offs.to(values.device).contiguous()
+    if offs is not offsets:   # copied here: on the stream the library reads on
+        torch.cuda.current_stream(values.device).synchronize()
+    return offs
+
+
+def _update(s, fn, values, offsets, idx):
+    """fn (an add_many / remove_many entry point; fn + "_device" for CUDA tensor values) on the
+    selection idx of the set s, with one list of values per selected bitmap."""
+    idx, ip, n = _selection(idx, len(s))
+    if getattr(values, "is_cuda", False):
+        offs = s._device_offsets(values, offsets)
+        vp, op, m = values.data_ptr(), offs.data_ptr(), offs.numel() - 1
+        fn += "_device"
+    else:
+        flat, offs = s._host_values(values, offsets)   # held until the call returns
+        vp, op, m = flat.ctypes.data, offs.ctypes.data, offs.size - 1
+    if m != n:
+        raise RB200Error(f"{m} lists of values for {n} items")
+    return getattr(lib(), fn)(s.ptr, ip, n, vp, op)
+
+
 class DeviceSet:
     """An ordered collection of bitmaps resident in HBM (rb200_set_t*)."""
 
@@ -586,6 +624,17 @@ class DeviceSet:
         (order its writes before the call, e.g. by building it on the stream given to set_stream)."""
         if getattr(values, "is_cuda", False):
             return cls._from_device_values(values, offsets)
+        flat, offs = cls._host_values(values, offsets)
+        return cls(lib().rb200_set_from_uint32(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+
+    @classmethod
+    def _from_device_values(cls, values, offsets):
+        offs = cls._device_offsets(values, offsets)
+        return cls(lib().rb200_set_from_uint32_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
+
+    @staticmethod
+    def _host_values(values, offsets):
+        """(flat uint32 values, uint64 offsets) of the host forms from_values takes."""
         if offsets is None:
             arrays = [np.asarray(a).reshape(-1) for a in values]
             offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
@@ -596,25 +645,15 @@ class DeviceSet:
             offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
             if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
                 raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
-        return cls(lib().rb200_set_from_uint32(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+        return flat, offs
 
-    @classmethod
-    def _from_device_values(cls, values, offsets):
+    @staticmethod
+    def _device_offsets(values, offsets):
+        """The offsets of CUDA tensor values as a contiguous tensor on the values' device."""
         import torch
         if values.dtype not in (torch.int32, torch.uint32) or values.dim() != 1 or not values.is_contiguous():
             raise RB200Error("device values must be a contiguous 1-D int32 / uint32 CUDA tensor")
-        if offsets is None:
-            raise RB200Error("device values need offsets")
-        offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
-        if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
-            raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
-        last = int(offs[-1].item())
-        if last < 0 or last > values.numel():
-            raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
-        offs = offs.to(values.device).contiguous()
-        if offs is not offsets:   # copied here: on the stream the library reads on
-            torch.cuda.current_stream(values.device).synchronize()
-        return cls(lib().rb200_set_from_uint32_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
+        return _device_offsets(values, offsets)
 
     def free(self):
         if self.ptr:
@@ -685,6 +724,15 @@ class DeviceSet:
         idx, ip, n = _selection(idx, len(self))
         offs = _offsets_i64(offsets, n)   # held until the call returns
         return DeviceSet(lib().rb200_batch_add_offset(self.ptr, ip, n, offs.ctypes.data))
+
+    def add_many(self, values, offsets=None, idx=None):
+        """roaring_bitmap_add_many of every (or the selected) bitmap: result[k] = self[idx[k]] with the
+        values of item k added.  values: any form from_values takes, one list of values per item."""
+        return DeviceSet(_update(self, "rb200_batch_add_many", values, offsets, idx))
+
+    def remove_many(self, values, offsets=None, idx=None):
+        """roaring_bitmap_remove_many of every (or the selected) bitmap, as add_many."""
+        return DeviceSet(_update(self, "rb200_batch_remove_many", values, offsets, idx))
 
     def op_stats(self):
         """(device_ms, compute_kernel_ms, algorithmic_bytes) of the batch op that produced this set."""
@@ -876,6 +924,17 @@ class DeviceSet64:
         uint64) with offsets as a CUDA or CPU tensor, read in place on the library stream."""
         if getattr(values, "is_cuda", False):
             return cls._from_device_values(values, offsets)
+        flat, offs = cls._host_values(values, offsets)
+        return cls(lib().rb200_set64_from_uint64(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+
+    @classmethod
+    def _from_device_values(cls, values, offsets):
+        offs = cls._device_offsets(values, offsets)
+        return cls(lib().rb200_set64_from_uint64_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
+
+    @staticmethod
+    def _host_values(values, offsets):
+        """(flat uint64 values, uint64 offsets) of the host forms from_values takes."""
         if offsets is None:
             arrays = [np.asarray(a).reshape(-1) for a in values]
             offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
@@ -886,25 +945,15 @@ class DeviceSet64:
             offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
             if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
                 raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
-        return cls(lib().rb200_set64_from_uint64(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
+        return flat, offs
 
-    @classmethod
-    def _from_device_values(cls, values, offsets):
+    @staticmethod
+    def _device_offsets(values, offsets):
+        """The offsets of CUDA tensor values as a contiguous tensor on the values' device."""
         import torch
         if values.dtype not in (torch.int64, torch.uint64) or values.dim() != 1 or not values.is_contiguous():
             raise RB200Error("device values must be a contiguous 1-D int64 / uint64 CUDA tensor")
-        if offsets is None:
-            raise RB200Error("device values need offsets")
-        offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
-        if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
-            raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
-        last = int(offs[-1].item())
-        if last < 0 or last > values.numel():
-            raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
-        offs = offs.to(values.device).contiguous()
-        if offs is not offsets:   # copied here: on the stream the library reads on
-            torch.cuda.current_stream(values.device).synchronize()
-        return cls(lib().rb200_set64_from_uint64_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
+        return _device_offsets(values, offsets)
 
     def free(self):
         if self.ptr:
@@ -941,6 +990,15 @@ class DeviceSet64:
         if lib().rb200_set64_cardinalities(self.ptr, out.ctypes.data) != 0:
             raise RB200Error(last_error())
         return out
+
+    def add_many(self, values, offsets=None, idx=None):
+        """roaring64_bitmap_add_many of every (or the selected) bitmap: result[k] = self[idx[k]] with the
+        values of item k added.  values: any form from_values takes, one list of values per item."""
+        return DeviceSet64(_update(self, "rb200_set64_batch_add_many", values, offsets, idx))
+
+    def remove_many(self, values, offsets=None, idx=None):
+        """roaring64_bitmap_remove_many of every (or the selected) bitmap, as add_many."""
+        return DeviceSet64(_update(self, "rb200_set64_batch_remove_many", values, offsets, idx))
 
     def run_optimize(self, mode=1):
         """mode 1: roaring64_bitmap_run_optimize of every bitmap; mode 0: the run containers removed."""

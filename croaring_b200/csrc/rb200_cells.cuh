@@ -12,6 +12,14 @@ namespace rb200 {
 #endif
 
 // ------------------------------------------------------------------------------ grid cells
+// add_many / remove_many (RULES_KEEP_RUN): the cell's left run stays a run, counted and emitted at any
+// length.  cell_compute evaluates this where it is used: one flag held live across the cell costs the
+// OR and ANDNOT kernels spills.
+template <int OP, bool LAZY>
+__device__ __forceinline__ bool keep_run_cell(int rules, int tA) {
+    return !LAZY && (OP == OP_OR || OP == OP_ANDNOT) && (rules & RULES_KEEP_RUN) && tA == T_RUN;
+}
+
 // Evaluate one matched cell on the warp's accumulator and write the result payload.
 template <int OP, bool LAZY>
 __device__ __forceinline__ void
@@ -26,7 +34,7 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
     constexpr uint32_t AV = (OP == OP_OR || OP == OP_XOR) ? APPLY_VECS_OR : APPLY_VECS;   // array rasterise batch
     if (!lazy && (tA == T_RUN || tB == T_RUN) && tA != T_BITSET && tB != T_BITSET &&
         (tA == T_RUN ? lA : cA) + (tB == T_RUN ? lB : cB) <= 512u) {
-        if (interval_cell(acc, op, tA, tB, pa, pb, cA, cB, lA, lB, out, cap, lane, otype, ocard, olen))
+        if (interval_cell(acc, op, tA, tB, pa, pb, cA, cB, lA, lB, out, cap, lane, otype, ocard, olen, keep_run_cell<OP, LAZY>(rules, tA)))
             return;
     }
 
@@ -160,12 +168,12 @@ cell_compute(uint32_t *acc, int tA, int tB, const uint8_t *pa, const uint8_t *pb
         __syncwarp();
     }
     const bool want_runs = lazy ? ((tA == T_RUN || tB == T_RUN) && tA != T_BITSET && tB != T_BITSET)
-                                : cell_needs_runs(op, tA, tB);
+                                : (keep_run_cell<OP, LAZY>(rules, tA) || cell_needs_runs(op, tA, tB));
     if (card < 0 || want_runs) acc_count(acc, lane, want_runs, card, nruns);
     if (card == 0) { otype = 0; ocard = olen = 0; return; }
     bool unknown = false;
     int t = lazy ? decide_type_lazy(op, rules, tA, tB, cA, cB, lA, lB, unkA, card, nruns, unknown)
-                 : decide_type(op, tA, tB, cA, cB, lA, lB, card, nruns);
+                 : decide_type_keep_run(keep_run_cell<OP, LAZY>(rules, tA), op, tA, tB, cA, cB, lA, lB, card, nruns);
     if (OP == OP_OR && inplace_rules && !lazy) {
         // roaring_bitmap_or_inplace: a full left container is left untouched (roaring.c:1081-1083)
         // and container_ior turns a saturated bitset|bitset into the full run (containers.h:1234-1242)

@@ -52,7 +52,11 @@ constexpr uint32_t CARD_UNKNOWN = 0x80000000u, CARD_MASK = 0x7fffffffu;
 //   RULES_FLIP             (with RULES_LAZY's kernel instantiation, op XOR) roaring_bitmap_flip: the
 //                          right operand is the range as run containers, types follow the
 //                          negation cells (mixed_negation.c), see decide_type_lazy
-constexpr int RULES_INPLACE = 1, RULES_LAZY = 2, RULES_CONV = 4, RULES_NOFULL = 8, RULES_FLIP = 16;
+//   RULES_KEEP_RUN         (op OR or ANDNOT, not lazy) roaring_bitmap_add_many / remove_many: the right
+//                          operand is the values' bitmap, a run on the left stays a run, see
+//                          decide_type_keep_run
+constexpr int RULES_INPLACE = 1, RULES_LAZY = 2, RULES_CONV = 4, RULES_NOFULL = 8, RULES_FLIP = 16,
+              RULES_KEEP_RUN = 32;
 
 // Device view of a resident set: SoA container directory + payload.
 // Payload of container c starts at payload + c_off[c] (16-byte aligned, padded to 16 B).  `payload`

@@ -171,6 +171,19 @@ __host__ __device__ inline int decide_type(int op, int tA, int tB, uint32_t cA, 
     }
 }
 
+// Result type of a matched cell of roaring_bitmap_add_many / remove_many (RULES_KEEP_RUN): the left
+// container S with the bitmap V that roaring_bitmap_of_ptr builds from the values, OP_OR to add and
+// OP_ANDNOT to remove.  The reference adds (removes) one value at a time with container_add
+// (container_remove, containers.h:489, 530).  A run stays a run whatever it receives or loses
+// (run_container_add, run.c:39; run_container_remove, run.h:223).  Every other cell is the OR's (an
+// array becomes a bitset past 4096 values, a bitset stays a bitset) or the ANDNOT's (an array stays
+// an array, a bitset of a non-lazy set becomes an array at 4096 values or fewer).  Empty results are
+// dropped by the callers.  keep: the rule is on (RULES_KEEP_RUN).
+__host__ __device__ inline int decide_type_keep_run(bool keep, int op, int tA, int tB, uint32_t cA, uint32_t cB,
+                                                    uint32_t lA, uint32_t lB, int card, int nruns) {
+    return keep && tA == T_RUN ? T_RUN : decide_type(op, tA, tB, cA, cB, lA, lB, card, nruns);
+}
+
 // Final type of one output key of roaring_bitmap_add_offset (src/roaring.c:2470-2505) with a shift
 // that is not a multiple of 65536.  The key holds one or two parts, each of its source container's
 // type (container_add_offset, containers.h:1536); tB = 0 when there is one part.  Two parts were
@@ -252,6 +265,14 @@ __host__ __device__ inline uint32_t slot_bound(int op, int tA, int tB, uint32_t 
     const uint32_t g = cmax > (uint32_t)MAX_ARRAY ? FULLB : 2 * cmax;
     if (g < b) b = g;
     return round16(b);
+}
+
+// Slot bound of a matched cell with a run on the left under RULES_KEEP_RUN: the run stays a run, and
+// each value added adds at most one run, each value removed splits at most one; 32768 runs is the
+// most a container holds (every other value).  Up to 128 KiB, past the 8 KiB of slot_bound.
+__host__ __device__ __forceinline__ uint32_t slot_bound_keep_run(uint32_t lA, uint32_t cB) {
+    const uint32_t r = lA + cB;
+    return round16(4u * (r < 32768u ? r : 32768u));
 }
 
 // Slot bound of a matched cell under the lazy rules: unions / symmetric differences left as RUN
@@ -1071,7 +1092,8 @@ static __device__ __noinline__ uint32_t merge_arrays(uint32_t *acc, const uint8_
 // boundaries of each list were passed, and emits a boundary of the result wherever op(inA, inB)
 // flips (run_container_union / _intersection / _xor / _andnot, src/containers/run.c:231-633,
 // as one parallel sweep).  Returns false when the reference's type rule wants a bitset
-// (card > 4096), in which case the caller takes the general path.
+// (card > 4096), in which case the caller takes the general path.  keep_run: RULES_KEEP_RUN's type
+// rule (decide_type_keep_run).
 __device__ __forceinline__ bool op_state(int op, bool a, bool b) {
     return op == OP_AND ? (a && b) : op == OP_OR ? (a || b) : op == OP_XOR ? (a != b) : (a && !b);
 }
@@ -1117,7 +1139,7 @@ __device__ __forceinline__ uint32_t load_boundaries(uint32_t *pts, int type, con
 static __device__ __noinline__ bool
 interval_cell(uint32_t *acc, int op, int tA, int tB, const uint8_t *pa, const uint8_t *pb,
               uint32_t cA, uint32_t cB, uint32_t lA, uint32_t lB, uint8_t *out, uint32_t cap,
-              int lane, int &otype, uint32_t &ocard, uint32_t &olen) {
+              int lane, int &otype, uint32_t &ocard, uint32_t &olen, bool keep_run) {
     uint32_t *pA = acc;
     const uint32_t nA = load_boundaries(pA, tA, pa, lA, lane);
     uint32_t *pB = acc + 2 * nA;
@@ -1172,7 +1194,7 @@ interval_cell(uint32_t *acc, int op, int tA, int tB, const uint8_t *pa, const ui
     for (uint32_t k = lane; k < nruns; k += 32) card += ev[2 * k + 1] - ev[2 * k];
     card = __reduce_add_sync(FULLMASK, card);
     if (card == 0) { otype = 0; ocard = olen = 0; __syncwarp(); return true; }
-    const int t = decide_type(op, tA, tB, cA, cB, lA, lB, (int)card, (int)nruns);
+    const int t = decide_type_keep_run(keep_run, op, tA, tB, cA, cB, lA, lB, (int)card, (int)nruns);
     if (t == T_BITSET) { __syncwarp(); return false; }
     if (t == T_RUN) {
         if (4 * nruns > cap) { __syncwarp(); return false; }

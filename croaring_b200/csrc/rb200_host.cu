@@ -1277,9 +1277,11 @@ struct PairBuf {
     // shared, bit 1: B's), and the bound when everything is copied
     uint64_t slab_bound = 0, slab_bound_copy = 0;
     // op: OP_* of the batch (OP_AND also for the cardinality-only sweeps, which need no slab)
-    // flip: B is the range bitmap of rb200_batch_flip (every container ONE run)
+    // rules: RULES_* of the batch; with RULES_FLIP, B is the range bitmap of rb200_batch_flip (every
+    // container ONE run)
     bool build(const rb200_set *A, const rb200_set *B, const uint32_t *ia, const uint32_t *ib,
-               size_t np, int op, bool lazy = false, bool flip = false, int share = 0) {
+               size_t np, int op, int rules = 0, int share = 0) {
+        const bool lazy = (rules & RULES_LAZY) != 0, flip = (rules & RULES_FLIP) != 0;
         if (!ensure_mirrors(A) || !ensure_mirrors(B)) return false;
         if (np > 0xffffffffull) { t_err = "too many pairs in one batch (2^32 - 1 at most)"; return false; }
         const size_t o_off = 0, o_ia = al256(8 * (np + 1)), o_ib = o_ia + al256(4 * np);
@@ -1318,6 +1320,18 @@ struct PairBuf {
                 sb += 3 * (EA + EB) + m * (uint64_t)BITSET_BYTES + 512;
             } else if (op == OP_AND) {
                 sb += (EA < EB ? EA : EB) + 64;
+            } else if (rules & RULES_KEEP_RUN) {
+                // add_many / remove_many: a cell with a run on the left takes slot_bound_keep_run,
+                // min(128 KiB, 4 (lA + cB)) <= A's container's bytes + min(128 KiB, 4 cB), and the last
+                // term is at most 16 x the effective bytes of B's container (2 cB up to 4096 values,
+                // 8 KiB above).  Every other slot is bounded as for the op itself.
+                const uint64_t E = EA + 16 * EB;
+                sb += E + 64;
+                if (share) {
+                    const uint64_t own = (share & 1 ? 0 : EA) + (share & 2 || op == OP_ANDNOT ? 0 : EB) +
+                                         (uint64_t)(na < nb ? na : nb) * 131072;
+                    sbs += (own < E ? own : E) + 64;
+                }
             } else {
                 const uint64_t E = op == OP_ANDNOT ? EA : EA + EB;
                 sb += E + 64;
@@ -1358,6 +1372,20 @@ bool reject_lazy(const rb200_set *s, const char *what) {
     return true;
 }
 
+// idx[0..n) of a selection of a set of `count` bitmaps: n < 2^32 (checked before idx is read) and
+// every entry in range; `what` heads t_err.
+bool check_indices(const char *what, const uint32_t *idx, size_t n, uint64_t count) {
+    if (n > 0xffffffffull) { t_err = std::string(what) + ": more than 2^32 - 1 bitmaps selected"; return false; }
+    for (size_t k = 0; k < n; k++) {
+        if (idx[k] >= count) {
+            t_err = std::string(what) + ": index out of range: idx[" + std::to_string(k) + "] = " +
+                    std::to_string(idx[k]) + ", the set holds " + std::to_string(count) + " bitmaps";
+            return false;
+        }
+    }
+    return true;
+}
+
 // The bitmaps S[idx[0..n)] an entry point works on; idx == NULL selects every bitmap of S in order.
 struct Selection {
     const rb200_set *S;
@@ -1369,15 +1397,7 @@ struct Selection {
         if (!S) { t_err = std::string(what) + ": S is NULL"; return false; }
         if (reject_lazy(S, what)) return false;
         if (!idx) { n = S->n_bitmaps; return true; }
-        if (n > 0xffffffffull) { t_err = std::string(what) + ": more than 2^32 - 1 bitmaps selected"; return false; }
-        for (size_t k = 0; k < n; k++) {
-            if (idx[k] >= S->n_bitmaps) {
-                t_err = std::string(what) + ": index out of range: idx[" + std::to_string(k) + "] = " +
-                        std::to_string(idx[k]) + ", the set holds " + std::to_string(S->n_bitmaps) + " bitmaps";
-                return false;
-            }
-        }
-        return true;
+        return check_indices(what, idx, n, S->n_bitmaps);
     }
     uint32_t operator[](size_t k) const { return idx ? idx[k] : (uint32_t)k; }
     bool all() const { return idx == nullptr; }
@@ -1448,7 +1468,11 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         if (op == OP_XOR && (rules & (RULES_CONV | RULES_NOFULL))) { t_err = "bad lazy flags for XOR"; return nullptr; }
         if ((rules & RULES_FLIP) && op != OP_XOR) { t_err = "bad flags"; return nullptr; }
     } else {
-        if (rules & ~RULES_INPLACE) { t_err = "bad flags"; return nullptr; }
+        if (rules & ~(RULES_INPLACE | RULES_KEEP_RUN)) { t_err = "bad flags"; return nullptr; }
+        if ((rules & RULES_KEEP_RUN) && ((op != OP_OR && op != OP_ANDNOT) || (rules & RULES_INPLACE))) {
+            t_err = "bad flags";
+            return nullptr;
+        }
         if (reject_lazy(A, "batch op") || reject_lazy(B, "batch op")) return nullptr;
     }
     if (np > 0xffffffffull) { t_err = "too many pairs"; return nullptr; }
@@ -1463,8 +1487,7 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     if (!ensure_mirrors(A) || !ensure_mirrors(B)) return nullptr;
     const bool can_share = !(rules & RULES_LAZY) && op != OP_AND && np > 0;
     const bool onA = can_share && !A->sharing(), onB = can_share && op != OP_ANDNOT && !B->sharing();
-    bool ok = pb.build(A, B, ia, ib, np, op, (rules & RULES_LAZY) != 0, (rules & RULES_FLIP) != 0,
-                       (onA ? 1 : 0) | (onB ? 2 : 0));
+    bool ok = pb.build(A, B, ia, ib, np, op, rules, (onA ? 1 : 0) | (onB ? 2 : 0));
     // class-ordered tickets pay one more small kernel: only for batches that fill the GPU
     static const uint64_t order_min = []() { const char *e = getenv("RB200_ORDER_MIN"); return e ? (uint64_t)atoll(e) : 16384ull; }();
     // (tried in round 2: ONE launch with a CTA per pair doing plan -> cells -> finalize for small batches —
@@ -3278,6 +3301,62 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     if (!Rg) return nullptr;
     return batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), sel.n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
 }
+// ---- updates: roaring_bitmap_add_many / remove_many (src/roaring.c:134, 696) ----------------------
+// result[k] = S[idx[k]] after adding (removing) the values vals[off[k] .. off[k+1]).  The values become
+// a bitmap V[k] with roaring_bitmap_of_ptr's builder (from_uint32_impl), and the update is the batch op
+// (S[idx[k]], V[k]) under RULES_KEEP_RUN: OR to add, ANDNOT to remove (decide_type_keep_run).  The
+// containers the values do not touch stay shared with S.  An added key that S lacks takes V's
+// container, which the result holds like any operand's (rb200_set::held), so V is freed on return.
+namespace {
+rb200_set *update_op(int op, const Selection &sel, const rb200_set *V) {
+    if (!V) return nullptr;
+    std::vector<uint32_t> ia(sel.n), ib(sel.n);
+    for (size_t k = 0; k < sel.n; k++) {
+        ia[k] = sel[k];
+        ib[k] = (uint32_t)k;
+    }
+    return batch_op_impl(op, sel.S, V, ia.data(), ib.data(), sel.n, RULES_KEEP_RUN);
+}
+rb200_set *update_host(int op, const char *what, const rb200_set *S, const uint32_t *idx, size_t n,
+                       const uint32_t *vals, const uint64_t *off) {
+    Selection sel{S, idx, n};
+    if (!sel.check(what) || !check_value_offsets(off, sel.n, what)) return nullptr;   // before any CUDA call
+    if (!vals && off[sel.n]) { t_err = std::string(what) + ": values are NULL"; return nullptr; }
+    if (!ctx_init()) return nullptr;
+    static const uint32_t none = 0;
+    const SetPtr V(from_uint32_impl(vals ? vals : &none, nullptr, off, sel.n));
+    return update_op(op, sel, V.get());
+}
+rb200_set *update_device(int op, const char *what, const rb200_set *S, const uint32_t *idx, size_t n,
+                         const uint32_t *d_vals, const uint64_t *d_off) {
+    Selection sel{S, idx, n};
+    PinBlock<uint64_t> h_off;
+    if (!sel.check(what) || !device_offsets(d_off, d_vals, sel.n, what, what, h_off)) return nullptr;
+    const SetPtr V(from_uint32_impl(nullptr, d_vals, h_off.get(), sel.n));
+    return update_op(op, sel, V.get());
+}
+}  // namespace
+rb200_set_t *rb200_batch_add_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                  const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update_host(OP_OR, "add_many", S, idx, n, vals, off);
+}
+rb200_set_t *rb200_batch_remove_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                     const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update_host(OP_ANDNOT, "remove_many", S, idx, n, vals, off);
+}
+rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *d_vals,
+                                         const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update_device(OP_OR, "add_many_device", S, idx, n, d_vals, d_off);
+}
+rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
+                                            const uint32_t *d_vals, const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update_device(OP_ANDNOT, "remove_many_device", S, idx, n, d_vals, d_off);
+}
+
 roaring_bitmap_t *roaring_bitmap_flip(const roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     const SetPtr S = upload_bound({r1});
@@ -3447,7 +3526,7 @@ bool plan64(int op, const rb200_set64 *A, const rb200_set64 *B, const uint32_t *
 }
 
 rb200_set64 *batch_op64_impl(int op, const rb200_set64 *A, const rb200_set64 *B, const uint32_t *ia,
-                             const uint32_t *ib, size_t np) {
+                             const uint32_t *ib, size_t np, int rules = 0) {
     if (!ctx_init()) return nullptr;
     if (op < 0 || op > 3) { t_err = "bad op"; return nullptr; }
     if (np > 0xffffffffull) { t_err = "too many pairs"; return nullptr; }
@@ -3464,7 +3543,7 @@ rb200_set64 *batch_op64_impl(int op, const rb200_set64 *A, const rb200_set64 *B,
         dir[np + p] = P.cnt[p];
     }
     memcpy(dir + 2 * np, P.high.data(), 4 * P.high.size());
-    R->inner.reset(batch_op_impl(op, A->inner.get(), B->inner.get(), P.pa.data(), P.pb.data(), P.pa.size()));
+    R->inner.reset(batch_op_impl(op, A->inner.get(), B->inner.get(), P.pa.data(), P.pb.data(), P.pa.size(), rules));
     return R->inner ? R.release() : nullptr;
 }
 
@@ -3585,6 +3664,37 @@ rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, cons
     return R.release();
 }
 
+// roaring64_bitmap_add_many / remove_many (roaring64.c:606, 950) of S[idx[k]] with the values
+// vals[off[k] .. off[k+1]): the same container_add / container_remove per 48-bit key as the 32-bit
+// update, so the inner sets take the same batch op under RULES_KEEP_RUN (update_op).  plan64 keeps the
+// buckets only V holds for OR and drops them for ANDNOT; a bucket a removal empties stays an empty
+// inner bitmap, which is never planned, counted or serialized.  device: vals / off are in device memory.
+rb200_set64 *update64(int op, const char *what, const rb200_set64 *S, const uint32_t *idx, size_t n,
+                      const uint64_t *vals, const uint64_t *off, bool device) {
+    if (!S) { t_err = std::string(what) + ": S is NULL"; return nullptr; }
+    if (!idx) n = S->n;
+    else if (!check_indices(what, idx, n, S->n)) return nullptr;
+    PinBlock<uint64_t> d_h_off;
+    const uint64_t *h_off = off;
+    if (!device) {
+        if (!check_value_offsets(off, n, what)) return nullptr;   // before any CUDA call
+        if (!vals && off[n]) { t_err = std::string(what) + ": values are NULL"; return nullptr; }
+        if (!ctx_init()) return nullptr;
+    } else {
+        if (!device_offsets(off, vals, n, what, what, d_h_off)) return nullptr;
+        h_off = d_h_off.get();
+    }
+    static const uint64_t none = 0;
+    const Set64Ptr V(device ? from_uint64_impl(nullptr, vals, h_off, n) : from_uint64_impl(vals ? vals : &none, nullptr, h_off, n));
+    if (!V) return nullptr;
+    std::vector<uint32_t> ia(n), ib(n);
+    for (size_t k = 0; k < n; k++) {
+        ia[k] = idx ? idx[k] : (uint32_t)k;
+        ib[k] = (uint32_t)k;
+    }
+    return batch_op64_impl(op, S, V.get(), ia.data(), ib.data(), n, RULES_KEEP_RUN);
+}
+
 // a[] then b[] as ONE resident set (one H2D); ib2 = ib shifted past a[]
 rb200_set64 *r64_operands(const char *const *a, const size_t *alen, size_t na, const char *const *b,
                           const size_t *blen, size_t nb, const uint32_t *ia, const uint32_t *ib, size_t np,
@@ -3647,6 +3757,26 @@ int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_
                                       const uint32_t *ib, size_t npairs, uint64_t *out) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return and_cardinality64_impl(A, B, ia, ib, npairs, out);
+}
+rb200_set64_t *rb200_set64_batch_add_many(const rb200_set64_t *S, const uint32_t *idx, size_t n, const uint64_t *vals,
+                                          const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update64(OP_OR, "set64_add_many", S, idx, n, vals, off, false);
+}
+rb200_set64_t *rb200_set64_batch_remove_many(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                             const uint64_t *vals, const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update64(OP_ANDNOT, "set64_remove_many", S, idx, n, vals, off, false);
+}
+rb200_set64_t *rb200_set64_batch_add_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                 const uint64_t *d_vals, const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update64(OP_OR, "set64_add_many_device", S, idx, n, d_vals, d_off, true);
+}
+rb200_set64_t *rb200_set64_batch_remove_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                    const uint64_t *d_vals, const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update64(OP_ANDNOT, "set64_remove_many_device", S, idx, n, d_vals, d_off, true);
 }
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);

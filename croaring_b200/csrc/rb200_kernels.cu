@@ -89,7 +89,8 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
                             d.shared = (rules & (RULES_INPLACE | RULES_LAZY)) == RULES_INPLACE && A.c_src[ca] == SRC_SHARED;
                             const uint32_t cA = d.cA & CARD_MASK;
                             cap = (rules & RULES_LAZY) ? slot_bound_lazy(d.tA, d.tB, cA, d.cB, d.lA, d.lB)
-                                                       : slot_bound(op, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
+                                  : (rules & RULES_KEEP_RUN) && d.tA == T_RUN ? slot_bound_keep_run(d.lA, d.cB)
+                                                                              : slot_bound(op, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
                             cls = cell_class(op, rules, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
                         }
                     } else if (op != OP_AND && !card_only) {

@@ -202,7 +202,7 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
 int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint32_t *ia,
                           const uint32_t *ib, size_t npairs, uint8_t *out);
 
-/* Selections.  rb200_batch_flip, rb200_batch_add_offset and the or_many / xor_many entry points work on
+/* Selections.  rb200_batch_flip, rb200_batch_add_offset, the add_many / remove_many family and the or_many / xor_many entry points work on
  * S[idx[0..n)]; idx == NULL selects every bitmap of S in order (n is then ignored).  A NULL or lazy S, and
  * with an idx, n >= 2^32 or an entry out of range, is refused before any device work; rb200_last_error()
  * names the entry point. */
@@ -216,6 +216,22 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
  * dropped.  Key-aligned shifts (offset % 65536 == 0) share the operand's containers instead of copying them.
  * Returns a new resident set, NULL on error (rb200_last_error). */
 rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, size_t n, const int64_t *offsets);
+
+/* result[k] = S[idx[k]] after roaring_bitmap_add_many / _remove_many of vals[off[k] .. off[k+1]) (any order,
+ * duplicates allowed); idx == NULL: every bitmap, off then has rb200_set_count(S) + 1 entries.  Results match
+ * the reference's bytes: a run container stays a run, whatever it gains or loses; containers the values do
+ * not touch are shared with S, not copied.  Offsets: off[0] == 0, non-decreasing, checked on the host
+ * with the selection before any device work; NULL vals need off[n] == 0.  _device: vals / off in device
+ * memory of the library's device, read on the library stream and not modified.  Returns a new resident
+ * set, NULL on error (rb200_last_error). */
+rb200_set_t *rb200_batch_add_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                  const uint64_t *off);
+rb200_set_t *rb200_batch_remove_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                     const uint64_t *off);
+rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *d_vals,
+                                         const uint64_t *d_off);
+rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
+                                            const uint32_t *d_vals, const uint64_t *d_off);
 
 /* 64-bit bitmaps (src/roaring64.c) through their portable format: result[k] =
  * roaring64_bitmap_{and,or,xor,andnot}(a[ia[k]], b[ib[k]]) — the same container grid per
@@ -289,6 +305,17 @@ rb200_set64_t *rb200_set64_batch_op(int op, const rb200_set64_t *A, const rb200_
 /* out[k] = roaring64_bitmap_and_cardinality(A[ia[k]], B[ib[k]]); 0 on success. */
 int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_t *B, const uint32_t *ia,
                                       const uint32_t *ib, size_t npairs, uint64_t *out);
+/* result[k] = S[idx[k]] after roaring64_bitmap_add_many / _remove_many of vals[off[k] .. off[k+1]), with the
+ * selection, offsets and values of rb200_batch_add_many (idx == NULL: off has rb200_set64_count(S) + 1
+ * entries).  Buckets a removal empties are left out of the result. */
+rb200_set64_t *rb200_set64_batch_add_many(const rb200_set64_t *S, const uint32_t *idx, size_t n, const uint64_t *vals,
+                                          const uint64_t *off);
+rb200_set64_t *rb200_set64_batch_remove_many(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                             const uint64_t *vals, const uint64_t *off);
+rb200_set64_t *rb200_set64_batch_add_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                 const uint64_t *d_vals, const uint64_t *d_off);
+rb200_set64_t *rb200_set64_batch_remove_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                    const uint64_t *d_vals, const uint64_t *d_off);
 /* mode 1 = roaring64_bitmap_run_optimize, mode 0 = remove the run containers (as rb200_set_run_optimize). */
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *s, int mode);
 /* Device-side roaring64_bitmap_portable_serialize of every bitmap + one D2H: blob i = *buf + (*off)[i],
