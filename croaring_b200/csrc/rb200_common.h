@@ -403,8 +403,11 @@ void launch_offset_plan(const SetView &S, const uint32_t *idx, const int64_t *of
 void launch_offset_cells(const SetView &S, Items it, const uint4 *cell, uint64_t W, uint64_t bias, uint8_t *slab,
                          OpStats *st, cudaStream_t s);
 
+// cow: one byte per selected position, non-zero where that input is copy-on-write (null: none is);
+// live: null, or n int32 zeroed, to which every key adds +1 at the position where its accumulator
+// becomes non-empty and -1 where it becomes empty (the host replays the result's COW flag from them)
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
-                     uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
-                     cudaStream_t s);
+                     const uint8_t *cow, int32_t *live, uint8_t *t_type, uint32_t *t_card, uint32_t *t_len,
+                     SetOut out, OpStats *st, cudaStream_t s);
 
 }  // namespace rb200

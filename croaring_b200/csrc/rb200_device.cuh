@@ -184,6 +184,22 @@ __host__ __device__ inline int decide_type_keep_run(bool keep, int op, int tA, i
     return keep && tA == T_RUN ? T_RUN : decide_type(op, tA, tB, cA, cB, lA, lB, card, nruns);
 }
 
+// Type of roaring_bitmap_xor_many's accumulator for one key after it takes one more input (k_xor_many):
+// the accumulator (tA, cA, lA) xor the input (tB, cB, lB), whose result holds card values in nruns
+// runs.  lazy: the step is container_lazy_xor (containers.h:1570-1654): the first step, x[0] ^ x[1]
+// (roaring.c:2684-2761), and every step on a SHARED accumulator, which roaring_bitmap_lazy_xor_inplace
+// does not compute in place (:2794-2797).  Otherwise it is container_lazy_ixor (:1749-1776): lazy for
+// bitset x bitset, the eager container_ixor rules for everything else.
+__host__ __device__ inline int xor_many_step_type(bool lazy, int tA, int tB, uint32_t cA, uint32_t cB,
+                                                  uint32_t lA, uint32_t lB, int card, int nruns) {
+    if (tA == T_BITSET && tB == T_BITSET) return T_BITSET;   // lazy in both (containers.h:1579-1585, 1757-1761)
+    if (!lazy) return decide_type(OP_XOR, tA, tB, cA, cB, lA, lB, card, nruns);
+    if (tA == T_ARRAY && tB == T_ARRAY) return cA + cB <= 1024u ? T_ARRAY : T_BITSET;   // mixed_xor.c:221-252
+    if (tA == T_RUN && tB == T_RUN) return rule_eff(card, nruns);
+    if (tA == T_BITSET || tB == T_BITSET) return T_BITSET;
+    return T_RUN;   // array x run is left a run (mixed_xor.c:145-174)
+}
+
 // Final type of one output key of roaring_bitmap_add_offset (src/roaring.c:2470-2505) with a shift
 // that is not a multiple of 65536.  The key holds one or two parts, each of its source container's
 // type (container_add_offset, containers.h:1536); tB = 0 when there is one part.  Two parts were

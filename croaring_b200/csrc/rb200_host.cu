@@ -1401,16 +1401,30 @@ struct Selection {
     }
     uint32_t operator[](size_t k) const { return idx ? idx[k] : (uint32_t)k; }
     bool all() const { return idx == nullptr; }
-    // containers of the selected bitmaps and the OR of their COW flags (S's mirrors must be current)
+    // containers of the selected bitmaps (S's mirrors must be current)
     uint64_t containers() const {
         uint64_t t = 0;
         for (size_t k = 0; k < n; k++) t += S->h_cnt[(*this)[k]];
         return t;
     }
-    uint8_t cow() const {
-        uint8_t f = 0;
-        for (size_t k = 0; k < n; k++) f |= S->h_flags[(*this)[k]];
-        return f & FLAG_COW;
+    uint8_t cow(size_t k) const { return S->h_flags[(*this)[k]] & FLAG_COW; }
+    // whether the selected flags differ, which is when a fold's flag depends on its order
+    bool cow_mixed() const {
+        for (size_t k = 1; k < n; k++) if (cow(k) != cow(0)) return true;
+        return false;
+    }
+    // The COW flag of the lazy fold roaring_bitmap_or_many / xor_many (roaring.c:775-809) of the
+    // selection.  lazy_<op>(x0, x1) returns a copy of a non-empty operand next to an empty one and
+    // takes both flags otherwise (:2509-2523, 2684-2697); a later step keeps the flag, unless it
+    // overwrites an empty accumulator with a non-empty input (:2609-2610, 2772-2773).
+    // acc_empty(k): the fold of inputs [0, k) is empty, for k >= 2.
+    template <typename F> uint8_t fold_cow(F acc_empty) const {
+        if (n < 2) return n ? cow(0) : 0;
+        const auto empty = [&](size_t k) { return S->h_cnt[(*this)[k]] == 0; };
+        uint8_t f = empty(0) ? cow(1) : empty(1) ? cow(0) : cow(0) | cow(1);
+        for (size_t k = 2; k < n; k++)
+            if (!empty(k) && acc_empty(k)) f = cow(k);
+        return f;
     }
     // idx on the device through the pinned block h, which must outlive the copy; d stays NULL for
     // all(), which the kernels read as the identity
@@ -1422,14 +1436,34 @@ struct Selection {
     }
 };
 
-// Host fields of a one-bitmap result of `containers` bitset slots (or_many, xor_many): the COW flag
-// is propagated from the inputs (roaring_bitmap_lazy_or, roaring.c:2523).
-void fill_single_result(rb200_set *R, uint32_t containers, uint64_t slab_used, const Selection &sel) {
+// Host fields of a one-bitmap result of `containers` bitset slots (or_many, xor_many).
+void fill_single_result(rb200_set *R, uint32_t containers, uint64_t slab_used, uint8_t cow) {
     R->n_containers = containers;
     R->slab_used = slab_used;
     R->h_cnt[0] = containers;
     R->h_bytes[0] = R->h_ebytes[0] = (uint64_t)containers * BITSET_BYTES;
-    R->h_flags[0] = sel.cow();
+    R->h_flags[0] = cow;
+}
+
+// The COW flag the reference gives x1 op x2 under `rules`, from the operands' flags and whether they
+// are empty (hold no container).
+// - A union or xor with an empty operand is a copy of the other (roaring.c:882-886, 1126-1130,
+//   2515-2519, 2689-2693), and so is an andnot with an empty x2 (:1286).  Other results take both
+//   flags (:738, 890, 1283, 1290).
+// - The in-place twins keep x1's flag, unless a union or xor overwrites an empty x1 with a non-empty
+//   x2 (roaring_bitmap_overwrite, :1072, 1210, 2610, 2773).  So do flips (:2307) and the updates of
+//   add_many / remove_many, which modify x1.
+// - lazy_or_from_lazy_inputs (RULES_NOFULL, roaring_priority_queue.c:99-111) returns its non-empty
+//   operand next to an empty one, and otherwise a new bitmap without the flag.
+uint8_t result_cow(int op, int rules, uint8_t fa, uint8_t fb, bool emptyA, bool emptyB) {
+    fa &= FLAG_COW;
+    fb &= FLAG_COW;
+    const bool unite = op == OP_OR || op == OP_XOR;
+    if (rules & (RULES_FLIP | RULES_KEEP_RUN)) return fa;
+    if (rules & RULES_NOFULL) return emptyA ? fb : emptyB ? fa : 0;
+    if (rules & RULES_INPLACE) return unite && emptyA && !emptyB ? fb : fa;
+    if (unite) return emptyA ? fb : emptyB ? fa : fa | fb;
+    return op == OP_ANDNOT && emptyB && !emptyA ? fa : fa | fb;
 }
 
 // Let R point into A's payload (onA) and / or B's (onB): R holds their slabs and its payload base
@@ -1525,7 +1559,9 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         R->parentA = A->h_ptr;
         R->parentB = B->h_ptr;
         R->lazy = (rules & RULES_LAZY) != 0 && !(rules & RULES_FLIP);
-        for (size_t p = 0; p < np; p++) R->h_flags[p] = (A->h_flags[ia[p]] | B->h_flags[ib[p]]) & FLAG_COW;
+        for (size_t p = 0; p < np; p++)
+            R->h_flags[p] = result_cow(op, rules, A->h_flags[ia[p]], B->h_flags[ib[p]], A->h_cnt[ia[p]] == 0,
+                                       B->h_cnt[ib[p]] == 0);
     }
     // the device buffers go back when pb / ib_ leave scope: stream-ordered reuse
     return call.finish(ok);
@@ -1678,7 +1714,9 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
     if (ok) {
         const uint32_t *h_ck = ck.get();
         const uint32_t nk = g.h_stats->nk;
-        fill_single_result(R.get(), nk, (uint64_t)nk * BITSET_BYTES, sel);
+        size_t first = 0;   // the first non-empty input: a union is empty until it
+        while (first < n && S->h_cnt[sel[first]] == 0) first++;
+        fill_single_result(R.get(), nk, (uint64_t)nk * BITSET_BYTES, sel.fold_cow([&](size_t k) { return k <= first; }));
         if (card_per_key)
             for (int k = 0; k < 65536; k++) card_per_key[k] += h_ck[k];
         if (sh) {
@@ -1756,20 +1794,44 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
     DevBlock<uint32_t> t_card(maxk), t_len(maxk);
     SyncCall call("xor_many", "xor_many launch", true);
     bool ok = t_type && t_card && t_len && sel.to_device(d_idx, h_idx);
+    // Copy-on-write inputs only: their COW bits per position (the kernel's SHARED accumulators), and
+    // when the flags are mixed, where each key's accumulator turns live or empty (the result's flag).
+    bool any_cow = false;
+    for (size_t k = 0; k < sel.n && !any_cow; k++) any_cow = sel.cow(k) != 0;
+    const bool mixed = sel.cow_mixed();
+    DevBlock<uint8_t> d_cow;
+    PinBlock<uint8_t> h_cow;
+    DevBlock<int32_t> d_live;
+    PinBlock<int32_t> h_live;
+    if (ok && any_cow) {
+        ok = d_cow.reset(sel.n) && h_cow.reset(sel.n);
+        for (size_t k = 0; ok && k < sel.n; k++) h_cow.get()[k] = sel.cow(k);
+        ok = ok && cudaMemcpyAsync(d_cow.get(), h_cow.get(), sel.n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    }
+    if (ok && mixed)
+        ok = d_live.reset(sel.n) && h_live.reset(sel.n) &&
+             cudaMemsetAsync(d_live.get(), 0, 4 * sel.n, g.stream) == cudaSuccess;
     if (ok) {
         ok = call.begin();
         const SetView vs = S->view();
         launch_many_mark(vs, d_idx.get(), (uint32_t)sel.n, 0, 65535, g.d_flags, g.stream);
         launch_many_compact(g.d_flags, g.d_keys, g.d_stats, g.stream);
         call.kernels_begin();
-        launch_xor_many(vs, d_idx.get(), (uint32_t)sel.n, g.d_keys, t_type.get(), t_card.get(), t_len.get(), R->out(),
-                        g.d_stats, g.stream);
+        launch_xor_many(vs, d_idx.get(), (uint32_t)sel.n, g.d_keys, d_cow.get(), d_live.get(), t_type.get(), t_card.get(),
+                        t_len.get(), R->out(), g.d_stats, g.stream);
         call.kernels_end();
         call.end();
+        if (mixed)
+            ok = ok && cudaMemcpyAsync(h_live.get(), d_live.get(), 4 * sel.n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
         ok = call.finish(ok);
     }
     if (ok) {
-        fill_single_result(R.get(), (uint32_t)g.h_stats->dir_cursor, (uint64_t)g.h_stats->nk * BITSET_BYTES, sel);
+        // live keys after input k: the prefix sums of the kernel's +1 / -1 per position
+        std::vector<int64_t> live_after(mixed ? sel.n : 0);
+        int64_t live = 0;
+        for (size_t k = 0; k < live_after.size(); k++) live_after[k] = live += h_live.get()[k];
+        const uint8_t cow = mixed ? sel.fold_cow([&](size_t k) { return live_after[k - 1] == 0; }) : sel.n ? sel.cow(0) : 0;
+        fill_single_result(R.get(), (uint32_t)g.h_stats->dir_cursor, (uint64_t)g.h_stats->nk * BITSET_BYTES, cow);
         g.last_algo_bytes = sel.all() ? S->portable_bytes : 0;
     }
     return ok ? R.release() : nullptr;
@@ -3025,7 +3087,7 @@ static int pair_fused(int op, const roaring_bitmap_t *r1, const roaring_bitmap_t
     roaring_bitmap_t *r = bitmap_alloc((int32_t)no);
     if (!r) { t_err = "out of host memory"; return -1; }
     roaring_array_t *rr = &r->high_low_container;
-    rr->flags = (ra[0]->flags | ra[1]->flags) & FLAG_COW;   // roaring.c:738, 890
+    rr->flags = result_cow(op, rules, ra[0]->flags, ra[1]->flags, ra[0]->size == 0, ra[1]->size == 0);
     const uint8_t *ob = g.h_fused_out;
     const uint16_t *o_key = (const uint16_t *)(ob + FUSED_OUT_KEY);
     const uint8_t *o_type = ob + FUSED_OUT_TYPE;
@@ -3077,8 +3139,9 @@ roaring_bitmap_t *roaring_bitmap_or_many(size_t number, const roaring_bitmap_t *
 }
 
 // The end of an in-place call: the result `out` (consumed) replaces x1's directory and containers
-// (the old ones are released, x1's flags kept); without a result x1 is left untouched and the
-// failure of `fn` is reported.
+// (the old ones are released); x1 takes the result's COW flag, which follows the in-place rules of
+// result_cow, and keeps its other flags.  Without a result x1 is left untouched and the failure of
+// `fn` is reported.
 static void finish_inplace(roaring_bitmap_t *x1, roaring_bitmap_t *out, const char *fn) {
     if (!out) { dropin_failed(fn); return; }
     roaring_array_t *ra = &x1->high_low_container, *rn = &out->high_low_container;
@@ -3088,7 +3151,7 @@ static void finish_inplace(roaring_bitmap_t *x1, roaring_bitmap_t *out, const ch
         h_free(ra->containers);
     }
     *ra = *rn;
-    ra->flags = flags;
+    ra->flags = (flags & ~FLAG_COW) | (rn->flags & FLAG_COW);
     h_free(out);
 }
 // In-place twins (src/roaring.c:812 and_inplace, :1063 or_inplace, :1200 xor_inplace, :1342
@@ -3299,7 +3362,10 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     const size_t bl = blob.size();
     SetPtr Rg(upload_blobs_impl(&bp, &bl, 1, false));
     if (!Rg) return nullptr;
-    return batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), sel.n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
+    rb200_set *R = batch_op_impl(OP_XOR, S, Rg.get(), ia.data(), ib.data(), sel.n, noop ? 0 : (RULES_LAZY | RULES_FLIP));
+    // an empty range copies every bitmap with its flag (roaring.c:2293), an empty one included
+    if (R && noop) for (size_t p = 0; p < sel.n; p++) R->h_flags[p] = sel.cow(p);
+    return R;
 }
 // ---- updates: roaring_bitmap_add_many / remove_many (src/roaring.c:134, 696) ----------------------
 // result[k] = S[idx[k]] after adding (removing) the values vals[off[k] .. off[k+1]).  The values become
@@ -4101,7 +4167,9 @@ rb200_set_t *rb200_or_many_heap(const rb200_set_t *S, const uint32_t *idx, size_
         bitmap_free_host(e);
         if (!E) return nullptr;
         const uint32_t a = sel[0], z = 0;
-        return batch_op_impl(OP_OR, S, E.get(), &a, &z, 1, 0);
+        rb200_set *R = batch_op_impl(OP_OR, S, E.get(), &a, &z, 1, 0);
+        if (R) R->h_flags[0] = sel.cow(0);   // the copy's flag, an empty input's included
+        return R;
     }
     std::vector<uint32_t> sz;
     if (!portable_sizes(S, sz)) return nullptr;

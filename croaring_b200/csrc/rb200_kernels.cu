@@ -84,14 +84,16 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
                             d.lB = B.c_len[cb];
                             d.offA = A.c_off[ca];
                             d.offB = B.c_off[cb];
-                            // in-place twins: a SHARED left container takes the functional cell (roaring.c:1085-1088);
-                            // the lazy in-place twins work on a writable copy instead (roaring.c:2636)
-                            d.shared = (rules & (RULES_INPLACE | RULES_LAZY)) == RULES_INPLACE && A.c_src[ca] == SRC_SHARED;
+                            // in-place twins: a SHARED left container takes the functional cell (roaring.c:1085-1088),
+                            // and so does lazy_xor_inplace (container_lazy_xor, :2794-2797); lazy_or_inplace
+                            // works on a writable copy instead (:2624, 2636)
+                            d.shared = (rules & RULES_INPLACE) && (!(rules & RULES_LAZY) || op == OP_XOR) &&
+                                       A.c_src[ca] == SRC_SHARED;
                             const uint32_t cA = d.cA & CARD_MASK;
                             cap = (rules & RULES_LAZY) ? slot_bound_lazy(d.tA, d.tB, cA, d.cB, d.lA, d.lB)
                                   : (rules & RULES_KEEP_RUN) && d.tA == T_RUN ? slot_bound_keep_run(d.lA, d.cB)
                                                                               : slot_bound(op, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
-                            cls = cell_class(op, rules, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
+                            cls = cell_class(op, d.shared ? rules & ~RULES_INPLACE : rules, d.tA, d.tB, cA, d.cB, d.lA, d.lB);
                         }
                     } else if (op != OP_AND && !card_only) {
                         kind = K_COPY_A;

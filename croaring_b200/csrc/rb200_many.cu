@@ -96,12 +96,15 @@ __device__ __forceinline__ uint32_t many_gather(ManySmem &sm, const SetView &S,
 // becomes empty is removed and re-inserted as a clone by a later input.  So the fold is kept
 // sequential per key: a CTA owns the key, applies one participant at a time to the shared
 // 65536-bit accumulator (bitsets: word xor; arrays: atomicXor; runs: range flips), recounts
-// cardinality and run starts, and thread 0 advances the (type, cardinality, runs) state with
-// the same decide_type() rules as the pairwise XOR cells.
+// cardinality and run starts, and every thread advances the (type, cardinality, runs) state with
+// xor_many_step_type().  A container cloned from a copy-on-write input (cow[pos]) enters the
+// accumulator SHARED (get_copy_of_container, roaring.c:2727-2745, 2825-2834; roaring_bitmap_copy and
+// _overwrite alike), so the next step on that key is a lazy xor, not an in-place one.
 __global__ void __launch_bounds__(OM_THREADS, 2)
 k_xor_many(SetView S, const uint32_t *__restrict__ idx, uint32_t n,
-           const uint16_t *__restrict__ keys, uint8_t *__restrict__ t_type,
-           uint32_t *__restrict__ t_card, uint32_t *__restrict__ t_len, uint8_t *slab, OpStats *st) {
+           const uint16_t *__restrict__ keys, const uint8_t *__restrict__ cow, int32_t *live,
+           uint8_t *__restrict__ t_type, uint32_t *__restrict__ t_card, uint32_t *__restrict__ t_len,
+           uint8_t *slab, OpStats *st) {
     __shared__ __align__(16) ManySmem sm;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint32_t nk = st->nk;
@@ -113,8 +116,8 @@ k_xor_many(SetView S, const uint32_t *__restrict__ idx, uint32_t n,
         if (ki >= nk) break;
         const uint32_t key = keys[ki];
         for (int i = tid; i < ACC_WORDS; i += OM_THREADS) sm.acc[i] = 0;
-        // fold state (thread 0): accumulator present?, its type, cardinality, run count
-        bool have = false;
+        // fold state (every thread): accumulator present?, SHARED?, its type, cardinality, run count
+        bool have = false, shared = false;
         int t_acc = 0;
         uint32_t card_acc = 0, nruns_acc = 0, m_total = 0, first_pos = 0;
         int card = 0, nruns = 0;
@@ -176,31 +179,20 @@ k_xor_many(SetView S, const uint32_t *__restrict__ idx, uint32_t n,
                 const uint32_t c2 = sm.pcard[j], pos = sm.ppos[j];
                 if (!have) {
                     have = true;  // clone (roaring.c:2724-2745 / :2822-2834)
+                    shared = cow && cow[pos];
                     t_acc = t2;
+                    if (live && tid == 0) atomicAdd(live + pos, 1);
                 } else {
-                    const bool non_inplace = (m_total == 1) && first_pos == 0 && pos == 1;
-                    int t;
-                    if (t_acc == T_BITSET && t2 == T_BITSET) {
-                        t = T_BITSET;  // lazy in both variants (containers.h:1579-1585, 1757-1761)
-                    } else if (non_inplace) {
-                        // container_lazy_xor, containers.h:1570-1654
-                        if (t_acc == T_ARRAY && t2 == T_ARRAY)
-                            t = (card_acc + c2 <= 1024u) ? T_ARRAY : T_BITSET;  // mixed_xor.c:221-252
-                        else if (t_acc == T_RUN && t2 == T_RUN)
-                            t = rule_eff(card, nruns);
-                        else if (t_acc == T_BITSET || t2 == T_BITSET)
-                            t = T_BITSET;
-                        else
-                            t = T_RUN;  // array x run left as run (mixed_xor.c:145-174)
-                    } else {
-                        // container_lazy_ixor -> container_ixor: the eager cell rules
-                        t = decide_type(OP_XOR, t_acc, t2, card_acc, c2, nruns_acc, l2, card, nruns);
-                    }
-                    t_acc = t;
+                    const bool lazy = shared || ((m_total == 1) && first_pos == 0 && pos == 1);
+                    t_acc = xor_many_step_type(lazy, t_acc, t2, card_acc, c2, nruns_acc, l2, card, nruns);
+                    shared = false;
                 }
                 if (m_total == 0) first_pos = pos;
                 m_total++;
-                if (card == 0) have = false;  // emptied: key removed (roaring.c:2714-2718, 2803-2808)
+                if (card == 0) {  // emptied: key removed (roaring.c:2714-2718, 2803-2808)
+                    have = false;
+                    if (live && tid == 0) atomicAdd(live + pos, -1);
+                }
                 card_acc = (uint32_t)card;
                 nruns_acc = (t_acc == T_RUN) ? (uint32_t)nruns : (t_acc == T_ARRAY ? (uint32_t)card : 1024u);
                 __syncthreads();
@@ -277,9 +269,10 @@ k_compact_dir(const uint16_t *__restrict__ keys, const uint8_t *__restrict__ t_t
 }
 
 void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const uint16_t *keys,
-                     uint8_t *t_type, uint32_t *t_card, uint32_t *t_len, SetOut out, OpStats *st,
-                     cudaStream_t s) {
-    launch_kernel(k_xor_many, g_sm_count * 2, OM_THREADS, 0, s, S, idx, n, keys, t_type, t_card, t_len, out.payload, st);
+                     const uint8_t *cow, int32_t *live, uint8_t *t_type, uint32_t *t_card, uint32_t *t_len,
+                     SetOut out, OpStats *st, cudaStream_t s) {
+    launch_kernel(k_xor_many, g_sm_count * 2, OM_THREADS, 0, s, S, idx, n, keys, cow, live, t_type, t_card, t_len,
+                  out.payload, st);
     launch_kernel(k_compact_dir, 1, 1024, 0, s, keys, t_type, t_card, t_len, out, st);
 }
 
