@@ -179,6 +179,10 @@ struct OpStats {
     unsigned int cls_cursor[8];       //               fill cursors of k_order_items
     unsigned long long payload_bytes; // set builders: container_size_in_bytes of every container, summed
     unsigned int shared_used[2];      // pairwise ops: some result container points into A's / B's payload
+    unsigned int fin_blocks;          // batch ops: CTAs of k_finalize_pairs done (the last one delivers)
+    // batch ops, %globaltimer ns: the first CTA of the planner past its wait, the first and last
+    // moments of the cell kernel, the end of k_finalize_pairs' last CTA (rb200_set_op_stats)
+    unsigned long long t_begin, t_cells0, t_cells1, t_end;
 };
 
 // Code-path classes of the pairwise work items.  k_compute_items is one large kernel (a code path
@@ -277,8 +281,10 @@ bool launch_pair_fused(int op, const uint8_t *d_in, uint8_t *out_mapped, uint32_
 // g_launches: kernels launched so far (rb200_kernel_launches); launch_kernel counts each of its
 // launches, the cub calls of rb200_build.cu count their own.
 // g_sm_count: multiprocessor count of the library's device (rb200_init).
+// g_pdl: launch_kernel_chained uses programmatic dependent launch (RB200_PDL=0 at load: plain launches).
 extern unsigned long long g_launches;
 extern int g_sm_count;
+extern bool g_pdl;
 
 // Blocks for `units` work units at `per_block` units per block: at least one, at most
 // `blocks_per_sm` per multiprocessor.
@@ -294,8 +300,36 @@ inline void launch_kernel(void (*kernel)(Params...), dim3 grid, dim3 block, size
     kernel<<<grid, block, smem, s>>>(args...);
     g_launches++;
 }
+// A launch that may start while the kernel before it on the stream drains (programmatic dependent
+// launch): its CTAs run up to pdl_wait() (rb200_device.cuh) once every CTA of that kernel has called
+// pdl_trigger() or exited.  Only for kernels that call pdl_wait() before they read what an earlier
+// kernel writes or write any device memory, and pdl_trigger() only after it: then everything queued
+// before the previous kernel is complete when such a kernel starts.
+template <typename... Params, typename... Args>
+inline void launch_kernel_chained(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                                  Args... args) {
+    if (!g_pdl) {
+        launch_kernel(kernel, grid, block, smem, s, args...);
+        return;
+    }
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, (Params)args...);
+    g_launches++;
+}
 #endif
 
+// The batch-op chain k_plan_pairs -> k_order_items -> k_compute_items -> k_finalize_pairs (and
+// k_sum_cards after it) is launched with launch_kernel_chained.
+// deliver: see k_finalize_pairs (null: the counters stay in st).
 void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, const uint32_t *ib,
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
                        const PassShare &sh, Items it, OpStats *st, cudaStream_t s);
@@ -306,7 +340,8 @@ void launch_compute_items(const SetView &A, const SetView &B, Items it, uint64_t
 void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W, OpStats *st,
                        cudaStream_t s);
 void launch_finalize_pairs(const SetView &A, const SetView &B, Items it, const uint64_t *item_off,
-                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, cudaStream_t s);
+                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, OpStats *deliver,
+                           cudaStream_t s);
 void launch_finalize_cards(Items it, const uint64_t *item_off, uint32_t npairs, uint64_t *out,
                            cudaStream_t s);
 void launch_sum_cardinalities(const uint64_t *bm_card, uint32_t n, uint64_t *d_acc, cudaStream_t s);

@@ -54,6 +54,10 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
     // (tried: a lean kernel of its own for the pass-through class — 40 registers, no accumulator —
     //  launched behind this one: slower, the copies no longer overlap the cells)
     const uint4 *D = it.desc_cls ? it.desc_cls : it.desc;
+    // Wait: the class counts, the descriptors and the work counter are written by the kernels ahead
+    // (k_plan_pairs, k_order_items), and the result slab may still be read by an earlier op.
+    pdl_wait();
+    if (threadIdx.x == 0) stamp_first(&st->t_cells0);
     // (unit numbers are 32-bit: the host keeps W below 2^32; counter values past T are clamped to T)
     uint32_t n_cells = (uint32_t)W, T = (uint32_t)W;
     if (it.desc_cls) {
@@ -97,6 +101,10 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
         uint32_t nu = u + 1;
         if (nu >= e) {   // the chunk in flight becomes current, the next one is claimed
             nu = __shfl_sync(FULLMASK, pend, 0);
+            // Trigger: the claim came back past T, so every unit is handed out and this warp has only
+            // its current one left.  k_finalize_pairs may launch into the drain; it reads the results
+            // after its wait, which waits for this whole grid.
+            if (nu >= T) pdl_trigger();
             e = kc < T - nu ? nu + kc : T;
             kc = chunk(e);
             if (lane == 0) pend = claim(kc);
@@ -215,6 +223,7 @@ k_compute_items(SetView A, SetView B, Items it, uint64_t W, uint8_t *slab,
         }
 #endif
     }
+    if (lane == 0) atomicMax(&st->t_cells1, global_ns());
 #ifdef RB200_PROBE
     if (lane == 0) {
         const unsigned long long dt = (unsigned long long)(clock64() - probe_w0);
@@ -235,7 +244,7 @@ void launch_compute_items(const SetView &A, const SetView &B, Items it, uint64_t
             : op == OP_XOR  ? (lazy ? k_compute_items<OP_XOR, true> : k_compute_items<OP_XOR, false>)
                             : k_compute_items<OP_ANDNOT, false>;
     // a warp per unit, 4 per block, at most 6 resident blocks per SM
-    launch_kernel(k, grid_for(W, 4, 6), 128, 0, s, A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
+    launch_kernel_chained(k, grid_for(W, 4, 6), 128, 0, s, A, B, it, W, slab, slab_cap, st, rules, copy_ticket);
 }
 
 }  // namespace rb200

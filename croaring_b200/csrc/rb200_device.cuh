@@ -29,6 +29,21 @@ __device__ __forceinline__ unsigned lanemask_lt() {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// Programmatic dependent launch (launch_kernel_chained).  pdl_wait: returns once the kernel before
+// this one on the stream has completed and its writes are visible.  pdl_trigger: this CTA no longer
+// holds back the launch of the next kernel.  Both are no-ops in a kernel launched the plain way.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+// *t = now, unless an earlier caller already stamped it (t starts at zero)
+__device__ __forceinline__ void stamp_first(unsigned long long *t) {
+    if (!__ldcg(t)) atomicCAS(t, 0ull, global_ns());
+}
+
 __device__ __forceinline__ int popc4(const uint4 &q) {
     return __popc(q.x) + __popc(q.y) + __popc(q.z) + __popc(q.w);
 }

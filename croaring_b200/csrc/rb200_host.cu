@@ -106,6 +106,10 @@ struct Ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evk0 = nullptr, evk1 = nullptr;
     OpStats *d_stats = nullptr;
     OpStats *h_stats = nullptr;  // pinned
+    // counters of the deferred ops (DeferredCall): zero between ops without a memset on the stream —
+    // the op's k_finalize_pairs hands them to the result's pinned block and zeroes them, and every
+    // kernel of the next op touches them only after it has waited for its predecessors
+    OpStats *d_dstats = nullptr;
     uint32_t *d_flags = nullptr;   // 65536 key flags (xor_many)
     uint16_t *d_keys = nullptr;    // 65536 compacted keys
     uint32_t *d_cardkey = nullptr; // 65536 per-key cardinalities
@@ -122,7 +126,7 @@ struct Ctx {
     float last_ms = 0.f, last_compute_ms = 0.f;
     uint64_t last_download_bytes = 0;
     uint64_t last_out_portable = 0;  // portable bytes of the last batch's results (all pairs)
-    std::vector<cudaEvent_t> evpool;  // timing events recycled between batch ops (under alloc_mu)
+    std::vector<cudaEvent_t> evpool, evpool_nt;  // timing / completion-only events recycled between ops (under alloc_mu)
     struct rb200_set *last_op = nullptr;  // result of the most recent batch op (counters may be pending)
 } g;
 // rb200_last_error() is per calling thread: concurrent callers do not read each other's failures
@@ -166,6 +170,8 @@ bool ctx_init(int device = -1) {
     CK(cudaEventCreate(&g.evk0));
     CK(cudaEventCreate(&g.evk1));
     CK(cudaMalloc(&g.d_stats, sizeof(OpStats)));
+    CK(cudaMalloc(&g.d_dstats, sizeof(OpStats)));
+    CK(cudaMemset(g.d_dstats, 0, sizeof(OpStats)));
     CK(cudaHostAlloc(&g.h_stats, sizeof(OpStats), cudaHostAllocDefault));
     CK(cudaMalloc(&g.d_flags, 65536 * sizeof(uint32_t)));
     CK(cudaMalloc(&g.d_keys, 65536 * sizeof(uint16_t)));
@@ -404,7 +410,7 @@ struct rb200_set {
     bool pending = false, failed = false;
     PinBlock<OpStats> pstats;
     PinBlock<uint8_t> staging;                  // pair list of the op (alive until it ran)
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // op start, kernel start, kernel end, op end
+    cudaEvent_t done = nullptr;                 // the op's end (completion only: its times are in pstats)
     float ms = 0.f, compute_ms = 0.f;
     uint64_t algo_bytes = 0, out_portable = 0;
     // payload address of every container in the caller's host bitmaps (sets made by
@@ -471,23 +477,26 @@ SetPtr set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
     return s;
 }
 
-cudaEvent_t ev_get() {
+// timing = false: an event that only marks completion (cudaEventDisableTiming).  Recorded between two
+// programmatic launches it keeps them chained; a timing event makes the second wait for the first.
+cudaEvent_t ev_get(bool timing = true) {
+    std::vector<cudaEvent_t> &pool = timing ? g.evpool : g.evpool_nt;
     {
         std::lock_guard<std::mutex> alk(g.alloc_mu);
-        if (!g.evpool.empty()) {
-            cudaEvent_t e = g.evpool.back();
-            g.evpool.pop_back();
+        if (!pool.empty()) {
+            cudaEvent_t e = pool.back();
+            pool.pop_back();
             return e;
         }
     }
     cudaEvent_t e = nullptr;
-    cudaEventCreate(&e);
+    cudaEventCreateWithFlags(&e, timing ? cudaEventDefault : cudaEventDisableTiming);
     return e;
 }
-void ev_put(cudaEvent_t e) {
+void ev_put(cudaEvent_t e, bool timing = true) {
     if (!e) return;
     std::lock_guard<std::mutex> alk(g.alloc_mu);
-    g.evpool.push_back(e);
+    (timing ? g.evpool : g.evpool_nt).push_back(e);
 }
 
 // Host bytes -> one device buffer as a stream through two pinned chunks on the library stream: the
@@ -587,31 +596,31 @@ class SyncCall {
 
 // The ending of a batch op that returns as soon as its work is queued: its counters are taken over
 // by resolve() on first use, so consecutive ops pipeline on the stream without a host round trip.
-// begin() gives the result R four events and pinned counters, records the op's start and resets
-// the stats; kernels_begin() / kernels_end() bracket the compute kernel; finish(ok) queues the copy
-// of the counters and the op's end and hands R over, pending, with the staging block its H2D copies
-// read.  A failed call returns NULL (R is freed by its owner) after waiting for the stream while it
-// holds a staging block.  `what` heads the default t_err.
+// begin() gives the result R an event and pinned counters (zero until the op's k_finalize_pairs
+// writes them through deliver()); the op's kernels count and time themselves in g.d_dstats (see
+// OpStats::t_begin); finish(ok) records the op's end and hands R over, pending, with the staging
+// block its kernels or copies read.  No memset, copy or timing event sits between the op's kernels
+// and those of the ops before and after it, so their launches stay chained (launch_kernel_chained).
+// A failed call returns NULL (R is freed by its owner) after waiting for the stream and zeroing the
+// counters it may have left behind.  `what` heads the default t_err.
 class DeferredCall {
    public:
     DeferredCall(const char *what, SetPtr &R, PinBlock<uint8_t> &staging) : what_(what), R_(R), staging_(staging) {}
     DeferredCall(const DeferredCall &) = delete;
     bool begin() {
-        for (int k = 0; k < 4; k++) R_->ev[k] = ev_get();
-        if (!R_->pstats.reset(1) || !R_->ev[0] || !R_->ev[1] || !R_->ev[2] || !R_->ev[3]) return false;
-        cudaEventRecord(R_->ev[0], g.stream);
-        return stats_reset();
+        R_->done = ev_get(false);
+        if (!R_->pstats.reset(1) || !R_->done) return false;
+        memset(R_->pstats.get(), 0, sizeof(OpStats));
+        return cudaHostGetDevicePointer((void **)&deliver_, R_->pstats.get(), 0) == cudaSuccess;
     }
-    void kernels_begin() { cudaEventRecord(R_->ev[1], g.stream); }
-    void kernels_end() { cudaEventRecord(R_->ev[2], g.stream); }
+    OpStats *deliver() const { return deliver_; }
     rb200_set *finish(bool ok) {
-        if (ok) {
-            ok = cudaMemcpyAsync(R_->pstats.get(), g.d_stats, sizeof(OpStats), cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
-            cudaEventRecord(R_->ev[3], g.stream);
-        }
+        if (ok) ok = cudaEventRecord(R_->done, g.stream) == cudaSuccess;
         if (!ok) {
             if (t_err.empty()) t_err = std::string(what_) + ": enqueue failed";
-            if (staging_) cudaStreamSynchronize(g.stream);
+            // a chain cut short leaves its counters in g.d_dstats: zero them for the next op
+            if (deliver_) cudaMemsetAsync(g.d_dstats, 0, sizeof(OpStats), g.stream);
+            if (staging_ || deliver_) cudaStreamSynchronize(g.stream);
             return nullptr;
         }
         R_->pending = true;
@@ -625,12 +634,14 @@ class DeferredCall {
     const char *what_;
     SetPtr &R_;
     PinBlock<uint8_t> &staging_;
+    OpStats *deliver_ = nullptr;   // R's pinned counters, device address
 };
 
 // The batch op that produced s has run (or was never enqueued): its events, counters and pair list
 // go back to the pools.
 void retire_op(rb200_set *s) {
-    for (int k = 0; k < 4; k++) { ev_put(s->ev[k]); s->ev[k] = nullptr; }
+    ev_put(s->done, false);
+    s->done = nullptr;
     s->pstats.reset();
     s->staging.reset();
 }
@@ -645,7 +656,7 @@ bool resolve(const rb200_set *cs) {
     }
     s->pending = false;
     const OpStats &st = *s->pstats.get();
-    cudaError_t e = cudaEventSynchronize(s->ev[3]);
+    cudaError_t e = cudaEventSynchronize(s->done);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) {
         t_err = std::string("batch op: ") + cudaGetErrorString(e);
@@ -654,8 +665,8 @@ bool resolve(const rb200_set *cs) {
         t_err = st.error == 2 ? "internal: result slab bound exceeded" : "internal: result slot bound exceeded";
         s->failed = true;
     } else {
-        cudaEventElapsedTime(&s->ms, s->ev[0], s->ev[3]);
-        cudaEventElapsedTime(&s->compute_ms, s->ev[1], s->ev[2]);
+        s->ms = st.t_end > st.t_begin ? (float)((st.t_end - st.t_begin) * 1e-6) : 0.f;
+        s->compute_ms = st.t_cells1 > st.t_cells0 ? (float)((st.t_cells1 - st.t_cells0) * 1e-6) : 0.f;
         s->algo_bytes = st.algo_bytes;
         s->out_portable = st.out_portable;
         s->n_containers = st.dir_cursor;
@@ -1267,6 +1278,8 @@ struct ItemsBuf {
 };
 
 // pair lists + item offsets: one pinned staging block, one H2D copy
+// (tried: k_plan_pairs reading the staging block through its mapped address instead, which keeps the
+//  copy off the stream — its scattered 4- and 8-byte reads over PCIe made the kernel 2-3x slower)
 struct PairBuf {
     PinBlock<uint8_t> h;
     DevBlock<uint8_t> d;
@@ -1276,6 +1289,7 @@ struct PairBuf {
     // result slab bound for the sharing mode `share` of build() (bit 0: A's pass-through containers
     // shared, bit 1: B's), and the bound when everything is copied
     uint64_t slab_bound = 0, slab_bound_copy = 0;
+    bool cow = false;   // some selected bitmap of A or B carries the COW flag
     // op: OP_* of the batch (OP_AND also for the cardinality-only sweeps, which need no slab)
     // rules: RULES_* of the batch; with RULES_FLIP, B is the range bitmap of rb200_batch_flip (every
     // container ONE run)
@@ -1290,6 +1304,7 @@ struct PairBuf {
         uint64_t *off = (uint64_t *)(h.get() + o_off);
         uint32_t *hia = (uint32_t *)(h.get() + o_ia), *hib = (uint32_t *)(h.get() + o_ib);
         uint64_t w = 0, sb = 0, sbs = 0;
+        uint8_t flags = 0;
         for (size_t p = 0; p < np; p++) {
             const uint32_t a = ia[p], b = ib[p];
             if (a >= A->n_bitmaps || b >= B->n_bitmaps) {
@@ -1298,6 +1313,7 @@ struct PairBuf {
             }
             hia[p] = a;
             hib[p] = b;
+            flags |= A->h_flags[a] | B->h_flags[b];
             off[p] = w;
             const uint32_t na = A->h_cnt[a], nb = B->h_cnt[b];
             w += (uint64_t)na + nb;
@@ -1345,6 +1361,7 @@ struct PairBuf {
             }
         }
         off[np] = w;
+        cow = (flags & FLAG_COW) != 0;
         // item ids, directory positions of the result and the order list are 32-bit on the device
         if (w > 0xffffffffull) { t_err = "batch too large: more than 2^32 - 1 container slots, split the pair list"; return false; }
         W = w;
@@ -1542,9 +1559,8 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     if (ok) {
         const SetView va = A->view(), vb = B->view();
         launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, op, false, rules, sh, ib_.it,
-                          g.d_stats, g.stream);
-        launch_order_items(ib_.it, pb.W, g.d_stats, g.stream);
-        call.kernels_begin();
+                          g.d_dstats, g.stream);
+        launch_order_items(ib_.it, pb.W, g.d_dstats, g.stream);
         // pass-through tickets: one item per lane, fewer lanes when the operands' containers are big
         // (32 x 8 KiB on one warp would be the tail of the launch)
         const uint64_t n_cont = A->n_containers + B->n_containers;
@@ -1553,15 +1569,18 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
         //  clearly slower — RB200_COPY_TICKET overrides)
         static const int ct_env = []() { const char *e = getenv("RB200_COPY_TICKET"); return e ? std::min(32, std::max(1, atoi(e))) : 0; }();
         const int copy_ticket = ct_env ? ct_env : avg_b <= 256 ? 32 : avg_b <= 2048 ? 16 : 8;
-        launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_stats, rules, copy_ticket, g.stream);
-        call.kernels_end();
-        launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, sh, R->out(), g.d_stats, g.stream);
+        launch_compute_items(va, vb, ib_.it, pb.W, op, R->d_slab, R->slab_cap, g.d_dstats, rules, copy_ticket, g.stream);
+        launch_finalize_pairs(va, vb, ib_.it, pb.d_off, (uint32_t)np, sh, R->out(), g.d_dstats, call.deliver(),
+                              g.stream);
         R->parentA = A->h_ptr;
         R->parentB = B->h_ptr;
         R->lazy = (rules & RULES_LAZY) != 0 && !(rules & RULES_FLIP);
-        for (size_t p = 0; p < np; p++)
-            R->h_flags[p] = result_cow(op, rules, A->h_flags[ia[p]], B->h_flags[ib[p]], A->h_cnt[ia[p]] == 0,
-                                       B->h_cnt[ib[p]] == 0);
+        // without a COW operand every result flag is 0, as set_new left them (result_cow of two zero
+        // flags); the per-pair rules cost more host time than a small batch call takes on the device
+        if (pb.cow)
+            for (size_t p = 0; p < np; p++)
+                R->h_flags[p] = result_cow(op, rules, A->h_flags[ia[p]], B->h_flags[ib[p]], A->h_cnt[ia[p]] == 0,
+                                           B->h_cnt[ib[p]] == 0);
     }
     // the device buffers go back when pb / ib_ leave scope: stream-ordered reuse
     return call.finish(ok);
@@ -3319,11 +3338,9 @@ rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, s
         const SetView vs = S->view();
         const uint64_t *d_off = (const uint64_t *)(d.get() + o_off);
         launch_offset_plan(vs, (const uint32_t *)(d.get() + o_idx), (const int64_t *)(d.get() + o_ofs), d_off,
-                           (uint32_t)n, sh, ib_.it, cell.get(), R->slab_cap, g.d_stats, g.stream);
-        call.kernels_begin();
-        launch_offset_cells(vs, ib_.it, cell.get(), w, sh.bias, R->d_slab, g.d_stats, g.stream);
-        call.kernels_end();
-        launch_finalize_pairs(vs, vs, ib_.it, d_off, (uint32_t)n, sh, R->out(), g.d_stats, g.stream);
+                           (uint32_t)n, sh, ib_.it, cell.get(), R->slab_cap, g.d_dstats, g.stream);
+        launch_offset_cells(vs, ib_.it, cell.get(), w, sh.bias, R->d_slab, g.d_dstats, g.stream);
+        launch_finalize_pairs(vs, vs, ib_.it, d_off, (uint32_t)n, sh, R->out(), g.d_dstats, call.deliver(), g.stream);
         R->parentA = S->h_ptr;
         for (size_t p = 0; p < n; p++) R->h_flags[p] = S->h_flags[hidx[p]] & FLAG_COW;   // roaring.c:2449-2450
     }

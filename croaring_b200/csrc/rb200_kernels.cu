@@ -16,6 +16,7 @@ namespace rb200 {
 
 unsigned long long g_launches = 0;
 int g_sm_count = 132;   // until rb200_init reads the device's
+bool g_pdl = []() { const char *e = getenv("RB200_PDL"); return !(e && e[0] == '0'); }();
 
 // code-path class of a matched cell (see rb200_common.h CLS_*); mirrors the branches of cell_compute
 __device__ __forceinline__ int cell_class(int op, int rules, int tA, int tB, uint32_t cA, uint32_t cB, uint32_t lA,
@@ -48,16 +49,51 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
     __shared__ unsigned long long s_base;
     __shared__ unsigned int s_used[2];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    // Before the wait: lane r fetches the warp's pair of round r (the first 32 rounds, all loads in
+    // flight together) and the sizes of its two bitmaps.  The pair list arrives by a copy queued
+    // right before this launch, which is never overlapped, and the operands' directories were
+    // complete when the launch was queued (the host settles a pending operand before it plans a
+    // batch on it: ensure_mirrors), so none of this depends on the kernel still draining ahead.
+    const uint32_t stride = gridDim.x * 4;
+    uint32_t r_a0 = 0, r_na = 0, r_b0 = 0, r_nb = 0;
+    uint64_t r_off = 0;
+    {
+        const uint64_t p = (uint64_t)blockIdx.x * 4 + wid + (uint64_t)lane * stride;
+        if (p < npairs) {
+            const uint32_t a = ia[p], b = ib[p];
+            r_off = item_off[p];
+            r_a0 = A.bm_beg[a];
+            r_na = A.bm_cnt[a];
+            r_b0 = B.bm_beg[b];
+            r_nb = B.bm_cnt[b];
+        }
+    }
+    // Wait: from here on the kernel writes device buffers (item records, counters), which
+    // may have been released by the previous op to the stream-ordered pool while that op's kernels
+    // still read them, and the counters of `st` are zeroed by the previous op's k_finalize_pairs.
+    pdl_wait();
+    if (threadIdx.x == 0) stamp_first(&st->t_begin);
     if (threadIdx.x < N_CLS) s_cls[threadIdx.x] = 0;
     if (threadIdx.x < 2) s_used[threadIdx.x] = 0;
     __syncthreads();
-    for (uint32_t p0 = blockIdx.x * 4; p0 < npairs; p0 += gridDim.x * 4) {
+    uint32_t round = 0;
+    for (uint32_t p0 = blockIdx.x * 4; p0 < npairs; p0 += stride, round++) {
         const uint32_t p = p0 + wid;
         const bool vp = p < npairs;
-        const uint32_t a = vp ? ia[p] : 0, b = vp ? ib[p] : 0;
-        const uint32_t a0 = vp ? A.bm_beg[a] : 0, na = vp ? A.bm_cnt[a] : 0;
-        const uint32_t b0 = vp ? B.bm_beg[b] : 0, nb = vp ? B.bm_cnt[b] : 0;
-        const uint64_t base_item = vp ? item_off[p] : 0;
+        uint32_t a0, na, b0, nb;
+        uint64_t base_item;
+        if (round < 32) {
+            a0 = __shfl_sync(FULLMASK, r_a0, round);
+            na = __shfl_sync(FULLMASK, r_na, round);
+            b0 = __shfl_sync(FULLMASK, r_b0, round);
+            nb = __shfl_sync(FULLMASK, r_nb, round);
+            base_item = __shfl_sync(FULLMASK, r_off, round);
+        } else {
+            const uint32_t a = vp ? ia[p] : 0, b = vp ? ib[p] : 0;
+            a0 = vp ? A.bm_beg[a] : 0, na = vp ? A.bm_cnt[a] : 0;
+            b0 = vp ? B.bm_beg[b] : 0, nb = vp ? B.bm_cnt[b] : 0;
+            base_item = vp ? item_off[p] : 0;
+        }
         const uint32_t tot = na + nb;
         for (uint32_t t0 = 0;; t0 += 32) {
             if (!__syncthreads_or(t0 < tot)) break;   // (also keeps the rounds' shared words apart)
@@ -166,6 +202,9 @@ k_plan_pairs(SetView A, SetView B, const uint32_t *__restrict__ ia,
             }
         }
     }
+    // Trigger: what is left is one atomic per class.  The next kernel reads the counters and item
+    // records only after its own wait, which waits for this whole grid.
+    pdl_trigger();
     __syncthreads();
     if (it.cls && threadIdx.x < N_CLS && s_cls[threadIdx.x]) atomicAdd(&st->cls_count[threadIdx.x], s_cls[threadIdx.x]);
     if (threadIdx.x < 2 && s_used[threadIdx.x]) st->shared_used[threadIdx.x] = 1u;
@@ -178,6 +217,8 @@ __global__ void __launch_bounds__(256)
 k_order_items(Items it, uint64_t W, OpStats *st) {
     __shared__ uint32_t s_wcnt[8][N_CLS], s_base[N_CLS];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    // Wait: everything this kernel reads (class counts, classes, descriptors) is k_plan_pairs' output.
+    pdl_wait();
     uint32_t pre_l = 0;   // lane c (< N_CLS): first slot of class c in the order list
     for (int c = 0; c < N_CLS; c++)
         if (c < lane) pre_l += st->cls_count[c];
@@ -231,6 +272,9 @@ k_order_items(Items it, uint64_t W, OpStats *st) {
         }
         __syncthreads();
     }
+    // Trigger: this CTA has placed its last descriptor; the cell kernel waits for the whole grid
+    // before it reads the order list.
+    pdl_trigger();
 }
 
 // (the pairwise cell kernel, k_compute_items, is in rb200_compute.cu; the grid cells themselves —
@@ -302,15 +346,19 @@ k_card_items(SetView A, SetView B, Items it, uint64_t W, OpStats *st) {
 #ifndef RB200_FIN_BLOCKS
 #define RB200_FIN_BLOCKS 16
 #endif
+// deliver (null: the counters stay in st for the caller): the last CTA copies the counters resolve()
+// reads into this mapped pinned block, then zeroes st for the next op.
 __global__ void __launch_bounds__(128)
 k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ item_off,
-                 uint32_t npairs, uint32_t rw_a, uint32_t rw_b, SetOut out, OpStats *st) {
+                 uint32_t npairs, uint32_t rw_a, uint32_t rw_b, SetOut out, OpStats *st, OpStats *deliver) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     // the four pairs of a block reserve their directory range with ONE atomic (the cursor is a single
     // address: one returning atomic per pair serialised 19 900 of them per launch)
     __shared__ uint32_t s_cnt[4];
     __shared__ unsigned long long s_base;
     unsigned long long acc_bytes = 0, acc_outb = 0;  // per-warp totals: one atomic each at the end
+    // Wait before everything: the result records come from the cell kernel still draining ahead.
+    pdl_wait();
     for (uint32_t p0 = blockIdx.x * 4; p0 < npairs; p0 += gridDim.x * 4) {
         const uint32_t p = p0 + wid;
         const bool vp = p < npairs;
@@ -388,6 +436,9 @@ k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ it
             done += __popc(m);
         }
     }
+    // Trigger: the directory of this CTA's pairs is written; the next kernel waits for the whole
+    // grid before it reads the result.
+    pdl_trigger();
     __shared__ unsigned long long s_tot[4][2];
     if (lane == 0) { s_tot[wid][0] = acc_bytes; s_tot[wid][1] = acc_outb; }
     __syncthreads();
@@ -395,6 +446,31 @@ k_finalize_pairs(SetView A, SetView B, Items it, const uint64_t *__restrict__ it
         const unsigned long long v = s_tot[0][threadIdx.x] + s_tot[1][threadIdx.x] + s_tot[2][threadIdx.x] + s_tot[3][threadIdx.x];
         if (v) atomicAdd(threadIdx.x ? &st->out_portable : &st->algo_bytes, v);
     }
+    if (!deliver) return;
+    // the last CTA to get here sees every other CTA's counters (fence, then the ticket)
+    __shared__ bool s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(&st->fin_blocks, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (threadIdx.x == 0) {
+        deliver->slab_cursor = __ldcg(&st->slab_cursor);
+        deliver->dir_cursor = __ldcg(&st->dir_cursor);
+        deliver->algo_bytes = __ldcg(&st->algo_bytes);
+        deliver->out_portable = __ldcg(&st->out_portable);
+        deliver->error = __ldcg(&st->error);
+        deliver->shared_used[0] = __ldcg(&st->shared_used[0]);
+        deliver->shared_used[1] = __ldcg(&st->shared_used[1]);
+        deliver->t_begin = __ldcg(&st->t_begin);
+        deliver->t_cells0 = __ldcg(&st->t_cells0);
+        deliver->t_cells1 = __ldcg(&st->t_cells1);
+        deliver->t_end = global_ns();
+    }
+    __syncthreads();
+    // every kernel of the next op that touches st waits for this grid first
+    for (uint32_t k = threadIdx.x; k < sizeof(OpStats) / 4; k += blockDim.x) reinterpret_cast<uint32_t *>(st)[k] = 0u;
 }
 
 __global__ void __launch_bounds__(128)
@@ -428,8 +504,12 @@ __global__ void k_set_cardinalities(SetView S, uint32_t n, uint64_t *__restrict_
 
 // *acc += sum of bm_card[0..n) (device-resident checksum of a result set)
 __global__ void k_sum_cards(const uint64_t *__restrict__ bm_card, uint32_t n, unsigned long long *acc) {
+    // Wait: bm_card is written by the op that produced the set, usually the kernel right ahead.
+    pdl_wait();
     unsigned long long v = 0;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) v += bm_card[i];
+    // Trigger: only the warp sums and one atomic per warp are left.
+    pdl_trigger();
     v = warp_sum(v);
     if ((threadIdx.x & 31) == 0 && v) atomicAdd(acc, v);
 }
@@ -569,13 +649,13 @@ void launch_plan_pairs(const SetView &A, const SetView &B, const uint32_t *ia, c
                        const uint64_t *item_off, uint32_t npairs, int op, bool card_only, int rules,
                        const PassShare &sh, Items it, OpStats *st, cudaStream_t s) {
     if (!npairs) return;
-    launch_kernel(k_plan_pairs, grid_for(npairs, 4, 16), 128, 0, s, A, B, ia, ib, item_off, npairs, op, card_only,
-                  rules, sh, it, st);
+    launch_kernel_chained(k_plan_pairs, grid_for(npairs, 4, 16), 128, 0, s, A, B, ia, ib, item_off, npairs, op,
+                          card_only, rules, sh, it, st);
 }
 
 void launch_order_items(Items it, uint64_t W, OpStats *st, cudaStream_t s) {
     if (!W || !it.desc_cls) return;
-    launch_kernel(k_order_items, grid_for(W, 2048, 8), 256, 0, s, it, W, st);
+    launch_kernel_chained(k_order_items, grid_for(W, 2048, 8), 256, 0, s, it, W, st);
 }
 
 void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W, OpStats *st,
@@ -586,11 +666,12 @@ void launch_card_items(const SetView &A, const SetView &B, Items it, uint64_t W,
 }
 
 void launch_finalize_pairs(const SetView &A, const SetView &B, Items it, const uint64_t *item_off,
-                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, cudaStream_t s) {
+                           uint32_t npairs, const PassShare &sh, SetOut out, OpStats *st, OpStats *deliver,
+                           cudaStream_t s) {
     if (!npairs) return;
     // a warp per pair, full residency (16 CTAs of 4 warps per SM); counters: one atomic per block
-    launch_kernel(k_finalize_pairs, grid_for(npairs, 4, RB200_FIN_BLOCKS), 128, 0, s, A, B, it, item_off, npairs,
-                  sh.onA ? 0u : 2u, sh.onB ? 0u : 2u, out, st);
+    launch_kernel_chained(k_finalize_pairs, grid_for(npairs, 4, RB200_FIN_BLOCKS), 128, 0, s, A, B, it, item_off,
+                          npairs, sh.onA ? 0u : 2u, sh.onB ? 0u : 2u, out, st, deliver);
 }
 
 void launch_finalize_cards(Items it, const uint64_t *item_off, uint32_t npairs, uint64_t *out,
@@ -602,7 +683,7 @@ void launch_finalize_cards(Items it, const uint64_t *item_off, uint32_t npairs, 
 void launch_sum_cardinalities(const uint64_t *bm_card, uint32_t n, uint64_t *d_acc, cudaStream_t s) {
     if (!n) return;
     const uint32_t blocks = (n + 255) / 256 < 592u ? (n + 255) / 256 : 592u;
-    launch_kernel(k_sum_cards, blocks, 256, 0, s, bm_card, n, (unsigned long long *)d_acc);
+    launch_kernel_chained(k_sum_cards, blocks, 256, 0, s, bm_card, n, (unsigned long long *)d_acc);
 }
 void launch_set_cardinalities(const SetView &S, uint32_t n, uint64_t *out, cudaStream_t s) {
     if (!n) return;

@@ -56,6 +56,7 @@ k_offset_plan(SetView S, const uint32_t *__restrict__ idx, const int64_t *__rest
               uint64_t slab_cap, OpStats *st) {
     const int lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+    if (threadIdx.x == 0) stamp_first(&st->t_begin);
     bool used = false;
     for (uint32_t p = warp; p < n; p += nwarps) {
         const uint32_t b = idx ? idx[p] : p;
@@ -204,6 +205,7 @@ k_offset_cells(SetView S, Items it, const uint4 *__restrict__ cell, uint64_t W, 
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     uint32_t *acc = s_acc[wid];
     const uint64_t warp = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * (uint64_t)blockDim.x) >> 5;
+    if (threadIdx.x == 0) stamp_first(&st->t_cells0);
     for (uint64_t j0 = warp * 32; j0 < W; j0 += nwarps * 32) {
         const uint64_t jl = j0 + lane;
         unsigned m = __ballot_sync(FULLMASK, jl < W && (cell[jl].z >> 16) != OFS_NONE);
@@ -302,6 +304,7 @@ k_offset_cells(SetView S, Items it, const uint4 *__restrict__ cell, uint64_t W, 
             }
         }
     }
+    if (lane == 0) atomicMax(&st->t_cells1, global_ns());
 }
 
 void launch_offset_plan(const SetView &S, const uint32_t *idx, const int64_t *offsets, const uint64_t *item_off,
