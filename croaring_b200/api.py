@@ -95,6 +95,8 @@ def lib():
                  "rb200_set64_batch_remove_many"):
         sig(name, _P, _P, _P, C.c_size_t, _P, _P)
         sig(name + "_device", _P, _P, _P, C.c_size_t, _P, _P)
+    sig("rb200_batch_query", C.c_int, C.c_int, _P, _P, C.c_size_t, _P, _P)
+    sig("rb200_batch_query_device", C.c_int, C.c_int, _P, _P, C.c_size_t, _P, _P)
     sig("rb200_r64_batch_op_serialized", C.c_int, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
         C.c_size_t, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t, _P, _P, C.c_size_t,
         C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)), C.POINTER(C.POINTER(C.c_uint64)))
@@ -584,6 +586,78 @@ def _update(s, fn, values, offsets, idx):
     return getattr(lib(), fn)(s.ptr, ip, n, vp, op)
 
 
+QUERIES = {"contains": 0, "rank": 1, "get_index": 2, "select": 3}   # RB200_Q_*
+
+
+def _query_index(idx, n, n_all):
+    """The bitmap of every query: (None, n_all) for idx None (one query per bitmap), else a uint32 array of
+    n entries, a scalar idx broadcast to all of them."""
+    if idx is None:
+        if n != n_all:
+            raise RB200Error(f"{n} values for the {n_all} bitmaps of the set (idx=None asks each bitmap once)")
+        return None
+    if np.ndim(idx) == 0:
+        if not isinstance(idx, (int, np.integer)) or isinstance(idx, bool) or not 0 <= int(idx) <= 0xFFFFFFFF:
+            raise RB200Error(f"idx must be an integer in [0, 2^32), got {idx!r}")
+        return int(idx)
+    ia = _values_u32(idx)
+    if ia.size != n:
+        raise RB200Error(f"idx has {ia.size} entries for {n} values")
+    return ia
+
+
+def _query(s, kind, values, idx):
+    """out[k] = the answer of bitmap idx[k] of the set s about values[k] (rb200_batch_query); CUDA tensor
+    values go through rb200_batch_query_device and the answers stay on their device."""
+    if kind not in QUERIES:
+        raise RB200Error(f"unknown query kind {kind!r}: one of {sorted(QUERIES)}")
+    if getattr(values, "is_cuda", False):
+        return _query_device(s, QUERIES[kind], values, idx)
+    vals = _values_u32(values)
+    ia = _query_index(idx, vals.size, len(s))
+    out = np.empty(vals.size, dtype=np.int64)
+    if ia is not None and not vals.size:
+        return out   # (the library reads a NULL idx as one query per bitmap)
+    if isinstance(ia, int):
+        ia = np.full(vals.size, ia, dtype=np.uint32)
+    if lib().rb200_batch_query(QUERIES[kind], s.ptr, None if ia is None else ia.ctypes.data, vals.size,
+                               vals.ctypes.data, out.ctypes.data) != 0:
+        raise RB200Error(last_error())
+    return out
+
+
+def _device_u32(t, what):
+    import torch
+    if t.dtype not in (torch.int32, torch.uint32) or t.dim() != 1 or not t.is_contiguous():
+        raise RB200Error(f"device {what} must be a contiguous 1-D int32 / uint32 CUDA tensor")
+    return t
+
+
+def _query_device(s, code, values, idx):
+    import torch
+    values = _device_u32(values, "values")
+    dev, n = values.device, values.numel()
+    if isinstance(idx, torch.Tensor):
+        ia = _device_u32(idx.to(dev), "idx")
+        if ia.numel() != n:
+            raise RB200Error(f"idx has {ia.numel()} entries for {n} values")
+    else:
+        ia = _query_index(idx, n, len(s))
+        if isinstance(ia, int):   # expanded on the values' device, as the int32 of the same bits
+            ia = torch.full((n,), ia - (1 << 32) if ia >= 1 << 31 else ia, dtype=torch.int32, device=dev)
+        elif ia is not None:
+            ia = torch.from_numpy(ia.view(np.int32)).to(dev)
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    if ia is not None and not n:
+        return out   # (an empty tensor's address is NULL, which the library reads as one query per bitmap)
+    # the library stream reads and writes these: what torch's stream queued on them comes first
+    torch.cuda.current_stream(dev).synchronize()
+    if lib().rb200_batch_query_device(code, s.ptr, None if ia is None else ia.data_ptr(), n, values.data_ptr(),
+                                      out.data_ptr()) != 0:
+        raise RB200Error(last_error())
+    return out
+
+
 class DeviceSet:
     """An ordered collection of bitmaps resident in HBM (rb200_set_t*)."""
 
@@ -733,6 +807,26 @@ class DeviceSet:
     def remove_many(self, values, offsets=None, idx=None):
         """roaring_bitmap_remove_many of every (or the selected) bitmap, as add_many."""
         return DeviceSet(_update(self, "rb200_batch_remove_many", values, offsets, idx))
+
+    # -- point queries.  values[k] is asked of bitmap idx[k]: idx None asks bitmap k (one value per bitmap),
+    # an array gives one bitmap per value, a scalar asks every value of one bitmap.  Host values (arrays,
+    # lists) give a numpy int64 array; a CUDA tensor of int32 / uint32 values (read in place on the library
+    # stream, order its writes before the call as for from_values) gives an int64 tensor on its device.
+    def contains(self, values, idx=None):
+        """roaring_bitmap_contains per query: 1 or 0."""
+        return _query(self, "contains", values, idx)
+
+    def rank(self, values, idx=None):
+        """roaring_bitmap_rank per query: the number of values <= values[k] (up to 2^32)."""
+        return _query(self, "rank", values, idx)
+
+    def get_index(self, values, idx=None):
+        """roaring_bitmap_get_index per query: the index of values[k] in its bitmap, or -1."""
+        return _query(self, "get_index", values, idx)
+
+    def select(self, ranks, idx=None):
+        """roaring_bitmap_select per query: the value of 0-based rank ranks[k], or -1 past the cardinality."""
+        return _query(self, "select", ranks, idx)
 
     def op_stats(self):
         """(device_ms, compute_kernel_ms, algorithmic_bytes) of the batch op that produced this set."""

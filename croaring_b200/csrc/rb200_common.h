@@ -445,4 +445,14 @@ void launch_xor_many(const SetView &S, const uint32_t *idx, uint32_t n, const ui
                      const uint8_t *cow, int32_t *live, uint8_t *t_type, uint32_t *t_card, uint32_t *t_len,
                      SetOut out, OpStats *st, cudaStream_t s);
 
+// Point queries (rb200_query.cu), the RB200_Q_* kinds of include/roaring_b200.h.  Query k asks bitmap
+// idx[k] (idx null: k) of S about vals[k] and writes out[k]; an idx[k] >= n_bitmaps gets -1, and the
+// least such k is atomicMin'ed into *bad.  c_cum: the exclusive scan of the masked cardinalities of
+// S's directory entries (null for Q_CONTAINS, which never reads it), built from what
+// launch_query_cards writes (nc + 1 entries, the last zero).
+constexpr int Q_CONTAINS = 0, Q_RANK = 1, Q_GET_INDEX = 2, Q_SELECT = 3;
+void launch_query(int kind, const SetView &S, const uint64_t *c_cum, uint32_t n_bitmaps, const uint32_t *idx,
+                  const uint32_t *vals, uint32_t n, int64_t *out, unsigned long long *bad, cudaStream_t s);
+void launch_query_cards(const uint32_t *c_card, uint64_t nc, uint64_t *out, cudaStream_t s);
+
 }  // namespace rb200

@@ -424,6 +424,9 @@ struct rb200_set {
     // host copy of the directory (pinned) and, for a set packed for download, of its payload
     PinBlock<uint8_t> m_dir, m_slab;
     SetPtr mirror;                  // rb200_set_download: this set packed, directory and payload on the host
+    // exclusive scan of the directory's cardinalities (n_containers + 1 entries), built by the first
+    // rank / get_index / select query (ensure_cum); a set never changes after the op that made it
+    DevBlock<uint64_t> c_cum;
 
     SetView view() const {
         const uint8_t *d = d_dir.get();
@@ -1389,14 +1392,19 @@ bool reject_lazy(const rb200_set *s, const char *what) {
     return true;
 }
 
+// the message of a selection whose entry idx[k] = v is out of range of a set of `count` bitmaps
+void index_error(const char *what, size_t k, uint32_t v, uint64_t count) {
+    t_err = std::string(what) + ": index out of range: idx[" + std::to_string(k) + "] = " + std::to_string(v) +
+            ", the set holds " + std::to_string(count) + " bitmaps";
+}
+
 // idx[0..n) of a selection of a set of `count` bitmaps: n < 2^32 (checked before idx is read) and
 // every entry in range; `what` heads t_err.
 bool check_indices(const char *what, const uint32_t *idx, size_t n, uint64_t count) {
     if (n > 0xffffffffull) { t_err = std::string(what) + ": more than 2^32 - 1 bitmaps selected"; return false; }
     for (size_t k = 0; k < n; k++) {
         if (idx[k] >= count) {
-            t_err = std::string(what) + ": index out of range: idx[" + std::to_string(k) + "] = " +
-                    std::to_string(idx[k]) + ", the set holds " + std::to_string(count) + " bitmaps";
+            index_error(what, k, idx[k], count);
             return false;
         }
     }
@@ -3438,6 +3446,128 @@ rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t
                                             const uint32_t *d_vals, const uint64_t *d_off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return update_device(OP_ANDNOT, "remove_many_device", S, idx, n, d_vals, d_off);
+}
+
+// ---- point queries: roaring_bitmap_contains / rank / get_index / select (roaring.h:478, src/roaring.c:2862,
+// 2916, 2974) ---------------------------------------------------------------------------------------
+// out[k] = the answer of bitmap S[idx[k]] about vals[k], a warp per query (rb200_query.cu).  rank, get_index
+// and select add the cardinalities of the containers before the answer's; they come from the set's c_cum,
+// built once by the first such query.
+namespace {
+// The arguments of a query call other than its selection: the kind, then vals / out (NULL only if n == 0).
+bool query_args(const char *what, int kind, size_t n, const void *vals, const void *out) {
+    if (kind < Q_CONTAINS || kind > Q_SELECT) {
+        t_err = std::string(what) + ": unknown query kind " + std::to_string(kind);
+        return false;
+    }
+    if (n && !vals) { t_err = std::string(what) + ": vals are NULL"; return false; }
+    if (n && !out) { t_err = std::string(what) + ": out is NULL"; return false; }
+    return true;
+}
+// p is device (or managed) memory of the library's device
+bool device_memory(const char *what, const char *name, const void *p) {
+    cudaPointerAttributes a = {};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        (void)cudaGetLastError();
+        a.type = cudaMemoryTypeUnregistered;
+    }
+    if ((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == g.device) return true;
+    t_err = std::string(what) + ": " + name + " is not device memory of the library's device";
+    return false;
+}
+// The set's c_cum on the library stream, unless it is there already.  A set without containers has
+// none: every bitmap is empty and no query reads it.
+bool ensure_cum(const rb200_set *cs) {
+    rb200_set *s = const_cast<rb200_set *>(cs);
+    const uint64_t nc = s->n_containers;
+    if (s->c_cum || !nc) return true;
+    if (nc >= 0x7fffffffull) { t_err = "query: more than 2^31 - 2 containers in the set"; return false; }
+    DevBlock<uint64_t> cards(nc + 1), cum(nc + 1);
+    DevBlock<uint8_t> temp;
+    size_t tb = 0;
+    if (!cards || !cum) return false;
+    if (!build_scan(nullptr, &tb, cards.get(), cum.get(), nc + 1, g.stream) || !temp.reset(tb)) {
+        if (t_err.empty()) t_err = "query: scan setup failed";
+        return false;
+    }
+    launch_query_cards(s->view().c_card, nc, cards.get(), g.stream);
+    if (!build_scan(temp.get(), &tb, cards.get(), cum.get(), nc + 1, g.stream)) {
+        t_err = "query: scan launch failed";
+        return false;
+    }
+    s->c_cum = std::move(cum);   // cards and temp go back to the pool: stream-ordered reuse
+    return true;
+}
+bool query_enqueue(int kind, const rb200_set *S, const uint32_t *d_idx, size_t n, const uint32_t *d_vals,
+                   int64_t *d_out, unsigned long long *d_bad) {
+    if (kind != Q_CONTAINS && !ensure_cum(S)) return false;
+    launch_query(kind, S->view(), S->c_cum.get(), S->n_bitmaps, d_idx, d_vals, (uint32_t)n, d_out, d_bad, g.stream);
+    return true;
+}
+}  // namespace
+
+int rb200_batch_query(int kind, const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                      int64_t *out) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    Selection sel{S, idx, n};
+    if (!sel.check("query") || !query_args("query", kind, sel.n, vals, out)) return -1;   // before any CUDA call
+    if (!ctx_init() || !ensure_mirrors(S)) return -1;   // a failed batch op fails here, not as data
+    n = sel.n;
+    if (!n) return 0;
+    // one block each way: [first bad position | idx | vals] up, out down
+    const size_t o_idx = al256(8), o_vals = o_idx + (sel.all() ? 0 : al256(4 * n)), o_out = o_vals + al256(4 * n);
+    const size_t bytes = o_out + 8 * n;
+    PinBlock<uint8_t> h(bytes);
+    DevBlock<uint8_t> d(bytes);
+    if (!h || !d) return -1;
+    memset(h.get(), 0xff, 8);
+    if (!sel.all()) memcpy(h.get() + o_idx, idx, 4 * n);
+    memcpy(h.get() + o_vals, vals, 4 * n);
+    SyncCall call("query", "query launch");
+    bool ok = cudaMemcpyAsync(d.get(), h.get(), o_out, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+              query_enqueue(kind, S, sel.all() ? nullptr : (const uint32_t *)(d.get() + o_idx), n,
+                            (const uint32_t *)(d.get() + o_vals), (int64_t *)(d.get() + o_out),
+                            (unsigned long long *)d.get()) &&
+              cudaMemcpyAsync(h.get() + o_out, d.get() + o_out, 8 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    ok = call.finish(ok, false);
+    if (ok) memcpy(out, h.get() + o_out, 8 * n);
+    return ok ? 0 : -1;
+}
+
+int rb200_batch_query_device(int kind, const rb200_set_t *S, const uint32_t *d_idx, size_t n, const uint32_t *d_vals,
+                             int64_t *d_out) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    Selection sel{S, nullptr, n};
+    if (!sel.check("query_device")) return -1;   // the entries of d_idx are checked by the kernel
+    if (d_idx) {
+        if (n > 0xffffffffull) { t_err = "query_device: more than 2^32 - 1 queries"; return -1; }
+        sel.n = n;
+    }
+    n = sel.n;
+    if (!query_args("query_device", kind, n, d_vals, d_out) || !ctx_init()) return -1;
+    // a host pointer never reaches the kernel
+    if (n && (!device_memory("query_device", "vals", d_vals) || !device_memory("query_device", "out", d_out) ||
+              (d_idx && !device_memory("query_device", "idx", d_idx))))
+        return -1;
+    if (!ensure_mirrors(S)) return -1;
+    if (!n) return 0;
+    DevBlock<unsigned long long> d_bad(1);
+    PinBlock<unsigned long long> h_bad(1);
+    if (!d_bad || !h_bad) return -1;
+    SyncCall call("query_device", "query_device launch");
+    bool ok = cudaMemsetAsync(d_bad.get(), 0xff, 8, g.stream) == cudaSuccess &&
+              query_enqueue(kind, S, d_idx, n, d_vals, d_out, d_bad.get()) &&
+              cudaMemcpyAsync(h_bad.get(), d_bad.get(), 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    ok = call.finish(ok, false);
+    if (ok && *h_bad.get() != ~0ull) {   // the first out-of-range entry, reported as the host check does
+        const uint64_t k = *h_bad.get();
+        uint32_t v = 0;
+        if (cudaMemcpyAsync(&v, d_idx + k, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess)
+            cudaStreamSynchronize(g.stream);
+        index_error("query_device", k, v, S->n_bitmaps);
+        ok = false;
+    }
+    return ok ? 0 : -1;
 }
 
 roaring_bitmap_t *roaring_bitmap_flip(const roaring_bitmap_t *r1, uint64_t range_start, uint64_t range_end) {

@@ -202,10 +202,11 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
 int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint32_t *ia,
                           const uint32_t *ib, size_t npairs, uint8_t *out);
 
-/* Selections.  rb200_batch_flip, rb200_batch_add_offset, the add_many / remove_many family and the or_many / xor_many entry points work on
- * S[idx[0..n)]; idx == NULL selects every bitmap of S in order (n is then ignored).  A NULL or lazy S, and
- * with an idx, n >= 2^32 or an entry out of range, is refused before any device work; rb200_last_error()
- * names the entry point. */
+/* Selections.  rb200_batch_flip, rb200_batch_add_offset, the add_many / remove_many family, the or_many / xor_many
+ * entry points and rb200_batch_query work on S[idx[0..n)]; idx == NULL selects every bitmap of S in order (n is
+ * then ignored).  A NULL or lazy S, and with an idx, n >= 2^32 or an entry out of range, is refused before any
+ * device work; rb200_last_error() names the entry point.  rb200_batch_query_device reads its idx on the
+ * device: the kernel checks every entry, and the call fails after it with the same message. */
 
 /* result[k] = roaring_bitmap_flip(S[idx[k]], range_start, range_end) (idx == NULL: every bitmap). */
 rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t n, uint64_t range_start,
@@ -232,6 +233,23 @@ rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *i
                                          const uint64_t *d_off);
 rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
                                             const uint32_t *d_vals, const uint64_t *d_off);
+
+/* Point queries, one value per query.  Query k asks bitmap S[idx[k]] about vals[k], k < n; idx == NULL: query k
+ * asks bitmap k (n = rb200_set_count(S)).  Values in any order, repeats allowed.  out[k]:
+ *   RB200_Q_CONTAINS   1 / 0                                        as roaring_bitmap_contains, roaring.h:478
+ *   RB200_Q_RANK       the number of values <= vals[k], 0 .. 2^32   as roaring_bitmap_rank, src/roaring.c:2862
+ *   RB200_Q_GET_INDEX  the index of vals[k], or -1 when absent      as roaring_bitmap_get_index, src/roaring.c:2916
+ *   RB200_Q_SELECT     the value of rank vals[k] (0-based), or -1 when vals[k] >= the cardinality
+ *                                                                   as roaring_bitmap_select, src/roaring.c:2974
+ * The minimum is select 0, the maximum select(cardinality - 1), a range count the difference of two ranks.
+ * vals / out may be NULL only when n == 0.  0 on success, -1 on error (rb200_last_error). */
+enum { RB200_Q_CONTAINS = 0, RB200_Q_RANK = 1, RB200_Q_GET_INDEX = 2, RB200_Q_SELECT = 3 };
+int rb200_batch_query(int kind, const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                      int64_t *out);
+/* Same with idx / vals / out in device memory of the library's device (anything else is refused before the
+ * launch): read and written on the library stream, complete when the call returns. */
+int rb200_batch_query_device(int kind, const rb200_set_t *S, const uint32_t *d_idx, size_t n,
+                             const uint32_t *d_vals, int64_t *d_out);
 
 /* 64-bit bitmaps (src/roaring64.c) through their portable format: result[k] =
  * roaring64_bitmap_{and,or,xor,andnot}(a[ia[k]], b[ib[k]]) — the same container grid per
