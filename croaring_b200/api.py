@@ -552,38 +552,57 @@ def _offsets_i64(offsets, n):
     return np.ascontiguousarray(a, dtype=np.int64)
 
 
-def _device_offsets(values, offsets):
-    """Offsets of CUDA tensor values (n + 1 entries, as a CUDA or CPU tensor or an array) as a
-    contiguous tensor on the values' device, ready for the library stream."""
-    import torch
+def _value_lists(values, offsets, width):
+    """One list of values per bitmap, in any form from_values takes, as (flat values, n + 1 offsets,
+    entry point suffix): numpy uint{width} values and uint64 offsets for host values, suffix ""; for
+    a CUDA tensor, the tensor itself and its offsets as a contiguous tensor on its device, ready for
+    the library stream, suffix "_device" (the entry points that read them in place)."""
+    if getattr(values, "is_cuda", False):
+        import torch
+        dtypes = (torch.int32, torch.uint32) if width == 32 else (torch.int64, torch.uint64)
+        if values.dtype not in dtypes or values.dim() != 1 or not values.is_contiguous():
+            raise RB200Error(f"device values must be a contiguous 1-D int{width} / uint{width} CUDA tensor")
+        if offsets is None:
+            raise RB200Error("device values need offsets")
+        offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
+        if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
+            raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
+        last = int(offs[-1].item())
+        if last < 0 or last > values.numel():
+            raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
+        offs = offs.to(values.device).contiguous()
+        if offs is not offsets:   # copied here: on the stream the library reads on
+            torch.cuda.current_stream(values.device).synchronize()
+        return values, offs, "_device"
+    conv = _values_u32 if width == 32 else _values_u64
     if offsets is None:
-        raise RB200Error("device values need offsets")
-    offs = offsets if isinstance(offsets, torch.Tensor) else torch.as_tensor(np.asarray(offsets, dtype=np.int64))
-    if offs.dtype not in (torch.int64, torch.uint64) or offs.dim() != 1 or offs.numel() < 1:
-        raise RB200Error("offsets must be a 1-D int64 / uint64 tensor of n + 1 entries")
-    last = int(offs[-1].item())
-    if last < 0 or last > values.numel():
-        raise RB200Error(f"offsets end at {last}, outside the {values.numel()} values")
-    offs = offs.to(values.device).contiguous()
-    if offs is not offsets:   # copied here: on the stream the library reads on
-        torch.cuda.current_stream(values.device).synchronize()
-    return offs
+        arrays = [np.asarray(a).reshape(-1) for a in values]
+        if width == 64:   # one by one: arrays of ints past 2^63 and below it would concatenate as float64
+            arrays = [conv(a) for a in arrays]
+        offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
+        np.cumsum([a.size for a in arrays], out=offs[1:])
+        flat = conv(np.concatenate(arrays) if arrays else np.zeros(0, np.uint32))
+    else:
+        flat = conv(values)
+        offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
+        if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
+            raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
+    return flat, offs, ""
+
+
+def _ptr(a):
+    """The address of a numpy array or a torch tensor."""
+    return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
 
 
 def _update(s, fn, values, offsets, idx):
     """fn (an add_many / remove_many entry point; fn + "_device" for CUDA tensor values) on the
     selection idx of the set s, with one list of values per selected bitmap."""
     idx, ip, n = _selection(idx, len(s))
-    if getattr(values, "is_cuda", False):
-        offs = s._device_offsets(values, offsets)
-        vp, op, m = values.data_ptr(), offs.data_ptr(), offs.numel() - 1
-        fn += "_device"
-    else:
-        flat, offs = s._host_values(values, offsets)   # held until the call returns
-        vp, op, m = flat.ctypes.data, offs.ctypes.data, offs.size - 1
-    if m != n:
-        raise RB200Error(f"{m} lists of values for {n} items")
-    return getattr(lib(), fn)(s.ptr, ip, n, vp, op)
+    flat, offs, suffix = _value_lists(values, offsets, s._width)   # held until the call returns
+    if len(offs) - 1 != n:
+        raise RB200Error(f"{len(offs) - 1} lists of values for {n} items")
+    return getattr(lib(), fn + suffix)(s.ptr, ip, n, _ptr(flat), _ptr(offs))
 
 
 QUERIES = {"contains": 0, "rank": 1, "get_index": 2, "select": 3}   # RB200_Q_*
@@ -660,6 +679,7 @@ def _query_device(s, code, values, idx):
 
 class DeviceSet:
     """An ordered collection of bitmaps resident in HBM (rb200_set_t*)."""
+    _width = 32   # bits per value
 
     def __init__(self, ptr):
         if not ptr:
@@ -696,38 +716,8 @@ class DeviceSet:
         uint32 array with n + 1 offsets (the layout of to_uint32_arrays); or a CUDA torch tensor of
         int32 / uint32 values with offsets as a CUDA or CPU tensor, read in place on the library stream
         (order its writes before the call, e.g. by building it on the stream given to set_stream)."""
-        if getattr(values, "is_cuda", False):
-            return cls._from_device_values(values, offsets)
-        flat, offs = cls._host_values(values, offsets)
-        return cls(lib().rb200_set_from_uint32(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
-
-    @classmethod
-    def _from_device_values(cls, values, offsets):
-        offs = cls._device_offsets(values, offsets)
-        return cls(lib().rb200_set_from_uint32_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
-
-    @staticmethod
-    def _host_values(values, offsets):
-        """(flat uint32 values, uint64 offsets) of the host forms from_values takes."""
-        if offsets is None:
-            arrays = [np.asarray(a).reshape(-1) for a in values]
-            offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
-            np.cumsum([a.size for a in arrays], out=offs[1:])
-            flat = _values_u32(np.concatenate(arrays) if arrays else np.zeros(0, np.uint32))
-        else:
-            flat = _values_u32(values)
-            offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
-            if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
-                raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
-        return flat, offs
-
-    @staticmethod
-    def _device_offsets(values, offsets):
-        """The offsets of CUDA tensor values as a contiguous tensor on the values' device."""
-        import torch
-        if values.dtype not in (torch.int32, torch.uint32) or values.dim() != 1 or not values.is_contiguous():
-            raise RB200Error("device values must be a contiguous 1-D int32 / uint32 CUDA tensor")
-        return _device_offsets(values, offsets)
+        flat, offs, suffix = _value_lists(values, offsets, 32)
+        return cls(getattr(lib(), "rb200_set_from_uint32" + suffix)(_ptr(flat), _ptr(offs), len(offs) - 1))
 
     def free(self):
         if self.ptr:
@@ -998,6 +988,7 @@ def _serialized(fn, ptr, n):
 
 class DeviceSet64:
     """An ordered collection of 64-bit bitmaps (roaring64_bitmap_t) resident in HBM (rb200_set64_t*)."""
+    _width = 64   # bits per value
 
     def __init__(self, ptr):
         if not ptr:
@@ -1016,38 +1007,8 @@ class DeviceSet64:
         .run_optimize() for those).  values: a list of 1-D integer arrays, one per bitmap; or one flat
         array with n + 1 offsets; or a CUDA torch tensor of int64 / uint64 values (its bits read as
         uint64) with offsets as a CUDA or CPU tensor, read in place on the library stream."""
-        if getattr(values, "is_cuda", False):
-            return cls._from_device_values(values, offsets)
-        flat, offs = cls._host_values(values, offsets)
-        return cls(lib().rb200_set64_from_uint64(flat.ctypes.data, offs.ctypes.data, offs.size - 1))
-
-    @classmethod
-    def _from_device_values(cls, values, offsets):
-        offs = cls._device_offsets(values, offsets)
-        return cls(lib().rb200_set64_from_uint64_device(values.data_ptr(), offs.data_ptr(), offs.numel() - 1))
-
-    @staticmethod
-    def _host_values(values, offsets):
-        """(flat uint64 values, uint64 offsets) of the host forms from_values takes."""
-        if offsets is None:
-            arrays = [np.asarray(a).reshape(-1) for a in values]
-            offs = np.zeros(len(arrays) + 1, dtype=np.uint64)
-            np.cumsum([a.size for a in arrays], out=offs[1:])
-            flat = _values_u64(np.concatenate([_values_u64(a) for a in arrays]) if arrays else np.zeros(0, np.uint64))
-        else:
-            flat = _values_u64(values)
-            offs = np.ascontiguousarray(offsets, dtype=np.int64).astype(np.uint64)
-            if offs.ndim != 1 or offs.size < 1 or int(offs[-1]) > flat.size:
-                raise RB200Error(f"offsets must be n + 1 entries ending at most at len(values) = {flat.size}")
-        return flat, offs
-
-    @staticmethod
-    def _device_offsets(values, offsets):
-        """The offsets of CUDA tensor values as a contiguous tensor on the values' device."""
-        import torch
-        if values.dtype not in (torch.int64, torch.uint64) or values.dim() != 1 or not values.is_contiguous():
-            raise RB200Error("device values must be a contiguous 1-D int64 / uint64 CUDA tensor")
-        return _device_offsets(values, offsets)
+        flat, offs, suffix = _value_lists(values, offsets, 64)
+        return cls(getattr(lib(), "rb200_set64_from_uint64" + suffix)(_ptr(flat), _ptr(offs), len(offs) - 1))
 
     def free(self):
         if self.ptr:

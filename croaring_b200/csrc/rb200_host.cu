@@ -29,6 +29,7 @@
 #include <mutex>
 #include <numeric>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #pragma GCC visibility push(default)
@@ -1412,17 +1413,25 @@ bool check_indices(const char *what, const uint32_t *idx, size_t n, uint64_t cou
 }
 
 // The bitmaps S[idx[0..n)] an entry point works on; idx == NULL selects every bitmap of S in order.
-struct Selection {
-    const rb200_set *S;
+// Set: rb200_set, or rb200_set64 for the checks and indices alone.
+template <typename Set>
+struct SelectionOf {
+    const Set *S;
     const uint32_t *idx;
     size_t n;
     // Refuse a selection the device must never see, before any device call; `what` heads t_err.
     // n is checked before idx is read, and becomes the set's size when idx is NULL.
     bool check(const char *what) {
         if (!S) { t_err = std::string(what) + ": S is NULL"; return false; }
-        if (reject_lazy(S, what)) return false;
-        if (!idx) { n = S->n_bitmaps; return true; }
-        return check_indices(what, idx, n, S->n_bitmaps);
+        uint64_t count;
+        if constexpr (std::is_same<Set, rb200_set>::value) {
+            if (reject_lazy(S, what)) return false;
+            count = S->n_bitmaps;
+        } else {
+            count = S->n;   // a 64-bit set is never lazy
+        }
+        if (!idx) { n = count; return true; }
+        return check_indices(what, idx, n, count);
     }
     uint32_t operator[](size_t k) const { return idx ? idx[k] : (uint32_t)k; }
     bool all() const { return idx == nullptr; }
@@ -1460,6 +1469,7 @@ struct Selection {
         return cudaMemcpyAsync(d.get(), h.get(), 4 * n, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
     }
 };
+using Selection = SelectionOf<rb200_set>;
 
 // Host fields of a one-bitmap result of `containers` bitset slots (or_many, xor_many).
 void fill_single_result(rb200_set *R, uint32_t containers, uint64_t slab_used, uint8_t cow) {
@@ -2654,35 +2664,89 @@ int rb200_set_to_uint32(const rb200_set_t *S, uint32_t **vals, uint64_t **off_ou
 
 void rb200_values_free(uint32_t *vals, uint64_t *off) { rb200_serialized_free((char *)vals, off, nullptr); }
 
-// Arguments of rb200_set_from_uint32* / rb200_set64_from_uint64*: n < 2^32 bitmaps; n + 1 offsets,
-// off[0] == 0, non-decreasing.  `what` names the entry point in the message.
-static bool check_bitmap_count(size_t n, const char *what = "set_from_uint32") {
-    if (n <= 0xffffffffull) return true;
-    t_err = std::string(what) + ": " + std::to_string((uint64_t)n) + " bitmaps, at most 2^32 - 1 fit in a set";
+extern "C++" {
+// p is device (or managed) memory of the library's device
+static bool device_memory(const char *what, const char *name, const void *p) {
+    cudaPointerAttributes a = {};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        (void)cudaGetLastError();
+        a.type = cudaMemoryTypeUnregistered;
+    }
+    if ((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == g.device) return true;
+    t_err = std::string(what) + ": " + name + " is not device memory of the library's device";
     return false;
 }
-static bool check_value_offsets(const uint64_t *off, size_t n, const char *what = "set_from_uint32") {
-    if (!check_bitmap_count(n, what)) return false;
-    if (!off) { t_err = std::string(what) + ": offsets are NULL"; return false; }
-    if (off[0] != 0) {
-        t_err = std::string(what) + ": offsets must start at 0 (off[0] = " + std::to_string(off[0]) + ")";
-        return false;
+
+// One list of values per bitmap, the argument of the set builders and of the add_many / remove_many
+// updates: bitmap k < n takes vals[off[k] .. off[k + 1]).  vals and off are both host memory, or both
+// device memory of the library's device (device: the *_device entry points read the values in place).
+template <typename V>
+struct ValueLists {
+    const V *vals;
+    const uint64_t *off;
+    size_t n;
+    bool device;
+    const uint64_t *h_off = nullptr;   // after check(): the checked offsets on the host; null: presorted()
+    uint64_t N = 0;                    // after check(): the number of values
+    PinBlock<uint64_t> read_back;      // device offsets as check() read them
+
+    ValueLists(const V *vals_, const uint64_t *off_, size_t n_, bool device_)
+        : vals(vals_), off(off_), n(n_), device(device_) {}
+    // Device offsets of N values in segments that are sorted already (the buckets of the 64-bit
+    // builder): never checked, and never sorted again.
+    static ValueLists presorted(const V *d_vals, const uint64_t *d_off, size_t n, uint64_t N) {
+        ValueLists in(d_vals, d_off, n, true);
+        in.N = N;
+        return in;
     }
-    for (size_t i = 0; i < n; i++)
-        if (off[i + 1] < off[i]) {
-            t_err = std::string(what) + ": offsets decrease at bitmap " + std::to_string((uint64_t)i) + " (off[" +
-                    std::to_string((uint64_t)i) + "] = " + std::to_string(off[i]) + ", off[" +
-                    std::to_string((uint64_t)i + 1) + "] = " + std::to_string(off[i + 1]) + ")";
+
+    // Refuse lists no kernel may read, then ready the library's device; host lists are refused before
+    // any CUDA call.  n < 2^32; off not NULL, off[0] == 0, non-decreasing; vals not NULL unless there
+    // are no values.  Device offsets are read back and checked here, and the builder uploads that
+    // checked copy.  `what` names the entry point in t_err; `name`, if given, names it in the messages
+    // about n and the offsets' values instead (set_from_uint32_device reports those as set_from_uint32).
+    bool check(const char *what, const char *name = nullptr) {
+        const std::string head = std::string(name ? name : what) + ": ";
+        if (n > 0xffffffffull) {
+            t_err = head + std::to_string((uint64_t)n) + " bitmaps, at most 2^32 - 1 fit in a set";
             return false;
         }
-    return true;
-}
+        if (!off) { t_err = std::string(what) + ": offsets are NULL"; return false; }
+        h_off = off;
+        if (device) {
+            // a host pointer never reaches the read back or a kernel
+            if (!ctx_init() || (vals && !device_memory(what, "vals", vals)) || !device_memory(what, "off", off) ||
+                !read_back.reset(n + 1))
+                return false;
+            if (cudaMemcpyAsync(read_back.get(), off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
+                cudaStreamSynchronize(g.stream) != cudaSuccess) {
+                (void)cudaGetLastError();
+                t_err = std::string(what) + ": offsets are not readable device memory of the library's device";
+                return false;
+            }
+            h_off = read_back.get();
+        }
+        if (h_off[0] != 0) {
+            t_err = head + "offsets must start at 0 (off[0] = " + std::to_string(h_off[0]) + ")";
+            return false;
+        }
+        for (size_t i = 0; i < n; i++)
+            if (h_off[i + 1] < h_off[i]) {
+                t_err = head + "offsets decrease at bitmap " + std::to_string((uint64_t)i) + " (off[" +
+                        std::to_string((uint64_t)i) + "] = " + std::to_string(h_off[i]) + ", off[" +
+                        std::to_string((uint64_t)i + 1) + "] = " + std::to_string(h_off[i + 1]) + ")";
+                return false;
+            }
+        N = h_off[n];
+        if (!vals && N) { t_err = std::string(what) + ": values are NULL"; return false; }
+        return device || ctx_init();
+    }
+};
 
 // Segmented sort of src (n segments: h_off on the host, d_off on the device) into `sorted`, a new device
 // buffer of h_off[n] values; the input stays as it was.  cub sorts fewer than 2^31 values per call, so
 // the segments go in chunks of that size; a segment too large for one call is sorted already (the
 // measure pass refuses it otherwise) and is copied.  temp: the caller's scratch, grown here.
-extern "C++" {
 template <typename T>
 static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d_off, size_t n, DevBlock<T> &sorted,
                           DevBlock<uint8_t> &temp) {
@@ -2734,6 +2798,7 @@ static bool sort_segments(const T *src, const uint64_t *h_off, const uint64_t *d
 template <typename V>
 struct BuildInput {
     const char *what;         // the builder, in messages
+    const ValueLists<V> &lists;   // checked by the entry point, or presorted
     size_t n;
     uint64_t N, ntiles;
     const uint64_t *h_off;    // checked host offsets; null: presorted device segments
@@ -2745,24 +2810,25 @@ struct BuildInput {
     DevBlock<uint8_t> temp;   // cub scratch, grown by grow_temp()
     PinBlock<uint64_t> meta;  // [count | unsorted flags | two words of the caller's]
 
-    BuildInput(const char *what_, const uint64_t *h_off_, size_t n_, uint64_t N_)
-        : what(what_), n(n_), N(N_), ntiles(build_tile_count(N_)), h_off(h_off_) {}
+    BuildInput(const char *what_, const ValueLists<V> &lists_)
+        : what(what_), lists(lists_), n(lists_.n), N(lists_.N), ntiles(build_tile_count(lists_.N)), h_off(lists_.h_off) {}
     bool grow_temp(size_t b) { return b <= temp.bytes() || temp.reset(b); }
 
-    // Offsets (h_off, or d_off_in already on the device) and values (h_vals from the host, or d_in
-    // on the device) in place; false: t_err says why.
-    bool load(const V *h_vals, const V *d_in, const uint64_t *d_off_in) {
+    // Offsets (the checked host copy uploaded, presorted ones in place) and values (host ones staged,
+    // device ones in place) on the device; false: t_err says why.
+    bool load() {
+        const bool stage_vals = !lists.device;
         if (ntiles >= (1ull << 31) - 1) { t_err = std::string(what) + ": too many values for one call"; return false; }
-        if (!d_off_in && !d_off.reset(n + 1)) return false;
-        if (h_vals && !vals.reset(N)) return false;
+        if (h_off && !d_off.reset(n + 1)) return false;
+        if (stage_vals && !vals.reset(N)) return false;
         if (!tcnt.reset(ntiles + 1) || !tbase.reset(ntiles + 1) || !flag.reset(1) || !meta.reset(4)) return false;
-        offs = d_off_in ? d_off_in : d_off.get();
-        src = h_vals ? vals.get() : d_in;
-        if (!d_off_in && cudaMemcpyAsync(d_off.get(), h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
+        offs = h_off ? d_off.get() : lists.off;
+        src = stage_vals ? vals.get() : lists.vals;
+        if (h_off && cudaMemcpyAsync(d_off.get(), h_off, 8 * (n + 1), cudaMemcpyHostToDevice, g.stream) != cudaSuccess)
             return false;
-        if (h_vals && N) {
+        if (stage_vals && N) {
             H2DStager stage((uint8_t *)vals.get());
-            const bool ok = stage.ok && stage.put(h_vals, sizeof(V) * N) && stage.flush();
+            const bool ok = stage.ok && stage.put(lists.vals, sizeof(V) * N) && stage.flush();
             return cudaStreamSynchronize(g.stream) == cudaSuccess && ok;   // the chunks are recycled after this
         }
         return true;
@@ -2811,19 +2877,17 @@ struct BuildInput {
 };
 }  // extern "C++"
 
-// roaring_bitmap_of_ptr of every bitmap (rb200_build.cu).  Values come from the host (h_vals, staged
-// through pinned chunks) or from the device (d_in, read in place).  Offsets: h_off, checked host
-// offsets; or d_off_in, device offsets of N values in segments that are sorted already (the buckets of
-// the 64-bit builder), which are never sorted again.
-static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in, const uint64_t *h_off, size_t n,
-                                   const uint64_t *d_off_in = nullptr, uint64_t N_in = 0) {
-    BuildInput<uint32_t> in("set_from_uint32", h_off, n, h_off ? h_off[n] : N_in);
+// roaring_bitmap_of_ptr of every bitmap (rb200_build.cu) of checked or presorted value lists.  Host
+// values are staged through pinned chunks, device values read in place.
+static rb200_set *from_uint32_impl(const ValueLists<uint32_t> &lists) {
+    BuildInput<uint32_t> in("set_from_uint32", lists);
+    const size_t n = lists.n;
     const uint64_t N = in.N;
     SetPtr s;
     DevBlock<uint64_t> d_cpos, d_slot;
     SyncCall call("set_from_uint32");
     uint64_t nc = 0;
-    bool ok = in.load(h_vals, d_in, d_off_in) && in.measure_sorted([&](const uint32_t *src) {
+    bool ok = in.load() && in.measure_sorted([&](const uint32_t *src) {
         launch_build_measure(src, in.offs, (uint32_t)n, N, in.tcnt.get(), in.flag.get(), g.stream);
     }, nc);
     if (ok && nc > 0xffffffffull) { t_err = "set_from_uint32: more than 2^32 - 1 containers"; ok = false; }
@@ -2867,37 +2931,14 @@ static rb200_set *from_uint32_impl(const uint32_t *h_vals, const uint32_t *d_in,
 
 rb200_set_t *rb200_set_from_uint32(const uint32_t *vals, const uint64_t *off, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!check_value_offsets(off, n)) return nullptr;   // before any CUDA call
-    if (!vals && off[n]) { t_err = "set_from_uint32: values are NULL"; return nullptr; }
-    if (!ctx_init()) return nullptr;
-    static const uint32_t none = 0;
-    return from_uint32_impl(vals ? vals : &none, nullptr, off, n);
-}
-
-// The offsets of a *_device builder, read back into h_off and checked on the host before any kernel
-// reads values through them.  `check` names the builder in the checks of the offsets, `entry` the
-// entry point in the others.
-static bool device_offsets(const uint64_t *d_off, const void *d_vals, size_t n, const char *check, const char *entry,
-                           PinBlock<uint64_t> &h_off) {
-    if (!check_bitmap_count(n, check)) return false;
-    if (!d_off) { t_err = std::string(entry) + ": offsets are NULL"; return false; }
-    if (!ctx_init() || !h_off.reset(n + 1)) return false;
-    if (cudaMemcpyAsync(h_off.get(), d_off, 8 * (n + 1), cudaMemcpyDeviceToHost, g.stream) != cudaSuccess ||
-        cudaStreamSynchronize(g.stream) != cudaSuccess) {
-        (void)cudaGetLastError();
-        t_err = std::string(entry) + ": offsets are not readable device memory of the library's device";
-        return false;
-    }
-    if (!check_value_offsets(h_off.get(), n, check)) return false;
-    if (!d_vals && h_off.get()[n]) { t_err = std::string(entry) + ": values are NULL"; return false; }
-    return true;
+    ValueLists<uint32_t> lists(vals, off, n, false);
+    return lists.check("set_from_uint32") ? from_uint32_impl(lists) : nullptr;
 }
 
 rb200_set_t *rb200_set_from_uint32_device(const uint32_t *d_vals, const uint64_t *d_off, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    PinBlock<uint64_t> h_off;
-    if (!device_offsets(d_off, d_vals, n, "set_from_uint32", "set_from_uint32_device", h_off)) return nullptr;
-    return from_uint32_impl(nullptr, d_vals, h_off.get(), n);
+    ValueLists<uint32_t> lists(d_vals, d_off, n, true);
+    return lists.check("set_from_uint32_device", "set_from_uint32") ? from_uint32_impl(lists) : nullptr;
 }
 
 // Device-side portable serialization of every bitmap of a set + one D2H copy.
@@ -3392,62 +3433,6 @@ rb200_set_t *rb200_batch_flip(const rb200_set_t *S, const uint32_t *idx, size_t 
     if (R && noop) for (size_t p = 0; p < sel.n; p++) R->h_flags[p] = sel.cow(p);
     return R;
 }
-// ---- updates: roaring_bitmap_add_many / remove_many (src/roaring.c:134, 696) ----------------------
-// result[k] = S[idx[k]] after adding (removing) the values vals[off[k] .. off[k+1]).  The values become
-// a bitmap V[k] with roaring_bitmap_of_ptr's builder (from_uint32_impl), and the update is the batch op
-// (S[idx[k]], V[k]) under RULES_KEEP_RUN: OR to add, ANDNOT to remove (decide_type_keep_run).  The
-// containers the values do not touch stay shared with S.  An added key that S lacks takes V's
-// container, which the result holds like any operand's (rb200_set::held), so V is freed on return.
-namespace {
-rb200_set *update_op(int op, const Selection &sel, const rb200_set *V) {
-    if (!V) return nullptr;
-    std::vector<uint32_t> ia(sel.n), ib(sel.n);
-    for (size_t k = 0; k < sel.n; k++) {
-        ia[k] = sel[k];
-        ib[k] = (uint32_t)k;
-    }
-    return batch_op_impl(op, sel.S, V, ia.data(), ib.data(), sel.n, RULES_KEEP_RUN);
-}
-rb200_set *update_host(int op, const char *what, const rb200_set *S, const uint32_t *idx, size_t n,
-                       const uint32_t *vals, const uint64_t *off) {
-    Selection sel{S, idx, n};
-    if (!sel.check(what) || !check_value_offsets(off, sel.n, what)) return nullptr;   // before any CUDA call
-    if (!vals && off[sel.n]) { t_err = std::string(what) + ": values are NULL"; return nullptr; }
-    if (!ctx_init()) return nullptr;
-    static const uint32_t none = 0;
-    const SetPtr V(from_uint32_impl(vals ? vals : &none, nullptr, off, sel.n));
-    return update_op(op, sel, V.get());
-}
-rb200_set *update_device(int op, const char *what, const rb200_set *S, const uint32_t *idx, size_t n,
-                         const uint32_t *d_vals, const uint64_t *d_off) {
-    Selection sel{S, idx, n};
-    PinBlock<uint64_t> h_off;
-    if (!sel.check(what) || !device_offsets(d_off, d_vals, sel.n, what, what, h_off)) return nullptr;
-    const SetPtr V(from_uint32_impl(nullptr, d_vals, h_off.get(), sel.n));
-    return update_op(op, sel, V.get());
-}
-}  // namespace
-rb200_set_t *rb200_batch_add_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
-                                  const uint64_t *off) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update_host(OP_OR, "add_many", S, idx, n, vals, off);
-}
-rb200_set_t *rb200_batch_remove_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
-                                     const uint64_t *off) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update_host(OP_ANDNOT, "remove_many", S, idx, n, vals, off);
-}
-rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *d_vals,
-                                         const uint64_t *d_off) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update_device(OP_OR, "add_many_device", S, idx, n, d_vals, d_off);
-}
-rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
-                                            const uint32_t *d_vals, const uint64_t *d_off) {
-    std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update_device(OP_ANDNOT, "remove_many_device", S, idx, n, d_vals, d_off);
-}
-
 // ---- point queries: roaring_bitmap_contains / rank / get_index / select (roaring.h:478, src/roaring.c:2862,
 // 2916, 2974) ---------------------------------------------------------------------------------------
 // out[k] = the answer of bitmap S[idx[k]] about vals[k], a warp per query (rb200_query.cu).  rank, get_index
@@ -3463,17 +3448,6 @@ bool query_args(const char *what, int kind, size_t n, const void *vals, const vo
     if (n && !vals) { t_err = std::string(what) + ": vals are NULL"; return false; }
     if (n && !out) { t_err = std::string(what) + ": out is NULL"; return false; }
     return true;
-}
-// p is device (or managed) memory of the library's device
-bool device_memory(const char *what, const char *name, const void *p) {
-    cudaPointerAttributes a = {};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        (void)cudaGetLastError();
-        a.type = cudaMemoryTypeUnregistered;
-    }
-    if ((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == g.device) return true;
-    t_err = std::string(what) + ": " + name + " is not device memory of the library's device";
-    return false;
 }
 // The set's c_cum on the library stream, unless it is there already.  A set without containers has
 // none: every bitmap is empty and no query reads it.
@@ -3834,10 +3808,11 @@ int serialize64_impl(const rb200_set64 *s, char **buf, uint64_t **off_out, uint6
     return out.hand_out(buf, off_out, len_out);
 }
 
-// roaring64_bitmap_of_ptr of every bitmap (rb200_build.cu): values from the host (staged through
-// pinned chunks) or the device (read in place); h_off: checked host offsets.
-rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, const uint64_t *h_off, size_t n) {
-    BuildInput<uint64_t> in("set64_from_uint64", h_off, n, h_off[n]);
+// roaring64_bitmap_of_ptr of every bitmap (rb200_build.cu) of checked value lists: host values staged
+// through pinned chunks, device values read in place.
+rb200_set64 *from_uint64_impl(const ValueLists<uint64_t> &lists) {
+    BuildInput<uint64_t> in("set64_from_uint64", lists);
+    const size_t n = lists.n;
     const uint64_t N = in.N;
     Set64Ptr R;
     DevBlock<uint32_t> d_lo;
@@ -3845,7 +3820,7 @@ rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, cons
     SyncCall call;
     uint64_t nbk = 0;
     // bucket starts per tile, scanned: the total is the bucket count if the values are sorted
-    bool ok = in.load(h_vals, d_in, nullptr) && in.measure_sorted([&](const uint64_t *src) {
+    bool ok = in.load() && in.measure_sorted([&](const uint64_t *src) {
         launch_build64_measure(src, in.offs, (uint32_t)n, N, in.tcnt.get(), in.flag.get(), g.stream);
     }, nbk);
     if (ok && nbk >= 0xffffffffull) { t_err = "set64_from_uint64: more than 2^32 - 2 buckets"; ok = false; }
@@ -3864,7 +3839,7 @@ rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, cons
             launch_build_bitmaps(in.offs, (uint32_t)n, d_bpos.get(), nbk, d_dir, d_dir + n, g.stream);
             in.vals.reset();     // stream-ordered reuse: the inner build may take their memory
             in.sorted.reset();
-            R->inner.reset(from_uint32_impl(nullptr, d_lo.get(), nullptr, nbk + 1, d_bpos.get(), N));
+            R->inner.reset(from_uint32_impl(ValueLists<uint32_t>::presorted(d_lo.get(), d_bpos.get(), nbk + 1, N)));
             ok = R->inner && cudaMemcpyAsync(R->h_dir.get(), d_dir, R->dir_bytes, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
             ok = call.finish(ok, false);
             R->dir_on_device = true;
@@ -3875,37 +3850,6 @@ rb200_set64 *from_uint64_impl(const uint64_t *h_vals, const uint64_t *d_in, cons
         return nullptr;
     }
     return R.release();
-}
-
-// roaring64_bitmap_add_many / remove_many (roaring64.c:606, 950) of S[idx[k]] with the values
-// vals[off[k] .. off[k+1]): the same container_add / container_remove per 48-bit key as the 32-bit
-// update, so the inner sets take the same batch op under RULES_KEEP_RUN (update_op).  plan64 keeps the
-// buckets only V holds for OR and drops them for ANDNOT; a bucket a removal empties stays an empty
-// inner bitmap, which is never planned, counted or serialized.  device: vals / off are in device memory.
-rb200_set64 *update64(int op, const char *what, const rb200_set64 *S, const uint32_t *idx, size_t n,
-                      const uint64_t *vals, const uint64_t *off, bool device) {
-    if (!S) { t_err = std::string(what) + ": S is NULL"; return nullptr; }
-    if (!idx) n = S->n;
-    else if (!check_indices(what, idx, n, S->n)) return nullptr;
-    PinBlock<uint64_t> d_h_off;
-    const uint64_t *h_off = off;
-    if (!device) {
-        if (!check_value_offsets(off, n, what)) return nullptr;   // before any CUDA call
-        if (!vals && off[n]) { t_err = std::string(what) + ": values are NULL"; return nullptr; }
-        if (!ctx_init()) return nullptr;
-    } else {
-        if (!device_offsets(off, vals, n, what, what, d_h_off)) return nullptr;
-        h_off = d_h_off.get();
-    }
-    static const uint64_t none = 0;
-    const Set64Ptr V(device ? from_uint64_impl(nullptr, vals, h_off, n) : from_uint64_impl(vals ? vals : &none, nullptr, h_off, n));
-    if (!V) return nullptr;
-    std::vector<uint32_t> ia(n), ib(n);
-    for (size_t k = 0; k < n; k++) {
-        ia[k] = idx ? idx[k] : (uint32_t)k;
-        ib[k] = (uint32_t)k;
-    }
-    return batch_op64_impl(op, S, V.get(), ia.data(), ib.data(), n, RULES_KEEP_RUN);
 }
 
 // a[] then b[] as ONE resident set (one H2D); ib2 = ib shifted past a[]
@@ -3924,6 +3868,38 @@ rb200_set64 *r64_operands(const char *const *a, const size_t *alen, size_t na, c
     lens.insert(lens.end(), blen, blen + nb);
     return set64_upload_impl(ptrs.data(), lens.data(), ptrs.size());
 }
+
+// ---- updates: roaring_bitmap_add_many / remove_many (src/roaring.c:134, 696) and roaring64_bitmap_add_many /
+// remove_many (roaring64.c:606, 950) ----------------------------------------------------------------
+// result[k] = S[idx[k]] after adding (removing) the values vals[off[k] .. off[k+1]).  The values become
+// a set V with roaring_bitmap_of_ptr's builder (from_uint32_impl, from_uint64_impl), and the update is
+// the batch op (S[idx[k]], V[k]) under RULES_KEEP_RUN: OR to add, ANDNOT to remove
+// (decide_type_keep_run).  The containers the values do not touch stay shared with S.  An added key
+// that S lacks takes V's container, which the result holds like any operand's (rb200_set::held), so V
+// is freed on return.  A 64-bit update is the same container_add / container_remove per 48-bit key, so
+// the inner sets take the same batch op; plan64 keeps the buckets only V holds for OR and drops them
+// for ANDNOT, and a bucket a removal empties stays an empty inner bitmap, which is never planned,
+// counted or serialized.  device: vals / off are in device memory.
+extern "C++" template <typename Set, typename V>
+Set *update(int op, const char *what, const Set *S, const uint32_t *idx, size_t n, const V *vals,
+            const uint64_t *off, bool device) {
+    SelectionOf<Set> sel{S, idx, n};
+    if (!sel.check(what)) return nullptr;
+    ValueLists<V> lists(vals, off, sel.n, device);
+    if (!lists.check(what)) return nullptr;
+    std::vector<uint32_t> ia(sel.n), ib(sel.n);
+    for (size_t k = 0; k < sel.n; k++) {
+        ia[k] = sel[k];
+        ib[k] = (uint32_t)k;
+    }
+    if constexpr (std::is_same<Set, rb200_set>::value) {
+        const SetPtr W(from_uint32_impl(lists));
+        return W ? batch_op_impl(op, S, W.get(), ia.data(), ib.data(), sel.n, RULES_KEEP_RUN) : nullptr;
+    } else {
+        const Set64Ptr W(from_uint64_impl(lists));
+        return W ? batch_op64_impl(op, S, W.get(), ia.data(), ib.data(), sel.n, RULES_KEEP_RUN) : nullptr;
+    }
+}
 }  // namespace
 
 rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size_t *lens, size_t n) {
@@ -3932,17 +3908,13 @@ rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size
 }
 rb200_set64_t *rb200_set64_from_uint64(const uint64_t *vals, const uint64_t *off, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    if (!check_value_offsets(off, n, "set64_from_uint64")) return nullptr;   // before any CUDA call
-    if (!vals && off[n]) { t_err = "set64_from_uint64: values are NULL"; return nullptr; }
-    if (!ctx_init()) return nullptr;
-    static const uint64_t none = 0;
-    return from_uint64_impl(vals ? vals : &none, nullptr, off, n);
+    ValueLists<uint64_t> lists(vals, off, n, false);
+    return lists.check("set64_from_uint64") ? from_uint64_impl(lists) : nullptr;
 }
 rb200_set64_t *rb200_set64_from_uint64_device(const uint64_t *d_vals, const uint64_t *d_off, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    PinBlock<uint64_t> h_off;
-    if (!device_offsets(d_off, d_vals, n, "set64_from_uint64_device", "set64_from_uint64_device", h_off)) return nullptr;
-    return from_uint64_impl(nullptr, d_vals, h_off.get(), n);
+    ValueLists<uint64_t> lists(d_vals, d_off, n, true);
+    return lists.check("set64_from_uint64_device") ? from_uint64_impl(lists) : nullptr;
 }
 void rb200_set64_free(rb200_set64_t *s) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
@@ -3971,25 +3943,45 @@ int rb200_set64_batch_and_cardinality(const rb200_set64_t *A, const rb200_set64_
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return and_cardinality64_impl(A, B, ia, ib, npairs, out);
 }
+rb200_set_t *rb200_batch_add_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                  const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update(OP_OR, "add_many", S, idx, n, vals, off, false);
+}
+rb200_set_t *rb200_batch_remove_many(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *vals,
+                                     const uint64_t *off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update(OP_ANDNOT, "remove_many", S, idx, n, vals, off, false);
+}
+rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *d_vals,
+                                         const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update(OP_OR, "add_many_device", S, idx, n, d_vals, d_off, true);
+}
+rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
+                                            const uint32_t *d_vals, const uint64_t *d_off) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return update(OP_ANDNOT, "remove_many_device", S, idx, n, d_vals, d_off, true);
+}
 rb200_set64_t *rb200_set64_batch_add_many(const rb200_set64_t *S, const uint32_t *idx, size_t n, const uint64_t *vals,
                                           const uint64_t *off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update64(OP_OR, "set64_add_many", S, idx, n, vals, off, false);
+    return update(OP_OR, "set64_add_many", S, idx, n, vals, off, false);
 }
 rb200_set64_t *rb200_set64_batch_remove_many(const rb200_set64_t *S, const uint32_t *idx, size_t n,
                                              const uint64_t *vals, const uint64_t *off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update64(OP_ANDNOT, "set64_remove_many", S, idx, n, vals, off, false);
+    return update(OP_ANDNOT, "set64_remove_many", S, idx, n, vals, off, false);
 }
 rb200_set64_t *rb200_set64_batch_add_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
                                                  const uint64_t *d_vals, const uint64_t *d_off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update64(OP_OR, "set64_add_many_device", S, idx, n, d_vals, d_off, true);
+    return update(OP_OR, "set64_add_many_device", S, idx, n, d_vals, d_off, true);
 }
 rb200_set64_t *rb200_set64_batch_remove_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
                                                     const uint64_t *d_vals, const uint64_t *d_off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
-    return update64(OP_ANDNOT, "set64_remove_many_device", S, idx, n, d_vals, d_off, true);
+    return update(OP_ANDNOT, "set64_remove_many_device", S, idx, n, d_vals, d_off, true);
 }
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);

@@ -68,7 +68,7 @@ def _cases(rb, R, blobs, S, lazy, S64):
          "malformed portable bitmap at index 2"),
         ("64-bit bucket contents", lambda: rb.DeviceSet64.from_serialized([_bad_bucket_contents()]),
          "invalid container contents"),
-        ("set_from_uint32_device", lambda: rb.DeviceSet._from_device_values(vals, offs),
+        ("set_from_uint32_device", lambda: rb.DeviceSet.from_values(vals, offs),
          "set_from_uint32: offsets decrease at bitmap 1"),
     ]
 

@@ -178,3 +178,28 @@ def test_device_input_matches_host_input(rb, R):
         assert S2.serialize_all() == host
     finally:
         rb.set_stream(None)
+
+
+@gpu
+def test_host_addresses_refused_as_device_input(rb):
+    """The _device entry points read device memory of the library's device only: a host address as
+    the values or as the offsets is refused before anything reads through it, and takes no memory."""
+    import torch
+    L = rb.api.lib()
+    d_vals = torch.arange(10, dtype=torch.int32, device="cuda")
+    d_off = torch.tensor([0, 4, 10], dtype=torch.int64, device="cuda")
+    h_vals = np.arange(10, dtype=np.uint32)
+    h_off = np.array([0, 4, 10], dtype=np.uint64)
+    S = rb.DeviceSet.from_values([[1, 2], [3]])
+    torch.cuda.synchronize()
+    calls = {"set_from_uint32_device": lambda v, o: L.rb200_set_from_uint32_device(v, o, 2),
+             "add_many_device": lambda v, o: L.rb200_batch_add_many_device(S.ptr, None, 2, v, o)}
+    for entry, call in calls.items():
+        for name, v, o in (("vals", h_vals.ctypes.data, d_off.data_ptr()), ("off", d_vals.data_ptr(), h_off.ctypes.data)):
+            rb.synchronize()
+            before = L.rb200_device_bytes_in_use()
+            assert not call(v, o)
+            assert rb.last_error() == f"{entry}: {name} is not device memory of the library's device"
+            rb.synchronize()
+            assert L.rb200_device_bytes_in_use() == before, (entry, name)
+    S.free()

@@ -143,7 +143,7 @@ class _Stub:
     """A stand-in set for the mirror's argument checks, which run before any library call."""
     def __init__(self, cls, n):
         self.ptr, self._n, self._cls = None, n, cls
-        self._host_values = cls._host_values
+        self._width = cls._width
 
     def __len__(self):
         return self._n
