@@ -91,6 +91,8 @@ def lib():
     sig("rb200_set_op_stats", C.c_int, _P, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64))
     sig("rb200_batch_flip", _P, _P, _P, C.c_size_t, C.c_uint64, C.c_uint64)
     sig("rb200_batch_add_offset", _P, _P, _P, C.c_size_t, _P)
+    sig("rb200_batch_add_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
+    sig("rb200_batch_remove_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
     for name in ("rb200_batch_add_many", "rb200_batch_remove_many", "rb200_set64_batch_add_many",
                  "rb200_set64_batch_remove_many"):
         sig(name, _P, _P, _P, C.c_size_t, _P, _P)
@@ -165,6 +167,8 @@ def lib():
     sig("rb200_set64_cardinalities", C.c_int, _P, _P)
     sig("rb200_set64_batch_op", _P, C.c_int, _P, _P, _P, _P, C.c_size_t)
     sig("rb200_set64_batch_and_cardinality", C.c_int, _P, _P, _P, _P, C.c_size_t, _P)
+    sig("rb200_set64_batch_add_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
+    sig("rb200_set64_batch_remove_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
     sig("rb200_set64_run_optimize", _P, _P, C.c_int)
     sig("rb200_set64_serialize", C.c_int, _P, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)),
         C.POINTER(C.POINTER(C.c_uint64)))
@@ -552,6 +556,55 @@ def _offsets_i64(offsets, n):
     return np.ascontiguousarray(a, dtype=np.int64)
 
 
+def _range_ends(x, n, top, what):
+    """One end of add_range / remove_range's half-open ranges as n Python ints in [0, top]: a scalar is
+    broadcast to every item, a 1-D integer sequence gives one per item."""
+    if np.ndim(x) == 0:
+        vals = [x] * n
+    else:
+        # (a list of Python ints is kept as it is: numpy would read ints past 2^63 next to others as floats)
+        a = x if isinstance(x, np.ndarray) else np.asarray(x, dtype=object)
+        if a.ndim != 1 or (a.size and a.dtype.kind not in "iuO"):
+            raise RB200Error(f"{what} must be an integer or a 1-D integer sequence, got {a.dtype} with shape {a.shape}")
+        vals = a.tolist()
+        if len(vals) != n:
+            raise RB200Error(f"{what} has {len(vals)} entries for {n} items")
+    if not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in vals):
+        raise RB200Error(f"{what} must be integers")
+    vals = [int(v) for v in vals]
+    if any(not 0 <= v <= top for v in vals):
+        raise RB200Error(f"{what} must lie in [0, {top}]")
+    return vals
+
+
+def _closed_ranges(start, end, n, width):
+    """The half-open [start, end) of every item as the closed (min, max) arrays the C ABI takes, converted
+    as the reference's inline wrappers convert them (a no-op item gets min > max):
+      32-bit, roaring_bitmap_add_range / remove_range (roaring.h:433-461): a no-op when end <= start or
+        start > 2^32, else [uint32(start), uint32(end - 1)], both truncated to 32 bits;
+      64-bit, roaring64_bitmap_add_range / remove_range (roaring64.c:643-649): a no-op when start >= end,
+        else [start, end - 1]; end may be 2^64."""
+    top = (1 << 64) - 1
+    s = _range_ends(start, n, top, "start")
+    e = _range_ends(end, n, top if width == 32 else top + 1, "end")
+    dt = np.uint32 if width == 32 else np.uint64
+    mins, maxs = np.ones(n, dtype=dt), np.zeros(n, dtype=dt)
+    for k, (a, b) in enumerate(zip(s, e)):
+        if b <= a or (width == 32 and a > 1 << 32):
+            continue
+        mask = (1 << width) - 1
+        mins[k], maxs[k] = a & mask, (b - 1) & mask
+    return mins, maxs
+
+
+def _range_update(s, fn, start, end, idx):
+    """fn (an add_range_closed / remove_range_closed entry point) on the selection idx of the set s, with
+    the half-open [start, end) of every item."""
+    idx, ip, n = _selection(idx, len(s))
+    mins, maxs = _closed_ranges(start, end, n, s._width)   # held until the call returns
+    return getattr(lib(), fn)(s.ptr, ip, n, mins.ctypes.data, maxs.ctypes.data)
+
+
 def _value_lists(values, offsets, width):
     """One list of values per bitmap, in any form from_values takes, as (flat values, n + 1 offsets,
     entry point suffix): numpy uint{width} values and uint64 offsets for host values, suffix ""; for
@@ -797,6 +850,16 @@ class DeviceSet:
     def remove_many(self, values, offsets=None, idx=None):
         """roaring_bitmap_remove_many of every (or the selected) bitmap, as add_many."""
         return DeviceSet(_update(self, "rb200_batch_remove_many", values, offsets, idx))
+
+    def add_range(self, start, end, idx=None):
+        """roaring_bitmap_add_range of every (or the selected) bitmap: result[k] = self[idx[k]] with the values
+        of [start[k], end[k]) added.  start / end: one integer for every item, or one per item, converted as
+        the reference's inline wrapper converts them (see _closed_ranges)."""
+        return DeviceSet(_range_update(self, "rb200_batch_add_range_closed", start, end, idx))
+
+    def remove_range(self, start, end, idx=None):
+        """roaring_bitmap_remove_range of every (or the selected) bitmap, as add_range."""
+        return DeviceSet(_range_update(self, "rb200_batch_remove_range_closed", start, end, idx))
 
     # -- point queries.  values[k] is asked of bitmap idx[k]: idx None asks bitmap k (one value per bitmap),
     # an array gives one bitmap per value, a scalar asks every value of one bitmap.  Host values (arrays,
@@ -1054,6 +1117,15 @@ class DeviceSet64:
     def remove_many(self, values, offsets=None, idx=None):
         """roaring64_bitmap_remove_many of every (or the selected) bitmap, as add_many."""
         return DeviceSet64(_update(self, "rb200_set64_batch_remove_many", values, offsets, idx))
+
+    def add_range(self, start, end, idx=None):
+        """roaring64_bitmap_add_range of every (or the selected) bitmap, as DeviceSet.add_range; end may be
+        2^64."""
+        return DeviceSet64(_range_update(self, "rb200_set64_batch_add_range_closed", start, end, idx))
+
+    def remove_range(self, start, end, idx=None):
+        """roaring64_bitmap_remove_range of every (or the selected) bitmap, as add_range."""
+        return DeviceSet64(_range_update(self, "rb200_set64_batch_remove_range_closed", start, end, idx))
 
     def run_optimize(self, mode=1):
         """mode 1: roaring64_bitmap_run_optimize of every bitmap; mode 0: the run containers removed."""

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libroaring_b200.so")
 SOURCES = ["rb200_kernels.cu", "rb200_compute.cu", "rb200_many.cu", "rb200_many2.cu", "rb200_convert.cu", "rb200_build.cu", "rb200_host.cu", "rb200_shard.cu",
-           "rb200_fused.cu", "rb200_offset.cu", "rb200_query.cu"]
+           "rb200_fused.cu", "rb200_offset.cu", "rb200_query.cu", "rb200_range.cu"]
 HEADERS = ["rb200_common.h", "rb200_device.cuh", "rb200_cells.cuh", "rb200_internal.h", "rb200_portable.h",
            os.path.join("..", "..", "include", "roaring_b200.h")]
 

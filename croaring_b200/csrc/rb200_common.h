@@ -438,6 +438,17 @@ void launch_offset_plan(const SetView &S, const uint32_t *idx, const int64_t *of
 void launch_offset_cells(const SetView &S, Items it, const uint4 *cell, uint64_t W, uint64_t bias, uint8_t *slab,
                          OpStats *st, cudaStream_t s);
 
+// roaring_bitmap_add_range_closed / remove_range_closed over a batch (rb200_range.cu): item p is bitmap
+// idx[p] of S with [mins[p], maxs[p]] added (add) or removed; its item slots start at item_off[p].
+// cell: two uint4 per item, its boundary keys for the cells kernel.  slab: the result's own slab, where
+// the plan writes the full runs and the new keys' containers.  The result directory is then built by
+// launch_finalize_pairs(S, S, ...).
+void launch_range_plan(const SetView &S, const uint32_t *idx, const uint32_t *mins, const uint32_t *maxs,
+                       const uint64_t *item_off, uint32_t n, bool add, const PassShare &sh, Items it, uint4 *cell,
+                       uint8_t *slab, uint64_t slab_cap, OpStats *st, cudaStream_t s);
+void launch_range_cells(const SetView &S, Items it, const uint4 *cell, uint32_t n, bool add, uint64_t bias,
+                        uint8_t *slab, OpStats *st, cudaStream_t s);
+
 // cow: one byte per selected position, non-zero where that input is copy-on-write (null: none is);
 // live: null, or n int32 zeroed, to which every key adds +1 at the position where its accumulator
 // becomes non-empty and -1 where it becomes empty (the host replays the result's COW flag from them)

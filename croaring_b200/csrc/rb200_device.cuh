@@ -232,6 +232,28 @@ __host__ __device__ inline int offset_type(int tA, int tB, int card, int nruns) 
     return rule_eff(card, nruns);           // a run with a run or an array: the efficient container
 }
 
+// Result type of one key of roaring_bitmap_add_range_closed / remove_range_closed (src/roaring.c:251,
+// 302) that the range covers in part: container_add_range / container_remove_range (containers.h:
+// 2280-2430) of S's container of type t, or container_range_of_ones (containers.h:300) when S lacks
+// the key (t = 0, add only).  roaring.c:291 hands that one an exclusive end, which its cardinality
+// test counts as a value: only a single new value is an array.  card: the result's cardinality.  nruns: for a run add, the runs the
+// reference counts before it decides, nruns_less + 1 + nruns_greater (rle16_count_less / _greater,
+// run.h:156-196, merge adjacent runs); for a run removal, the runs of the result.  0: dropped.  A key
+// the range covers whole is a full run after an add and dropped after a removal, whatever it held.
+__host__ __device__ inline int range_type(bool add, int t, int card, int nruns) {
+    if (card == 0) return 0;
+    if (add) {
+        if (t == 0) return card + 1 <= 2 ? T_ARRAY : T_RUN;
+        if (t == T_RUN)   // run_container_add_range_nruns, else container_from_run_range (convert.c:323)
+            return 4 * nruns <= BITSET_BYTES ? T_RUN : rule_ab(card);
+        if (card == 65536) return T_RUN;
+        return t == T_BITSET ? T_BITSET : rule_ab(card);   // an add never demotes a bitset
+    }
+    if (t == T_ARRAY) return T_ARRAY;
+    if (t == T_BITSET) return rule_ab(card);
+    return rule_eff(card, nruns);   // convert_run_to_efficient_container, even when no value went
+}
+
 __host__ __device__ __forceinline__ uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
 
 // payload bytes as stored in a slab (runs without the 2-byte n_runs prefix)

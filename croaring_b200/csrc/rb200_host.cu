@@ -3433,6 +3433,100 @@ rb200_set_t *rb200_batch_add_offset(const rb200_set_t *S, const uint32_t *idx, s
     return call.finish(ok);
 }
 
+// ---- range updates: roaring_bitmap_add_range_closed / remove_range_closed (src/roaring.c:251, 302) --
+// result[k] = S[idx[k]] with [mins[k], maxs[k]] added (add) or removed; mins[k] > maxs[k] changes
+// nothing.  An add gives item k one slot per container of S[idx[k]] plus one per key of its range, a
+// removal one per container (rb200_range.cu); k_finalize_pairs compacts them into the result
+// directory.  Containers outside the range are shared with S, or copied when S shares containers
+// itself (holds never chain, see rb200_set::held).  This is not a batch op with a range bitmap per item,
+// as flip is: the type rules differ from OR / ANDNOT, and every key the range covers whole would cost
+// a cell of its own.
+extern "C++" {
+namespace {
+// keys of [lo, hi] (0 for an empty range)
+uint64_t range_keys(uint32_t lo, uint32_t hi) { return lo <= hi ? (hi >> 16) - (lo >> 16) + 1 : 0; }
+
+const char *range_too_large = ": batch too large: more than 2^32 - 1 container slots, split it";
+
+rb200_set *range_impl(bool add, const std::string &what, const rb200_set *S, const uint32_t *idx, size_t n,
+                      const uint32_t *mins, const uint32_t *maxs) {
+    // the ranges of m items; an add whose range keys alone exceed the item slots a batch can address is
+    // refused here (a full 32-bit range is 65536 keys per item).  With an idx, n is known before S is read.
+    const auto ranges_ok = [&](size_t m) {
+        if (m && (!mins || !maxs)) { t_err = what + ": min / max is NULL"; return false; }
+        uint64_t keys = 0;
+        for (size_t p = 0; add && p < m && keys <= 0xffffffffull; p++) keys += range_keys(mins[p], maxs[p]);
+        if (keys > 0xffffffffull) { t_err = what + range_too_large; return false; }
+        return true;
+    };
+    Selection sel{S, idx, n};
+    if ((idx && !ranges_ok(n)) || !sel.check(what.c_str()) || (!idx && !ranges_ok(sel.n))) return nullptr;
+    n = sel.n;
+    if (!ctx_init() || !ensure_mirrors(S)) return nullptr;
+    // item slots and the result slab, sized from the host mirrors before the launch: 8 KiB for each
+    // of the at most two boundary cells (every result type is at most a bitset), 16 bytes for every
+    // key an add writes whole (a full run, or a new key's container_range_of_ones), and the stored
+    // bytes of S's containers when they are copied rather than shared.
+    const size_t o_off = 0, o_idx = al256(8 * (n + 1)), o_min = o_idx + al256(4 * n), o_max = o_min + al256(4 * n),
+                 bytes = o_max + al256(4 * n);
+    PinBlock<uint8_t> h(bytes);
+    DevBlock<uint8_t> d(bytes);
+    if (!h || !d) return nullptr;
+    uint64_t *off = (uint64_t *)(h.get() + o_off);
+    uint32_t *hidx = (uint32_t *)(h.get() + o_idx), *hmin = (uint32_t *)(h.get() + o_min), *hmax = (uint32_t *)(h.get() + o_max);
+    uint64_t w = 0, sb = 64, sb_copy = 0;
+    for (size_t p = 0; p < n; p++) {
+        const uint32_t b = sel[p];
+        const uint64_t nk = range_keys(mins[p], maxs[p]);
+        hidx[p] = b;
+        hmin[p] = mins[p];
+        hmax[p] = maxs[p];
+        off[p] = w;
+        w += S->h_cnt[b] + (add ? nk : 0);
+        sb += (nk ? 2 * (uint64_t)BITSET_BYTES : 0) + (add ? 16 * nk : 0);
+        sb_copy += S->h_bytes[b];
+    }
+    off[n] = w;
+    if (w > 0xffffffffull) { t_err = what + range_too_large; return nullptr; }
+    const bool share = !S->sharing();
+    SetPtr R = set_new((uint32_t)n, w, share ? sb : sb + sb_copy);
+    PassShare sh = {false, false, 0, 0, 0};
+    if (R && share && !share_operands(R.get(), S, S, true, false, sh)) {
+        R.reset();   // out of the offsets' reach: copy everything into a slab sized for it
+        R = set_new((uint32_t)n, w, sb + sb_copy);
+    }
+    ItemsBuf ib_;
+    DevBlock<uint4> cell;
+    DeferredCall call(what.c_str(), R, h);
+    const bool ok = R && ib_.alloc(w, false, false) && cell.reset(2 * n) && call.begin() &&
+                    cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+    if (ok) {
+        const SetView vs = S->view();
+        const uint64_t *d_off = (const uint64_t *)(d.get() + o_off);
+        launch_range_plan(vs, (const uint32_t *)(d.get() + o_idx), (const uint32_t *)(d.get() + o_min),
+                          (const uint32_t *)(d.get() + o_max), d_off, (uint32_t)n, add, sh, ib_.it, cell.get(),
+                          R->d_slab, R->slab_cap, g.d_dstats, g.stream);
+        launch_range_cells(vs, ib_.it, cell.get(), (uint32_t)n, add, sh.bias, R->d_slab, g.d_dstats, g.stream);
+        launch_finalize_pairs(vs, vs, ib_.it, d_off, (uint32_t)n, sh, R->out(), g.d_dstats, call.deliver(), g.stream);
+        R->parentA = S->h_ptr;
+        for (size_t p = 0; p < n; p++) R->h_flags[p] = sel.cow(p);   // the reference updates S in place
+    }
+    return call.finish(ok);
+}
+}  // namespace
+}  // extern "C++"
+
+rb200_set_t *rb200_batch_add_range_closed(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *min,
+                                          const uint32_t *max) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return range_impl(true, "add_range_closed", S, idx, n, min, max);
+}
+rb200_set_t *rb200_batch_remove_range_closed(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *min,
+                                             const uint32_t *max) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return range_impl(false, "remove_range_closed", S, idx, n, min, max);
+}
+
 // ---- negation: roaring_bitmap_flip (src/roaring.c:2289-2349) ------------------------------------
 // result[k] = S[idx[k]] with [range_start, range_end) negated.  The range is materialised as ONE
 // tiny bitmap of run containers (one {lo, hi-lo} run per key it touches) and every flip is a
@@ -3937,6 +4031,80 @@ Set *update(int op, const char *what, const Set *S, const uint32_t *idx, size_t 
         return W ? batch_op64_impl(op, S, W.get(), ia.data(), ib.data(), sel.n, RULES_KEEP_RUN) : nullptr;
     }
 }
+
+// ---- range updates: roaring64_bitmap_add_range_closed / remove_range_closed (roaring64.c:651, 996) ------
+// The same container_add_range / container_remove_range per 48-bit key, so one closed 32-bit range per
+// bucket: [min_lo32, 2^32 - 1] on the first bucket of the span (or [min_lo32, max_lo32] when it is also
+// the last), all of every middle bucket and [0, max_lo32] on the last.  The buckets are planned here as
+// plan64 plans them: a bucket outside the span is a no-op item; an add makes an item of every bucket of
+// its span, on the inner set's sentinel where S lacks it; a removal drops the middle buckets
+// (roaring64.c:1017-1025).  ONE call of the 32-bit path over the inner set then updates every bucket, and
+// a bucket a removal empties stays an empty inner bitmap, which is never planned, counted or serialized.
+extern "C++" rb200_set64 *range64_impl(bool add, const std::string &what, const rb200_set64 *S, const uint32_t *idx,
+                                       size_t n, const uint64_t *mins, const uint64_t *maxs) {
+    // as range_impl: an add whose 48-bit range keys alone exceed the item slots of a batch is refused
+    // before any device work (the keys also bound the buckets of the spans)
+    const auto ranges_ok = [&](size_t m) {
+        if (m && (!mins || !maxs)) { t_err = what + ": min / max is NULL"; return false; }
+        uint64_t keys = 0;
+        for (size_t p = 0; add && p < m && keys <= 0xffffffffull; p++)
+            if (mins[p] <= maxs[p]) keys += (maxs[p] >> 16) - (mins[p] >> 16) + 1;
+        if (keys > 0xffffffffull) { t_err = what + range_too_large; return false; }
+        return true;
+    };
+    SelectionOf<rb200_set64> sel{S, idx, n};
+    if ((idx && !ranges_ok(n)) || !sel.check(what.c_str()) || (!idx && !ranges_ok(sel.n))) return nullptr;
+    n = sel.n;
+    if (!ctx_init() || !ensure_mirrors(S->inner.get())) return nullptr;
+    const uint32_t *cnt = S->inner->h_cnt.data(), *high = S->high(), E = S->nbuckets - 1;
+    std::vector<uint32_t> ib, lo, hi, rhigh, rcnt(n);
+    const auto item = [&](uint32_t bucket, uint32_t h, uint32_t l, uint32_t u) {
+        ib.push_back(bucket);
+        rhigh.push_back(h);
+        lo.push_back(l);
+        hi.push_back(u);
+    };
+    for (size_t p = 0; p < n; p++) {
+        const uint32_t b = sel[p];
+        uint32_t i = S->b_beg()[b];
+        const uint32_t ie = i + S->b_cnt()[b];
+        const size_t first = ib.size();
+        const uint64_t mn = mins[p], mx = maxs[p];
+        const bool live = mn <= mx;
+        const uint32_t hmin = (uint32_t)(mn >> 32), hmax = (uint32_t)(mx >> 32);
+        for (; i < ie && (!live || high[i] < hmin); i++)
+            if (cnt[i]) item(i, high[i], 1, 0);
+        if (live && add) {
+            for (uint64_t h = hmin; h <= hmax; h++) {
+                const bool has = i < ie && high[i] == h;
+                item(has ? i : E, (uint32_t)h, h == hmin ? (uint32_t)mn : 0u, h == hmax ? (uint32_t)mx : 0xffffffffu);
+                i += has;
+            }
+        } else if (live) {
+            for (; i < ie && high[i] <= hmax; i++)
+                if (cnt[i] && (high[i] == hmin || high[i] == hmax))
+                    item(i, high[i], high[i] == hmin ? (uint32_t)mn : 0u, high[i] == hmax ? (uint32_t)mx : 0xffffffffu);
+        }
+        for (; i < ie; i++)
+            if (cnt[i]) item(i, high[i], 1, 0);
+        rcnt[p] = (uint32_t)(ib.size() - first);
+        if (ib.size() >= 0xffffffffull) {   // + the result's sentinel must fit a 32-bit bitmap index
+            t_err = what + ": more than 2^32 - 2 buckets, split the batch";
+            return nullptr;
+        }
+    }
+    item(E, 0, 1, 0);   // the result's own sentinel
+    Set64Ptr R = set64_new((uint32_t)n, (uint32_t)ib.size());
+    if (!R) return nullptr;
+    uint32_t *dir = R->h_dir.get();
+    for (size_t p = 0, b = 0; p < n; b += rcnt[p], p++) {
+        dir[p] = (uint32_t)b;
+        dir[n + p] = rcnt[p];
+    }
+    memcpy(dir + 2 * n, rhigh.data(), 4 * rhigh.size());
+    R->inner.reset(range_impl(add, what, S->inner.get(), ib.data(), ib.size(), lo.data(), hi.data()));
+    return R->inner ? R.release() : nullptr;
+}
 }  // namespace
 
 rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size_t *lens, size_t n) {
@@ -4019,6 +4187,16 @@ rb200_set64_t *rb200_set64_batch_remove_many_device(const rb200_set64_t *S, cons
                                                     const uint64_t *d_vals, const uint64_t *d_off) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return update(OP_ANDNOT, "set64_remove_many_device", S, idx, n, d_vals, d_off, true);
+}
+rb200_set64_t *rb200_set64_batch_add_range_closed(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                  const uint64_t *min, const uint64_t *max) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return range64_impl(true, "set64_add_range_closed", S, idx, n, min, max);
+}
+rb200_set64_t *rb200_set64_batch_remove_range_closed(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                     const uint64_t *min, const uint64_t *max) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return range64_impl(false, "set64_remove_range_closed", S, idx, n, min, max);
 }
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);

@@ -202,9 +202,9 @@ int rb200_batch_and_cardinality(const rb200_set_t *A, const rb200_set_t *B, cons
 int rb200_batch_relations(const rb200_set_t *A, const rb200_set_t *B, const uint32_t *ia,
                           const uint32_t *ib, size_t npairs, uint8_t *out);
 
-/* Selections.  rb200_batch_flip, rb200_batch_add_offset, the add_many / remove_many family, the or_many / xor_many
- * entry points and rb200_batch_query work on S[idx[0..n)]; idx == NULL selects every bitmap of S in order (n is
- * then ignored).  A NULL or lazy S, and with an idx, n >= 2^32 or an entry out of range, is refused before any
+/* Selections.  rb200_batch_flip, rb200_batch_add_offset, the add_many / remove_many and add_range / remove_range
+ * families, the or_many / xor_many entry points and rb200_batch_query work on S[idx[0..n)]; idx == NULL selects
+ * every bitmap of S in order (n is then ignored).  A NULL or lazy S, and with an idx, n >= 2^32 or an entry out of range, is refused before any
  * device work; rb200_last_error() names the entry point.  rb200_batch_query_device reads its idx on the
  * device: the kernel checks every entry, and the call fails after it with the same message. */
 
@@ -233,6 +233,18 @@ rb200_set_t *rb200_batch_add_many_device(const rb200_set_t *S, const uint32_t *i
                                          const uint64_t *d_off);
 rb200_set_t *rb200_batch_remove_many_device(const rb200_set_t *S, const uint32_t *idx, size_t n,
                                             const uint32_t *d_vals, const uint64_t *d_off);
+
+/* result[k] = S[idx[k]] after roaring_bitmap_add_range_closed / _remove_range_closed of the closed range
+ * [min[k], max[k]]; idx == NULL: every bitmap in order (n = rb200_set_count(S)).  min[k] > max[k] leaves the
+ * bitmap as it is.  Results match the reference's bytes and keep S's copy-on-write flag; containers outside
+ * the range are shared with S, not copied.  min / max: host arrays of n entries, NULL only when there are
+ * no items; a batch of more than 2^32 - 1 container slots (containers of the selected bitmaps, plus, for
+ * an add, the 65536-value keys the ranges touch) is refused before any device work.  Returns a new resident
+ * set, NULL on error (rb200_last_error). */
+rb200_set_t *rb200_batch_add_range_closed(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *min,
+                                          const uint32_t *max);
+rb200_set_t *rb200_batch_remove_range_closed(const rb200_set_t *S, const uint32_t *idx, size_t n, const uint32_t *min,
+                                             const uint32_t *max);
 
 /* Point queries, one value per query.  Query k asks bitmap S[idx[k]] about vals[k], k < n; idx == NULL: query k
  * asks bitmap k (n = rb200_set_count(S)).  Values in any order, repeats allowed.  out[k]:
@@ -334,6 +346,13 @@ rb200_set64_t *rb200_set64_batch_add_many_device(const rb200_set64_t *S, const u
                                                  const uint64_t *d_vals, const uint64_t *d_off);
 rb200_set64_t *rb200_set64_batch_remove_many_device(const rb200_set64_t *S, const uint32_t *idx, size_t n,
                                                     const uint64_t *d_vals, const uint64_t *d_off);
+/* result[k] = S[idx[k]] after roaring64_bitmap_add_range_closed / _remove_range_closed of [min[k], max[k]], with
+ * the selection and arguments of rb200_batch_add_range_closed; 2^64 - 1 is a valid max.  Buckets a removal
+ * empties are left out of the result. */
+rb200_set64_t *rb200_set64_batch_add_range_closed(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                  const uint64_t *min, const uint64_t *max);
+rb200_set64_t *rb200_set64_batch_remove_range_closed(const rb200_set64_t *S, const uint32_t *idx, size_t n,
+                                                     const uint64_t *min, const uint64_t *max);
 /* mode 1 = roaring64_bitmap_run_optimize, mode 0 = remove the run containers (as rb200_set_run_optimize). */
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *s, int mode);
 /* Device-side roaring64_bitmap_portable_serialize of every bitmap + one D2H: blob i = *buf + (*off)[i],

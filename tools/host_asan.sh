@@ -15,7 +15,7 @@ for f in rb200_host rb200_shard; do
        -c $f.cu -o "$OUT/$f.o" 2>&1 | grep -v deprecated || true
 done
 nvcc -shared -cudart static -o "$OUT/libroaring_b200_asan.so" "$OUT/rb200_host.o" "$OUT/rb200_shard.o" \
-     rb200_kernels.o rb200_compute.o rb200_many.o rb200_many2.o rb200_convert.o rb200_build.o rb200_fused.o rb200_offset.o rb200_query.o \
+     rb200_kernels.o rb200_compute.o rb200_many.o rb200_many2.o rb200_convert.o rb200_build.o rb200_fused.o rb200_offset.o rb200_query.o rb200_range.o \
      -Xlinker -Bsymbolic -ldl -lpthread -Xcompiler -fsanitize=address,-fsanitize=undefined 2>&1 | grep -v deprecated || true
 cd "$ROOT"
 export RB200_LIB="$OUT/libroaring_b200_asan.so" ASAN_OPTIONS=detect_leaks=0 UBSAN_OPTIONS=print_stacktrace=1
