@@ -104,6 +104,10 @@ struct Ctx {
     bool inited = false;
     int device = 0;
     cudaStream_t own_stream = nullptr, stream = nullptr;
+    // pair-list uploads (PairBuf): enqueued as soon as the host has built the list, ahead of the
+    // library stream's queue, which waits for them through an event instead of holding the copy
+    // between two chained launches
+    cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evk0 = nullptr, evk1 = nullptr;
     OpStats *d_stats = nullptr;
     OpStats *h_stats = nullptr;  // pinned
@@ -121,6 +125,9 @@ struct Ctx {
     uint8_t *h_fused_in = nullptr, *d_fused_in = nullptr, *h_fused_out = nullptr, *d_fused_out = nullptr;
     uint32_t fused_seq = 0;
     std::multimap<size_t, void *> dpool, hpool;
+    // device blocks the copy stream writes into: a block comes back here only once nothing queued
+    // can still read it (CopyBlock), so a copy into it never has to wait for the library stream
+    std::multimap<size_t, void *> cpool;
     std::mutex alloc_mu;  // dpool / hpool are also used by the background downloader thread
     uint64_t dev_in_use = 0;  // bytes of device blocks handed out by dev_alloc and not returned (under alloc_mu)
     uint64_t last_algo_bytes = 0;
@@ -166,6 +173,7 @@ bool ctx_init(int device = -1) {
     CK(cudaGetDevice(&g.device));
     CK(cudaStreamCreateWithFlags(&g.own_stream, cudaStreamNonBlocking));
     g.stream = g.own_stream;
+    CK(cudaStreamCreateWithFlags(&g.copy_stream, cudaStreamNonBlocking));
     CK(cudaEventCreate(&g.ev0));
     CK(cudaEventCreate(&g.ev1));
     CK(cudaEventCreate(&g.evk0));
@@ -193,14 +201,14 @@ bool ctx_init(int device = -1) {
     return true;
 }
 
-void *dev_alloc(size_t n) {
+void *dev_alloc(size_t n, std::multimap<size_t, void *> &pool = g.dpool) {
     std::lock_guard<std::mutex> alk(g.alloc_mu);
     if (n == 0) n = 1;
     const size_t b = bucket(n);
-    auto it = g.dpool.find(b);
-    if (it != g.dpool.end()) {
+    auto it = pool.find(b);
+    if (it != pool.end()) {
         void *p = it->second;
-        g.dpool.erase(it);
+        pool.erase(it);
         g.dev_in_use += b;
         return p;
     }
@@ -210,8 +218,10 @@ void *dev_alloc(size_t n) {
         // drop the cache and retry once; the failure is reported through t_err, so it must not stay
         // behind as the runtime's last error for the next launch check to find
         (void)cudaGetLastError();
-        for (auto &kv : g.dpool) cudaFree(kv.second);
-        g.dpool.clear();
+        for (auto *q : {&g.dpool, &g.cpool}) {
+            for (auto &kv : *q) cudaFree(kv.second);
+            q->clear();
+        }
         e = cudaMalloc(&p, b);
         if (e != cudaSuccess) {
             (void)cudaGetLastError();
@@ -222,11 +232,11 @@ void *dev_alloc(size_t n) {
     g.dev_in_use += b;
     return p;
 }
-void dev_free(void *p, size_t n) {
+void dev_free(void *p, size_t n, std::multimap<size_t, void *> &pool = g.dpool) {
     if (!p) return;
     std::lock_guard<std::mutex> alk(g.alloc_mu);
     if (n == 0) n = 1;
-    g.dpool.insert({bucket(n), p});
+    pool.insert({bucket(n), p});
     g.dev_in_use -= bucket(n);
 }
 bool enter_local_cpus(cpu_set_t *saved);
@@ -263,11 +273,13 @@ void pin_free(void *p, size_t n) {
     g.hpool.insert({bucket(n), p});
 }
 
-// Owner of one block of the device pool (Dev) or of the pinned pool: it keeps the byte size it
-// asked for, so the block goes back under the size class it came from.  A device block may be
-// released as soon as the work using it is enqueued (stream-ordered reuse on the library stream); a
-// pinned block only once no copy from or into it can still be in flight.
-template <typename T, bool Dev>
+// Owner of one block of the device pool, of the copy stream's device pool or of the pinned pool: it
+// keeps the byte size it asked for, so the block goes back under the size class it came from.  A
+// device block may be released as soon as the work using it is enqueued (stream-ordered reuse on the
+// library stream); a copy-stream block or a pinned block only once nothing that reads or writes it
+// can still be in flight.
+enum PoolKind { POOL_PINNED, POOL_DEVICE, POOL_COPY };
+template <typename T, PoolKind Kind>
 class PoolBlock {
    public:
     PoolBlock() = default;
@@ -287,12 +299,12 @@ class PoolBlock {
     bool reset(size_t count) {
         reset();
         const size_t b = count ? sizeof(T) * count : 1;
-        p_ = (T *)(Dev ? dev_alloc(b) : pin_alloc(b));
+        p_ = (T *)(Kind == POOL_PINNED ? pin_alloc(b) : dev_alloc(b, Kind == POOL_COPY ? g.cpool : g.dpool));
         bytes_ = p_ ? b : 0;
         return p_ != nullptr;
     }
     void reset() {
-        if (p_) Dev ? dev_free(p_, bytes_) : pin_free(p_, bytes_);
+        if (p_) Kind == POOL_PINNED ? pin_free(p_, bytes_) : dev_free(p_, bytes_, Kind == POOL_COPY ? g.cpool : g.dpool);
         p_ = nullptr;
         bytes_ = 0;
     }
@@ -304,8 +316,9 @@ class PoolBlock {
     T *p_ = nullptr;
     size_t bytes_ = 0;
 };
-template <typename T> using DevBlock = PoolBlock<T, true>;
-template <typename T> using PinBlock = PoolBlock<T, false>;
+template <typename T> using DevBlock = PoolBlock<T, POOL_DEVICE>;
+template <typename T> using PinBlock = PoolBlock<T, POOL_PINNED>;
+template <typename T> using CopyBlock = PoolBlock<T, POOL_COPY>;
 
 std::map<uint8_t *, PinBlock<uint8_t>> g_serialized;  // pinned blobs handed out, until rb200_serialized_free
 
@@ -411,6 +424,7 @@ struct rb200_set {
     bool pending = false, failed = false;
     PinBlock<OpStats> pstats;
     PinBlock<uint8_t> staging;                  // pair list of the op (alive until it ran)
+    CopyBlock<uint8_t> staging_dev;             // its device copy (alive until the op ran)
     cudaEvent_t done = nullptr;                 // the op's end (completion only: its times are in pstats)
     float ms = 0.f, compute_ms = 0.f;
     uint64_t algo_bytes = 0, out_portable = 0;
@@ -464,7 +478,10 @@ struct rb200_set {
 
 namespace {
 
-SetPtr set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
+// mirrors = false: h_cnt / h_bytes / h_ebytes stay empty, for a batch result whose first
+// ensure_mirrors() fills them from the device (a result that is only measured, chained on the device or
+// downloaded never needs them)
+SetPtr set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap, bool mirrors = true) {
     SetPtr s(new rb200_set());
     s->n_bitmaps = nb;
     s->dir_cap = dir_cap;
@@ -474,9 +491,11 @@ SetPtr set_new(uint32_t nb, uint64_t dir_cap, uint64_t slab_cap) {
     s->slab = std::make_shared<Slab>(slab_cap);
     if (!s->slab->p) return nullptr;
     s->d_slab = s->d_base = s->slab->p;
-    s->h_cnt.assign(nb, 0);
-    s->h_bytes.assign(nb, 0);
-    s->h_ebytes.assign(nb, 0);
+    if (mirrors) {
+        s->h_cnt.assign(nb, 0);
+        s->h_bytes.assign(nb, 0);
+        s->h_ebytes.assign(nb, 0);
+    }
     s->h_flags.assign(nb, 0);
     return s;
 }
@@ -609,7 +628,9 @@ class SyncCall {
 // counters it may have left behind.  `what` heads the default t_err.
 class DeferredCall {
    public:
-    DeferredCall(const char *what, SetPtr &R, PinBlock<uint8_t> &staging) : what_(what), R_(R), staging_(staging) {}
+    // staging_dev: a device block the copy stream filled for the op's kernels, held like staging
+    DeferredCall(const char *what, SetPtr &R, PinBlock<uint8_t> &staging, CopyBlock<uint8_t> *staging_dev = nullptr)
+        : what_(what), R_(R), staging_(staging), staging_dev_(staging_dev) {}
     DeferredCall(const DeferredCall &) = delete;
     bool begin() {
         R_->done = ev_get(false);
@@ -629,6 +650,7 @@ class DeferredCall {
         }
         R_->pending = true;
         R_->staging = std::move(staging_);
+        if (staging_dev_) R_->staging_dev = std::move(*staging_dev_);
         R_->mirrors_pending = R_->n_bitmaps > 0;  // h_cnt / h_bytes / h_card: see ensure_mirrors()
         g.last_op = R_.get();
         return R_.release();
@@ -638,6 +660,7 @@ class DeferredCall {
     const char *what_;
     SetPtr &R_;
     PinBlock<uint8_t> &staging_;
+    CopyBlock<uint8_t> *staging_dev_;
     OpStats *deliver_ = nullptr;   // R's pinned counters, device address
 };
 
@@ -648,6 +671,7 @@ void retire_op(rb200_set *s) {
     s->done = nullptr;
     s->pstats.reset();
     s->staging.reset();
+    s->staging_dev.reset();
 }
 
 // Wait for the op that produced `cs` (if it is still in flight) and take over its counters.
@@ -678,9 +702,9 @@ bool resolve(const rb200_set *cs) {
         for (int k = 0; k < 2; k++)   // an operand none of whose containers was shared is not held
             if (!st.shared_used[k]) s->held[k].reset();
         if (s->n_bitmaps == 1 && !s->sharing()) {  // a single result: its mirrors are the op's counters, no extra D2H
-            s->h_cnt[0] = (uint32_t)s->n_containers;
-            s->h_bytes[0] = s->slab_used;
-            s->h_ebytes[0] = std::max<uint64_t>(s->slab_used, s->n_containers * (uint64_t)BITSET_BYTES);
+            s->h_cnt.assign(1, (uint32_t)s->n_containers);
+            s->h_bytes.assign(1, s->slab_used);
+            s->h_ebytes.assign(1, std::max<uint64_t>(s->slab_used, s->n_containers * (uint64_t)BITSET_BYTES));
             s->mirrors_pending = false;
         }
     }
@@ -1234,11 +1258,9 @@ bool ensure_mirrors(const rb200_set *cs) {
         const uint64_t *bb = (const uint64_t *)(h + (s->L.o_bbytes - s->L.o_cnt));
         const uint64_t *be = (const uint64_t *)(h + (s->L.o_bebytes - s->L.o_cnt));
         s->h_card.assign(card, card + nb);
-        for (size_t p = 0; p < nb; p++) {
-            s->h_cnt[p] = cnt[p];
-            s->h_bytes[p] = bb[p];    // exact stored bytes (16-byte rounded slots) of this bitmap
-            s->h_ebytes[p] = be[p];   // what a later op on it can produce at most (see PairBuf::build)
-        }
+        s->h_cnt.assign(cnt, cnt + nb);
+        s->h_bytes.assign(bb, bb + nb);    // exact stored bytes (16-byte rounded slots) of each bitmap
+        s->h_ebytes.assign(be, be + nb);   // what a later op on it can produce at most (see PairBuf::build)
         s->mirrors_pending = false;
     } else {
         t_err = "fetching result directory failed";
@@ -1281,12 +1303,47 @@ struct ItemsBuf {
     }
 };
 
-// pair lists + item offsets: one pinned staging block, one H2D copy
+#ifdef RB200_HOST_TIMING
+// Host time of every batch_op_impl call, split by phase (tools/time_host_call.py reads it through
+// rb200_host_timing_take).  Only the timing variant of the library carries it.
+enum { HT_CHECKS, HT_STAGING, HT_PAIRS, HT_COPY, HT_ITEMS, HT_SET_NEW, HT_BEGIN, HT_LAUNCH, HT_FINISH, HT_N };
+struct HostTiming {
+    double last = 0, entry = 0, copied = 0, ph[HT_N] = {};
+    std::vector<double> rec;   // per call: entry, copy enqueued (CLOCK_MONOTONIC s), HT_N phase durations (s)
+};
+HostTiming g_ht;
+double ht_now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+void ht_mark(int k) {
+    const double t = ht_now();
+    g_ht.ph[k] += t - g_ht.last;
+    g_ht.last = t;
+    if (k == HT_COPY) g_ht.copied = t;
+}
+void ht_enter() {
+    g_ht = HostTiming{0, 0, 0, {}, std::move(g_ht.rec)};
+    g_ht.entry = g_ht.last = ht_now();
+}
+void ht_leave() {
+    ht_mark(HT_FINISH);
+    g_ht.rec.push_back(g_ht.entry);
+    g_ht.rec.push_back(g_ht.copied);
+    g_ht.rec.insert(g_ht.rec.end(), g_ht.ph, g_ht.ph + HT_N);
+}
+#define HT_MARK(k) ht_mark(k)
+#else
+#define HT_MARK(k) ((void)0)
+#endif
+
+// pair lists + item offsets: one pinned staging block, one H2D copy on the copy stream, which the
+// library stream waits for.  The copy starts as soon as the list is built instead of behind the
+// kernels already queued, and no copy sits between two chained launches.  The device block comes
+// from the copy stream's pool and stays with the caller (a batch result: until its op has run), so
+// the copy never overwrites what a queued kernel still reads.
 // (tried: k_plan_pairs reading the staging block through its mapped address instead, which keeps the
 //  copy off the stream — its scattered 4- and 8-byte reads over PCIe made the kernel 2-3x slower)
 struct PairBuf {
     PinBlock<uint8_t> h;
-    DevBlock<uint8_t> d;
+    CopyBlock<uint8_t> d;
     uint32_t *d_ia = nullptr, *d_ib = nullptr;
     uint64_t *d_off = nullptr;
     uint64_t W = 0;
@@ -1299,82 +1356,122 @@ struct PairBuf {
     // container ONE run)
     bool build(const rb200_set *A, const rb200_set *B, const uint32_t *ia, const uint32_t *ib,
                size_t np, int op, int rules = 0, int share = 0) {
-        const bool lazy = (rules & RULES_LAZY) != 0, flip = (rules & RULES_FLIP) != 0;
         if (!ensure_mirrors(A) || !ensure_mirrors(B)) return false;
         if (np > 0xffffffffull) { t_err = "too many pairs in one batch (2^32 - 1 at most)"; return false; }
         const size_t o_off = 0, o_ia = al256(8 * (np + 1)), o_ib = o_ia + al256(4 * np);
         const size_t bytes = o_ib + al256(4 * np);
+        HT_MARK(HT_CHECKS);
         if (!h.reset(bytes) || !d.reset(bytes)) return false;
-        uint64_t *off = (uint64_t *)(h.get() + o_off);
-        uint32_t *hia = (uint32_t *)(h.get() + o_ia), *hib = (uint32_t *)(h.get() + o_ib);
+        HT_MARK(HT_STAGING);
+        Lists L{(uint64_t *)(h.get() + o_off), (uint32_t *)(h.get() + o_ia), (uint32_t *)(h.get() + o_ib)};
+        const Side a = side(A), b = side(B);
+        const bool andnot = op == OP_ANDNOT;
+        bool ok;
+        if (rules & RULES_FLIP) ok = pairs<Bound::Flip>(a, b, ia, ib, np, andnot, share, L);
+        else if (rules & RULES_LAZY) ok = pairs<Bound::Lazy>(a, b, ia, ib, np, andnot, share, L);
+        else if (op == OP_AND) ok = pairs<Bound::And>(a, b, ia, ib, np, andnot, share, L);
+        else if (rules & RULES_KEEP_RUN) ok = pairs<Bound::KeepRun>(a, b, ia, ib, np, andnot, share, L);
+        else ok = pairs<Bound::Plain>(a, b, ia, ib, np, andnot, share, L);
+        if (!ok) return false;
+        // item ids, directory positions of the result and the order list are 32-bit on the device
+        if (W > 0xffffffffull) { t_err = "batch too large: more than 2^32 - 1 container slots, split the pair list"; return false; }
+        if (!share) slab_bound = slab_bound_copy;
+        d_off = (uint64_t *)(d.get() + o_off);
+        d_ia = (uint32_t *)(d.get() + o_ia);
+        d_ib = (uint32_t *)(d.get() + o_ib);
+        HT_MARK(HT_PAIRS);
+        ok = cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.copy_stream) == cudaSuccess;
+        if (ok) {
+            // completion only: the wait binds to this record, so the event can go back to the pool at once
+            cudaEvent_t ev = ev_get(false);
+            ok = ev && cudaEventRecord(ev, g.copy_stream) == cudaSuccess && cudaStreamWaitEvent(g.stream, ev, 0) == cudaSuccess;
+            ev_put(ev, false);
+            if (!ok) {
+                cudaStreamSynchronize(g.copy_stream);   // h and d are released with nothing in flight
+                t_err = "pair list upload failed";
+            }
+        }
+        HT_MARK(HT_COPY);
+        return ok;
+    }
+
+   private:
+    // The slab bound rule of a batch (see pairs()): each has its own instance of the pair loop, so the
+    // loop branches on neither the op nor its rules.
+    enum class Bound { Flip, Lazy, And, KeepRun, Plain };
+    // an operand's host mirrors (current: ensure_mirrors) as the pair loop reads them
+    struct Side {
+        const uint32_t *cnt;
+        const uint64_t *ebytes;
+        const uint8_t *flags;
+        uint64_t n;
+    };
+    static Side side(const rb200_set *S) { return {S->h_cnt.data(), S->h_ebytes.data(), S->h_flags.data(), S->n_bitmaps}; }
+    // the staging block's item offsets (np + 1) and pair lists
+    struct Lists {
+        uint64_t *off;
+        uint32_t *ia, *ib;
+    };
+    // One pass over the pairs: checks both indices, writes the pair lists and item offsets, and sums
+    // the items W, the slab bounds and the COW flags.
+    template <Bound R>
+    bool pairs(const Side A, const Side B, const uint32_t *ia, const uint32_t *ib, size_t np, bool andnot,
+               int share, const Lists L) {
+        // 1 where a side's pass-through containers are copied into the result's own slab
+        const uint64_t ownA = share & 1 ? 0 : 1, ownB = share & 2 || andnot ? 0 : 1, withB = andnot ? 0 : 1;
+        uint64_t *__restrict off = L.off;
+        uint32_t *__restrict hia = L.ia, *__restrict hib = L.ib;
         uint64_t w = 0, sb = 0, sbs = 0;
         uint8_t flags = 0;
         for (size_t p = 0; p < np; p++) {
             const uint32_t a = ia[p], b = ib[p];
-            if (a >= A->n_bitmaps || b >= B->n_bitmaps) {
+            if (a >= A.n || b >= B.n) {
                 t_err = "pair index out of range";
                 return false;
             }
             hia[p] = a;
             hib[p] = b;
-            flags |= A->h_flags[a] | B->h_flags[b];
+            flags |= A.flags[a] | B.flags[b];
             off[p] = w;
-            const uint32_t na = A->h_cnt[a], nb = B->h_cnt[b];
+            const uint32_t na = A.cnt[a], nb = B.cnt[b];
             w += (uint64_t)na + nb;
             // Upper bound of the result slab of this pair, from the per-bitmap "effective bytes" E
             // (sum over containers of max(stored, min(8192, 2 * card)), 16-byte rounded): every
             // result container — computed or passed through — is an array, a bitset or a run no
             // larger than either, so it fits min(8192, 2 * card_result); card_result <= cA + cB
             // (OR, XOR), <= min(cA, cB) (AND), <= cA (ANDNOT).  slot_bound() obeys the same limits.
-            const uint64_t EA = A->h_ebytes[a], EB = B->h_ebytes[b];
-            if (flip) {
+            const uint64_t EA = A.ebytes[a], EB = B.ebytes[b], m = na < nb ? na : nb;
+            if constexpr (R == Bound::Flip) {
                 // the slots k_plan_pairs reserves: a copy of A's container (<= its effective bytes),
                 // a copy of a one-run range container (16), a matched cell (slot_bound_lazy with
                 // nB = 1: <= 8 KiB + 16 + twice A's stored bytes).  EB counts 8 KiB for every key
                 // the range covers, which for a range over the whole universe is 512 MiB per pair.
-                const uint64_t m = na < nb ? na : nb;
                 sb += 2 * EA + 16 * (uint64_t)nb + m * (uint64_t)(BITSET_BYTES + 16) + 512;
-            } else if (lazy) {
+            } else if constexpr (R == Bound::Lazy) {
                 // lazy array x run unions stay runs (4 bytes per input value / run), flips add 8 KiB per key
-                const uint64_t m = na < nb ? na : nb;
                 sb += 3 * (EA + EB) + m * (uint64_t)BITSET_BYTES + 512;
-            } else if (op == OP_AND) {
+            } else if constexpr (R == Bound::And) {
                 sb += (EA < EB ? EA : EB) + 64;
-            } else if (rules & RULES_KEEP_RUN) {
-                // add_many / remove_many: a cell with a run on the left takes slot_bound_keep_run,
-                // min(128 KiB, 4 (lA + cB)) <= A's container's bytes + min(128 KiB, 4 cB), and the last
-                // term is at most 16 x the effective bytes of B's container (2 cB up to 4096 values,
-                // 8 KiB above).  Every other slot is bounded as for the op itself.
-                const uint64_t E = EA + 16 * EB;
-                sb += E + 64;
-                if (share) {
-                    const uint64_t own = (share & 1 ? 0 : EA) + (share & 2 || op == OP_ANDNOT ? 0 : EB) +
-                                         (uint64_t)(na < nb ? na : nb) * 131072;
-                    sbs += (own < E ? own : E) + 64;
-                }
             } else {
-                const uint64_t E = op == OP_ANDNOT ? EA : EA + EB;
+                // KeepRun (add_many / remove_many): a cell with a run on the left takes
+                // slot_bound_keep_run, min(128 KiB, 4 (lA + cB)) <= A's container's bytes + min(128 KiB,
+                // 4 cB), and the last term is at most 16 x the effective bytes of B's container (2 cB up
+                // to 4096 values, 8 KiB above).  Every other slot is bounded as for the op itself.
+                const uint64_t E = R == Bound::KeepRun ? EA + 16 * EB : EA + withB * EB;
                 sb += E + 64;
                 // shared pass-through containers take no slot: the result's own containers are the
                 // copied side's and cells of matched keys, at most min(na, nb) of them, each <= 8 KiB
-                if (share) {
-                    const uint64_t own = (share & 1 ? 0 : EA) + (share & 2 || op == OP_ANDNOT ? 0 : EB) +
-                                         (uint64_t)(na < nb ? na : nb) * BITSET_BYTES;
-                    sbs += (own < E ? own : E) + 64;
-                }
+                // (KeepRun: <= 128 KiB)
+                const uint64_t own = ownA * EA + ownB * EB + m * (uint64_t)(R == Bound::KeepRun ? 131072 : BITSET_BYTES);
+                sbs += (own < E ? own : E) + 64;
             }
         }
         off[np] = w;
-        cow = (flags & FLAG_COW) != 0;
-        // item ids, directory positions of the result and the order list are 32-bit on the device
-        if (w > 0xffffffffull) { t_err = "batch too large: more than 2^32 - 1 container slots, split the pair list"; return false; }
         W = w;
         slab_bound_copy = sb;
-        slab_bound = share ? sbs : sb;
-        d_off = (uint64_t *)(d.get() + o_off);
-        d_ia = (uint32_t *)(d.get() + o_ia);
-        d_ib = (uint32_t *)(d.get() + o_ib);
-        return cudaMemcpyAsync(d.get(), h.get(), bytes, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
+        slab_bound = sbs;   // used when share != 0 (build())
+        cow = (flags & FLAG_COW) != 0;
+        return true;
     }
 };
 
@@ -1530,6 +1627,10 @@ uint64_t stored_bytes_total(const rb200_set *s) {
 
 rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const uint32_t *ia,
                          const uint32_t *ib, size_t np, int rules = 0) {
+#ifdef RB200_HOST_TIMING
+    ht_enter();
+    struct Leave { ~Leave() { ht_leave(); } } leave;
+#endif
     if (!ctx_init()) return nullptr;
     if (op < 0 || op > 3) { t_err = "bad op"; return nullptr; }
     if (rules & RULES_LAZY) {
@@ -1563,17 +1664,20 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
     //  the 199-pair successive sweep took more device time per call: a pair's cells serialise on
     //  its 8 warps while the three-kernel path spreads them over the GPU)
     if (ok) ok = ib_.alloc(pb.W, true, pb.W >= order_min);
+    HT_MARK(HT_ITEMS);
     PassShare sh = {false, false, 0, 0, 0};
     if (ok) {
-        R = set_new((uint32_t)np, pb.W, pb.slab_bound);
+        R = set_new((uint32_t)np, pb.W, pb.slab_bound, false);
         if (R && (onA || onB) && !share_operands(R.get(), A, B, onA, onB, sh)) {
             R.reset();   // out of the offsets' reach: copy everything into a slab sized for it
-            R = set_new((uint32_t)np, pb.W, pb.slab_bound_copy);
+            R = set_new((uint32_t)np, pb.W, pb.slab_bound_copy, false);
         }
         ok = R != nullptr;
     }
-    DeferredCall call("batch op", R, pb.h);
+    HT_MARK(HT_SET_NEW);
+    DeferredCall call("batch op", R, pb.h, &pb.d);
     if (ok) ok = call.begin();
+    HT_MARK(HT_BEGIN);
     if (ok) {
         const SetView va = A->view(), vb = B->view();
         launch_plan_pairs(va, vb, pb.d_ia, pb.d_ib, pb.d_off, (uint32_t)np, op, false, rules, sh, ib_.it,
@@ -1600,6 +1704,7 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
                 R->h_flags[p] = result_cow(op, rules, A->h_flags[ia[p]], B->h_flags[ib[p]], A->h_cnt[ia[p]] == 0,
                                            B->h_cnt[ib[p]] == 0);
     }
+    HT_MARK(HT_LAUNCH);
     // the device buffers go back when pb / ib_ leave scope: stream-ordered reuse
     return call.finish(ok);
 }
@@ -1607,6 +1712,20 @@ rb200_set *batch_op_impl(int op, const rb200_set *A, const rb200_set *B, const u
 }  // namespace
 
 extern "C" {
+
+#ifdef RB200_HOST_TIMING
+// Copies up to `cap` doubles of the recorded calls (2 + HT_N per call, see HostTiming) to `out` and
+// forgets them; returns the number of doubles recorded (out == NULL: just count).
+__attribute__((visibility("default"))) size_t rb200_host_timing_take(double *out, size_t cap) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    const size_t n = g_ht.rec.size();
+    if (out) {
+        std::copy(g_ht.rec.begin(), g_ht.rec.begin() + std::min(n, cap), out);
+        g_ht.rec.clear();
+    }
+    return n;
+}
+#endif
 
 rb200_set_t *rb200_batch_op(int op, const rb200_set_t *A, const rb200_set_t *B, const uint32_t *ia,
                             const uint32_t *ib, size_t npairs) {
