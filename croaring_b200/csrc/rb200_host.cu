@@ -232,10 +232,25 @@ void *dev_alloc(size_t n, std::multimap<size_t, void *> &pool = g.dpool) {
     g.dev_in_use += b;
     return p;
 }
+// RB200_POISON_POOL=1 (read when the library loads): every block is zero-filled as it goes back to its
+// pool, so a kernel or copy that still reads a released block sees zeros instead of the old bytes, and
+// a lifetime bug shows up as wrong results (zeroed counts and offsets keep stale reads inside their
+// buffers).  Off by default: no fill, no other change.
+const bool g_poison = []() {
+    const char *e = getenv("RB200_POISON_POOL");
+    const bool on = e && e[0] == '1';
+    if (on) fprintf(stderr, "libroaring_b200: pool poisoning on\n");
+    return on;
+}();
+
 void dev_free(void *p, size_t n, std::multimap<size_t, void *> &pool = g.dpool) {
     if (!p) return;
-    std::lock_guard<std::mutex> alk(g.alloc_mu);
     if (n == 0) n = 1;
+    // ordered after every reader, which was queued before the release: the library stream for the
+    // device pool, the copy stream (the next writer of the block) for the copy pool
+    if (g_poison && cudaMemsetAsync(p, 0, bucket(n), &pool == &g.cpool ? g.copy_stream : g.stream) != cudaSuccess)
+        (void)cudaGetLastError();
+    std::lock_guard<std::mutex> alk(g.alloc_mu);
     pool.insert({bucket(n), p});
     g.dev_in_use -= bucket(n);
 }
@@ -268,8 +283,9 @@ void *pin_alloc(size_t n) {
 }
 void pin_free(void *p, size_t n) {
     if (!p) return;
-    std::lock_guard<std::mutex> alk(g.alloc_mu);
     if (n == 0) n = 1;
+    if (g_poison) memset(p, 0, bucket(n));   // pinned blocks come back only when nothing is in flight
+    std::lock_guard<std::mutex> alk(g.alloc_mu);
     g.hpool.insert({bucket(n), p});
 }
 
@@ -402,7 +418,10 @@ struct rb200_set {
     uint64_t dir_cap = 0;      // directory entries allocated
     uint64_t n_containers = 0; // directory entries in use
     uint64_t slab_cap = 0, slab_used = 0;
-    uint64_t portable_bytes = 0;  // sum of container_size_in_bytes
+    // sum of container_size_in_bytes: set by the uploads and builders that know it (portable_known),
+    // otherwise computed from the directory on first request (payload_bytes_of)
+    uint64_t portable_bytes = 0;
+    bool portable_known = false;
     DirLayout L;
     DevBlock<uint8_t> d_dir;    // one block
     uint8_t *d_slab = nullptr;  // own payload slab (owned through `slab`)
@@ -726,6 +745,35 @@ void set_delete(rb200_set *s) {
     delete s;  // the slabs return to the pool unless a result still points into them
 }
 void SetFree::operator()(rb200_set *s) const { set_delete(s); }
+
+// container_size_in_bytes summed over the set's containers, waiting for the op that produced it.  A set
+// made by an op is summed from its directory (types and lengths, one D2H) on the first request and
+// keeps the sum: a set never changes after the op that made it.  0 with t_err set if the set failed.
+uint64_t payload_bytes_of(const rb200_set *cs) {
+    rb200_set *s = const_cast<rb200_set *>(cs);
+    if (!resolve(s)) return 0;
+    if (s->portable_known) return s->portable_bytes;
+    const size_t nc = s->n_containers;
+    PinBlock<uint8_t> h(5 * nc);
+    const bool ok = h && (nc == 0 ||
+                          (cudaMemcpyAsync(h.get(), s->d_dir.get() + s->L.o_type, nc, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                           cudaMemcpyAsync(h.get() + nc, s->d_dir.get() + s->L.o_len, 4 * nc, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess &&
+                           cudaStreamSynchronize(g.stream) == cudaSuccess));
+    if (!ok) {
+        t_err = "fetching the set's directory failed";
+        return 0;
+    }
+    const uint8_t *type = h.get();
+    uint64_t sum = 0;
+    for (size_t c = 0; c < nc; c++) {
+        uint32_t len;
+        memcpy(&len, h.get() + nc + 4 * c, 4);
+        sum += portable_bytes(type[c], len);
+    }
+    s->portable_bytes = sum;
+    s->portable_known = true;
+    return sum;
+}
 
 // ------------------------------------------------------------------ host containers
 inline const void *unwrap_shared(const void *c, uint8_t &type) {  // containers.h:105-114
@@ -1071,6 +1119,7 @@ rb200_set *upload_impl(const roaring_bitmap_t *const *bms, size_t nb) {
             s->h_bytes[b] = bbytes;
             s->h_ebytes[b] = bebytes;
         }
+        s->portable_known = true;
         ok = ok && stage.flush() &&
              cudaMemcpyAsync(s->d_dir.get(), hd, s->L.total, cudaMemcpyHostToDevice, g.stream) == cudaSuccess;
         if (cudaStreamSynchronize(g.stream) != cudaSuccess) ok = false;
@@ -1138,7 +1187,10 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
     if (!s) return nullptr;
     s->n_containers = nc;
     s->slab_used = slab_total;
+    // a portable blob's payload is its containers' container_size_in_bytes; a frozen blob stores run
+    // containers without their 2-byte run count, so its sum is taken from the directory when asked
     s->portable_bytes = payload;
+    s->portable_known = !frozen;
     // per-bitmap tables: [roff | rlen | slab_base] for the kernels, bm_beg / bm_cnt into the directory
     PinBlock<uint64_t> tab(3 * n);
     PinBlock<uint32_t> bc(2 * n);
@@ -1231,7 +1283,10 @@ uint64_t rb200_set_container_count(const rb200_set_t *s) {
     resolve(s);
     return s->n_containers;
 }
-uint64_t rb200_set_payload_bytes(const rb200_set_t *s) { return s->portable_bytes; }
+uint64_t rb200_set_payload_bytes(const rb200_set_t *s) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    return payload_bytes_of(s);
+}
 
 }  // extern "C"
 
@@ -1887,7 +1942,7 @@ static rb200_set *or_many_impl(const rb200_set_t *S, const uint32_t *idx, size_t
         // output term is added by the caller-visible stat only when the set is downloaded,
         // here we account inputs exactly from the host mirrors when the whole key space is used.
         uint64_t inb = 0;
-        if (key_lo == 0 && key_hi == 65535 && sel.all()) inb = S->portable_bytes;
+        if (key_lo == 0 && key_hi == 65535 && sel.all()) inb = payload_bytes_of(S);
         g.last_algo_bytes = inb;
     }
     ev_put(evc0);
@@ -1988,7 +2043,7 @@ rb200_set_t *rb200_xor_many(const rb200_set_t *S, const uint32_t *idx, size_t n)
         for (size_t k = 0; k < live_after.size(); k++) live_after[k] = live += h_live.get()[k];
         const uint8_t cow = mixed ? sel.fold_cow([&](size_t k) { return live_after[k - 1] == 0; }) : sel.n ? sel.cow(0) : 0;
         fill_single_result(R.get(), (uint32_t)g.h_stats->dir_cursor, (uint64_t)g.h_stats->nk * BITSET_BYTES, cow);
-        g.last_algo_bytes = sel.all() ? S->portable_bytes : 0;
+        g.last_algo_bytes = sel.all() ? payload_bytes_of(S) : 0;
     }
     return ok ? R.release() : nullptr;
 }
@@ -3081,6 +3136,7 @@ static rb200_set *from_uint32_impl(const ValueLists<uint32_t> &lists) {
     s->n_containers = nc;
     s->slab_used = g.h_stats->slab_cursor;
     s->portable_bytes = g.h_stats->payload_bytes;
+    s->portable_known = true;
     s->mirrors_pending = n > 0;   // containers / bytes / effective bytes per bitmap: k_deser_bitmap_cards wrote them
     return s.release();
 }
