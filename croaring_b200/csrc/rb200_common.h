@@ -172,8 +172,10 @@ struct OpStats {
     unsigned long long work_counter;  // dynamic scheduler for the compute kernel
     unsigned long long work_counter2;
     unsigned long long out_portable;  // sum over result bitmaps of roaring_bitmap_portable_size_in_bytes
-    unsigned int error;               // 0 = ok; 1 = slot overflow; 2 = slab overflow; 3 = malformed blob
-    unsigned int nk;                  // or_many: number of distinct keys
+    unsigned int error;               // 0 = ok; 1 = slot overflow; 2 = slab overflow; 3 = malformed blob;
+                                      // 4 = a blob's container contents fail validation
+    unsigned int nk;                  // or_many: number of distinct keys; deserialization (errors 3, 4):
+                                      // nb - the index of the first malformed blob
     unsigned int units;               // or_many: number of (key, slice) work units
     unsigned int cls_count[8];        // pairwise ops: live work items per code-path class
     unsigned int cls_cursor[8];       //               fill cursors of k_order_items

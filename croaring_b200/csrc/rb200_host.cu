@@ -1143,7 +1143,8 @@ rb200_set_t *rb200_set_upload(const roaring_bitmap_t *const *bitmaps, size_t n) 
 // Portable-serialized inputs are parsed ON THE DEVICE (src/roaring_array.c:633-813 restated as
 // k_deser_dir / k_deser_copy): the host only reads each blob's cookie (to size the directory) and
 // streams the raw bytes through pinned staging chunks; no per-container host work.
-static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens, size_t n, bool frozen);
+static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens, size_t n, bool frozen,
+                                    size_t *bad_blob = nullptr);
 rb200_set_t *rb200_set_upload_serialized(const char *const *bufs, const size_t *lens, size_t n) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return upload_blobs_impl(bufs, lens, n, false);
@@ -1154,7 +1155,10 @@ rb200_set_t *rb200_set_upload_frozen(const char *const *bufs, const size_t *lens
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return upload_blobs_impl(bufs, lens, n, true);
 }
-static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens, size_t n, bool frozen) {
+// A malformed blob is named in t_err and, when bad_blob is given, its index is stored there.
+static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens, size_t n, bool frozen,
+                                    size_t *bad_blob) {
+    const char *what = frozen ? "malformed frozen bitmap at index " : "malformed portable bitmap at index ";
     if (!ctx_init()) return nullptr;
     if (n > 0xffffffffull) { t_err = "too many bitmaps"; return nullptr; }
     // pass 1 (host): container count of every blob from its cookie; staging offsets
@@ -1173,7 +1177,8 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
             ok = portable_count((const uint8_t *)bufs[i], lens[i], size, hasrun);
         }
         if (!ok) {
-            t_err = std::string(frozen ? "malformed frozen bitmap at index " : "malformed portable bitmap at index ") + std::to_string(i);
+            t_err = what + std::to_string(i);
+            if (bad_blob) *bad_blob = i;
             return nullptr;
         }
         cnt[i] = size;
@@ -1235,13 +1240,15 @@ static rb200_set *upload_blobs_impl(const char *const *bufs, const size_t *lens,
             launch_deserialize(d_raw.get(), t, t + n, t + 2 * n, (uint32_t)n, nc, s->out(), d_src.get(), g.d_stats,
                                g.stream);
         ok = call.finish(ok);
-        if (ok && g.h_stats->error == 4u) {
-            t_err = "malformed serialized bitmap: invalid container contents (a run ends past 65535, runs "
-                    "overlap or are out of order, or array values are not strictly increasing)";
-            ok = false;
-        } else if (ok && g.h_stats->error) {
-            t_err = std::string(frozen ? "malformed frozen bitmap at index " : "malformed portable bitmap at index ") +
-                    std::to_string((uint64_t)n - g.h_stats->nk);
+        if (ok && g.h_stats->error) {   // 3: structure (k_deser_dir / k_frozen_parse_dir), 4: contents (k_deser_copy)
+            const size_t bad = (size_t)n - g.h_stats->nk;
+            t_err = what + std::to_string(bad);
+            if (g.h_stats->error == 4u)
+                t_err += ": invalid container contents (the reference's validator refuses them: runs that are "
+                         "empty, end past 65535, overlap, touch or are out of order; an array above 4096 values "
+                         "or not strictly increasing; a bitset whose cardinality is not its popcount or is 4096 "
+                         "or less)";
+            if (bad_blob) *bad_blob = bad;
             ok = false;
         }
     }
@@ -3973,7 +3980,14 @@ rb200_set64 *set64_upload_impl(const char *const *bufs, const size_t *lens, size
         bc[i] = cnt[i];
     }
     memcpy(beg + 2 * n, highs.data(), 4 * highs.size());
-    s->inner.reset(upload_blobs_impl(ptrs.data(), blens.data(), ptrs.size(), false));
+    size_t bad = SIZE_MAX;
+    s->inner.reset(upload_blobs_impl(ptrs.data(), blens.data(), ptrs.size(), false, &bad));
+    if (!s->inner && bad < ptrs.size() - 1) {   // the device refused a bucket: name its 64-bit bitmap
+        const size_t i = std::upper_bound(beg, beg + n, (uint32_t)bad) - beg - 1;
+        const size_t why = t_err.find(": ");
+        t_err = "malformed 64-bit portable bitmap at index " + std::to_string((uint64_t)i) + ": the bucket of high 32 bits " +
+                std::to_string(highs[bad]) + (why == std::string::npos ? std::string(" is malformed") : t_err.substr(why));
+    }
     return s->inner ? s.release() : nullptr;
 }
 

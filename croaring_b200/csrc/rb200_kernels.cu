@@ -1038,8 +1038,19 @@ k_deser_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ roff,
     }
 }
 
+// The bitmap of nb that holds directory entry c: the last b with bm_beg[b] <= c (empty bitmaps share
+// their bm_beg with the next one, so the last such b is the one that owns c).
+__device__ __forceinline__ uint32_t bitmap_of(const uint32_t *__restrict__ bm_beg, uint32_t nb, uint64_t c) {
+    uint32_t lo = 0, hi = nb;   // bm_beg[lo] <= c < bm_beg[hi]
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (bm_beg[mid] <= c) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 __global__ void __launch_bounds__(128)
-k_deser_copy(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ src_pos, uint64_t nc,
+k_deser_copy(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ src_pos, uint64_t nc, uint32_t nb,
              SetOut out, OpStats *st) {
     if (st->error == 3u) return;  // a malformed blob leaves directory entries unwritten: nothing to move
     const int lane = threadIdx.x & 31;
@@ -1054,10 +1065,11 @@ k_deser_copy(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ src_p
         warp_copy_unaligned(dst, src, n, lane);
         const uint32_t pad = round16(n) - n;
         if ((uint32_t)lane < pad) dst[n + lane] = 0;
-        // Container CONTENTS of an untrusted blob (the device-side counterpart of the payload checks of
-        // roaring_bitmap_internal_validate, src/containers/run.c:693-713, array.c:469-487): the
-        // kernels rasterise runs and index by array values without further checks, so a run that
-        // ends past 65535 or unsorted data must never reach them.
+        // Container CONTENTS of an untrusted blob: what roaring_bitmap_internal_validate checks of each
+        // container (src/containers/run.c:669-713, array.c:456-487, bitset.c:1023-1042), so the device
+        // holds exactly the containers the reference's validator accepts.  The kernels rasterise runs
+        // and index by array values without further checks, and take c_card as exact (prefix sums,
+        // select, slot bounds, the type rules): nothing else may reach them.
         bool bad = false;
         if (t == T_RUN) {  // run_container_cardinality (run.c:1077) + bounds / order of the runs
             uint32_t card = 0;
@@ -1066,15 +1078,28 @@ k_deser_copy(const uint8_t *__restrict__ raw, const uint64_t *__restrict__ src_p
                 const uint32_t s0 = ld_u16(src + 4 * k), l0 = ld_u16(src + 4 * k + 2);
                 card += l0 + 1u;
                 if (s0 + l0 > 65535u) bad = true;
-                if (k > 0 && s0 <= ld_u16(src + 4 * k - 4) + ld_u16(src + 4 * k - 2)) bad = true;
+                // after the previous run's end + 1: neither overlapping nor adjacent (those combine)
+                if (k > 0 && s0 <= ld_u16(src + 4 * k - 4) + ld_u16(src + 4 * k - 2) + 1u) bad = true;
             }
             card = __reduce_add_sync(FULLMASK, card);
             if (lane == 0) out.c_card[c] = card;
-        } else if (t == T_ARRAY) {  // strictly increasing values
-            for (uint32_t k = lane + 1; k < len; k += 32)
+        } else if (t == T_ARRAY) {  // at most 4096 (only a frozen blob can say more) strictly increasing values
+            bad = len > (uint32_t)MAX_ARRAY;
+            for (uint32_t k = lane + 1; k < len && !bad; k += 32)
                 if (ld_u16(src + 2 * k) <= ld_u16(src + 2 * k - 2)) bad = true;
+        } else {  // the header's cardinality is the popcount, and above 4096 (a frozen blob may say less)
+            __syncwarp();
+            const uint64_t *w = (const uint64_t *)dst;
+            uint32_t pop = 0;
+            for (uint32_t k = lane; k < 1024u; k += 32) pop += __popcll(w[k]);
+            pop = __reduce_add_sync(FULLMASK, pop);
+            const uint32_t card = out.c_card[c];
+            bad = pop != card || card <= (uint32_t)MAX_ARRAY;
         }
-        if (__any_sync(FULLMASK, bad) && lane == 0) atomicCAS(&st->error, 0u, 4u);
+        if (__any_sync(FULLMASK, bad) && lane == 0) {  // error 4, and the first such blob as report_malformed names it
+            atomicCAS(&st->error, 0u, 4u);
+            atomicMax(&st->nk, nb - bitmap_of(out.bm_beg, nb, c));
+        }
     }
 }
 
@@ -1278,7 +1303,7 @@ k_frozen_parse_dir(const uint8_t *__restrict__ raw, const uint64_t *__restrict__
 // the directory parse (k_deser_dir / k_frozen_parse_dir), then the payload moves and the bitmap figures
 static void deserialize_tail(const uint8_t *raw, uint32_t nb, uint64_t nc, SetOut out, uint64_t *src_pos, OpStats *st,
                              cudaStream_t s) {
-    if (nc) launch_kernel(k_deser_copy, grid_for(nc, 4, 16), 128, 0, s, raw, src_pos, nc, out, st);
+    if (nc) launch_kernel(k_deser_copy, grid_for(nc, 4, 16), 128, 0, s, raw, src_pos, nc, nb, out, st);
     launch_kernel(k_deser_bitmap_cards, grid_for(nb, 4, 16), 128, 0, s, out, nb, st);
 }
 

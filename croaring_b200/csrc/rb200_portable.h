@@ -18,7 +18,8 @@ struct PortableEntry {
     uint16_t key;
     uint8_t type;
     uint32_t card;   // cardinality (written as card - 1; CARD_UNKNOWN is ignored).  Read: as the header
-                     // states it, which for a run container nothing checks
+                     // states it, except a run container's: the reference ignores that field and
+                     // writes the count of its runs, so the walk counts them too
     uint32_t len;
     const uint8_t *payload;
 };
@@ -82,6 +83,11 @@ size_t walk_portable(const uint8_t *buf, size_t len, F &&fn) {
         if (pos + sb > len) return 0;
         e.payload = buf + pos;
         pos += sb;
+        if (e.type == T_RUN) {
+            e.card = 0;
+            for (uint32_t k = 0; k < e.len; k++)
+                e.card += ((uint32_t)e.payload[4 * k + 2] | ((uint32_t)e.payload[4 * k + 3] << 8)) + 1u;
+        }
         fn(e);
     }
     return pos;

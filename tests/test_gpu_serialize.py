@@ -114,7 +114,7 @@ def test_device_deserialize_rejects_malformed(rb, R):
     for name, blob in content_cases.items():
         with pytest.raises(rb.RB200Error) as ei:
             rb.DeviceSet.from_serialized(good[:2] + [blob] + good[4:])
-        assert "invalid container contents" in str(ei.value), (name, str(ei.value))
+        assert "malformed portable bitmap at index 2: invalid container contents" in str(ei.value), (name, str(ei.value))
     # the library keeps working afterwards
     assert rb.DeviceSet.from_serialized(good).serialize_all() == good
 
@@ -149,8 +149,9 @@ def test_frozen_format_both_ways(rb, R):
     F = rb.DeviceSet.from_frozen(exp)
     assert F.serialize_all() == blobs
     assert F.cardinalities().tolist() == S.cardinalities().tolist()
-    for name, bad in {"truncated": exp[3][:-9], "cookie": exp[3][:-4] + b"\\x00\\x00\\x00\\x00",
-                      "length": exp[3][:100] + b"\\x00\\x00" + exp[3][100:]}.items():
+    for name, bad in {"truncated": exp[3][:-9], "cookie": exp[3][:-4] + b"\x00\x00\x00\x00",
+                      "cookie bit": exp[3][:-4] + bytes([exp[3][-4] ^ 0x01]) + exp[3][-3:],
+                      "length": exp[3][:100] + b"\x00\x00" + exp[3][100:]}.items():
         with pytest.raises(rb.RB200Error) as ei:
             rb.DeviceSet.from_frozen(exp[:2] + [bad] + exp[4:6])
         assert "malformed frozen bitmap at index 2" in str(ei.value), (name, str(ei.value))

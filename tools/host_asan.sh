@@ -20,4 +20,4 @@ nvcc -shared -cudart static -o "$OUT/libroaring_b200_asan.so" "$OUT/rb200_host.o
 cd "$ROOT"
 export RB200_LIB="$OUT/libroaring_b200_asan.so" ASAN_OPTIONS=detect_leaks=0 UBSAN_OPTIONS=print_stacktrace=1
 export LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)"
-python -m pytest tests/test_host_abi.py tests/test_set64_host.py tests/test_portable_codec.py tests/test_sharding_gloo.py -q -k "not world2 and not exports and not type_rules and not index_formats" 2>&1 | tail -n 4
+python -m pytest tests/test_host_abi.py tests/test_set64_host.py tests/test_portable_codec.py tests/test_sharding_gloo.py tests/test_malformed_host.py -q -k "not world2 and not exports and not type_rules and not index_formats" 2>&1 | tail -n 4
