@@ -170,6 +170,8 @@ def lib():
     sig("rb200_set64_batch_add_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
     sig("rb200_set64_batch_remove_range_closed", _P, _P, _P, C.c_size_t, _P, _P)
     sig("rb200_set64_run_optimize", _P, _P, C.c_int)
+    sig("rb200_set64_batch_query", C.c_int, C.c_int, _P, _P, C.c_size_t, _P, _P, _P)
+    sig("rb200_set64_batch_query_device", C.c_int, C.c_int, _P, _P, C.c_size_t, _P, _P, _P)
     sig("rb200_set64_serialize", C.c_int, _P, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint64)),
         C.POINTER(C.POINTER(C.c_uint64)))
     sig("rb200_set64_download_all", C.c_int, _P, _P)
@@ -705,20 +707,26 @@ def _device_u32(t, what):
     return t
 
 
-def _query_device(s, code, values, idx):
+def _device_index(idx, n, n_all, dev):
+    """The bitmap of every query of n device values, as _query_index takes it, on the device dev: None or a
+    contiguous int32 / uint32 tensor of n entries."""
     import torch
-    values = _device_u32(values, "values")
-    dev, n = values.device, values.numel()
     if isinstance(idx, torch.Tensor):
         ia = _device_u32(idx.to(dev), "idx")
         if ia.numel() != n:
             raise RB200Error(f"idx has {ia.numel()} entries for {n} values")
-    else:
-        ia = _query_index(idx, n, len(s))
-        if isinstance(ia, int):   # expanded on the values' device, as the int32 of the same bits
-            ia = torch.full((n,), ia - (1 << 32) if ia >= 1 << 31 else ia, dtype=torch.int32, device=dev)
-        elif ia is not None:
-            ia = torch.from_numpy(ia.view(np.int32)).to(dev)
+        return ia
+    ia = _query_index(idx, n, n_all)
+    if isinstance(ia, int):   # expanded on the values' device, as the int32 of the same bits
+        return torch.full((n,), ia - (1 << 32) if ia >= 1 << 31 else ia, dtype=torch.int32, device=dev)
+    return None if ia is None else torch.from_numpy(ia.view(np.int32)).to(dev)
+
+
+def _query_device(s, code, values, idx):
+    import torch
+    values = _device_u32(values, "values")
+    dev, n = values.device, values.numel()
+    ia = _device_index(idx, n, len(s), dev)
     out = torch.empty(n, dtype=torch.int64, device=dev)
     if ia is not None and not n:
         return out   # (an empty tensor's address is NULL, which the library reads as one query per bitmap)
@@ -1030,12 +1038,58 @@ class DeviceSet:
 
 def _values_u64(a):
     """1-D integer values as a contiguous uint64 array (refused if any lies outside [0, 2^64))."""
+    if isinstance(a, (list, tuple)) and np.asarray(a).dtype.kind not in "iu":
+        # Python ints past 2^63 next to others, which numpy reads as floats
+        if not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in a):
+            raise RB200Error("values must be 1-D integer arrays")
+        if any(not 0 <= int(v) < 1 << 64 for v in a):
+            raise RB200Error("values must lie in [0, 2^64)")
+        return np.array([int(v) for v in a], dtype=np.uint64)
     a = np.asarray(a)
     if a.ndim != 1 or (a.size and a.dtype.kind not in "iu"):
         raise RB200Error(f"values must be 1-D integer arrays, got {a.dtype} with shape {a.shape}")
     if a.size and a.dtype.kind == "i" and int(a.min()) < 0:
         raise RB200Error("values must lie in [0, 2^64)")
     return np.ascontiguousarray(a, dtype=np.uint64)
+
+
+def _query64(s, kind, values, idx):
+    """(out, found) of rb200_set64_batch_query: out[k] (uint64) the answer of 64-bit bitmap idx[k] of the set s
+    about values[k], found[k] (bool) the reference's return.  CUDA tensor values go through
+    rb200_set64_batch_query_device, and both stay on their device."""
+    if kind not in QUERIES:
+        raise RB200Error(f"unknown query kind {kind!r}: one of {sorted(QUERIES)}")
+    if getattr(values, "is_cuda", False):
+        return _query64_device(s, QUERIES[kind], values, idx)
+    vals = _values_u64(values)
+    ia = _query_index(idx, vals.size, len(s))
+    out, found = np.empty(vals.size, dtype=np.uint64), np.empty(vals.size, dtype=np.bool_)
+    if ia is not None and not vals.size:
+        return out, found   # (the library reads a NULL idx as one query per bitmap)
+    if isinstance(ia, int):
+        ia = np.full(vals.size, ia, dtype=np.uint32)
+    if lib().rb200_set64_batch_query(QUERIES[kind], s.ptr, None if ia is None else ia.ctypes.data, vals.size,
+                                     vals.ctypes.data, out.ctypes.data, found.ctypes.data) != 0:
+        raise RB200Error(last_error())
+    return out, found
+
+
+def _query64_device(s, code, values, idx):
+    import torch
+    if values.dtype not in (torch.int64, torch.uint64) or values.dim() != 1 or not values.is_contiguous():
+        raise RB200Error("device values must be a contiguous 1-D int64 / uint64 CUDA tensor")
+    dev, n = values.device, values.numel()
+    ia = _device_index(idx, n, len(s), dev)
+    out = torch.empty(n, dtype=values.dtype, device=dev)   # the u64 answers, as the values' dtype of the same bits
+    found = torch.empty(n, dtype=torch.bool, device=dev)
+    if ia is not None and not n:
+        return out, found   # (an empty tensor's address is NULL, which the library reads as one query per bitmap)
+    # the library stream reads and writes these: what torch's stream queued on them comes first
+    torch.cuda.current_stream(dev).synchronize()
+    if lib().rb200_set64_batch_query_device(code, s.ptr, None if ia is None else ia.data_ptr(), n, values.data_ptr(),
+                                            out.data_ptr(), found.data_ptr()) != 0:
+        raise RB200Error(last_error())
+    return out, found
 
 
 def _serialized(fn, ptr, n):
@@ -1130,6 +1184,28 @@ class DeviceSet64:
     def run_optimize(self, mode=1):
         """mode 1: roaring64_bitmap_run_optimize of every bitmap; mode 0: the run containers removed."""
         return DeviceSet64(lib().rb200_set64_run_optimize(self.ptr, int(mode)))
+
+    # -- point queries, with the selections of DeviceSet's: idx None asks bitmap k (one value per bitmap), an
+    # array gives one bitmap per value, a scalar asks every value of one bitmap.  Host values (arrays, lists)
+    # give numpy arrays; a CUDA tensor of int64 / uint64 values (read in place on the library stream) gives
+    # tensors on its device, the answers in the values' dtype (the same bits as uint64) and found as torch.bool.
+    def contains(self, values, idx=None):
+        """roaring64_bitmap_contains per query: a bool array."""
+        return _query64(self, "contains", values, idx)[1]
+
+    def rank(self, values, idx=None):
+        """roaring64_bitmap_rank per query: the number of values <= values[k], a uint64 array."""
+        return _query64(self, "rank", values, idx)[0]
+
+    def get_index(self, values, idx=None):
+        """roaring64_bitmap_get_index per query: (the index of values[k] in its bitmap, found); a miss gives
+        2^64 - 1 and found False."""
+        return _query64(self, "get_index", values, idx)
+
+    def select(self, ranks, idx=None):
+        """roaring64_bitmap_select per query: (the value of 0-based rank ranks[k], found); a rank past the
+        cardinality gives 2^64 - 1 and found False, which tells it from the value 2^64 - 1."""
+        return _query64(self, "select", ranks, idx)
 
     def serialize_all(self):
         """roaring64_bitmap_portable_serialize bytes of every bitmap, written on the device, one D2H."""

@@ -467,5 +467,17 @@ constexpr int Q_CONTAINS = 0, Q_RANK = 1, Q_GET_INDEX = 2, Q_SELECT = 3;
 void launch_query(int kind, const SetView &S, const uint64_t *c_cum, uint32_t n_bitmaps, const uint32_t *idx,
                   const uint32_t *vals, uint32_t n, int64_t *out, unsigned long long *bad, cudaStream_t s);
 void launch_query_cards(const uint32_t *c_card, uint64_t nc, uint64_t *out, cudaStream_t s);
+// The same against a set of n64 64-bit bitmaps whose buckets are the bitmaps of the inner set S (bitmap b:
+// buckets [b_beg[b], b_beg[b] + b_cnt[b]), bucket j holding high[j] << 32 | its inner values).  out[k]: the
+// u64 answer, 2^64 - 1 for a get_index / select miss and an idx[k] >= n64; found (null: not written): 1 for
+// a rank, the answer of a contains, 0 on a miss.  b_cum: the exclusive scan of what launch_query64_cards
+// writes (the values of every bucket, nb + 1 entries, the last zero); c_cum and b_cum are null for
+// Q_CONTAINS.
+void launch_query64(int kind, const SetView &S, const uint64_t *c_cum, const uint64_t *b_cum, const uint32_t *b_beg,
+                    const uint32_t *b_cnt, const uint32_t *high, uint32_t n64, const uint32_t *idx,
+                    const uint64_t *vals, uint32_t n, uint64_t *out, uint8_t *found, unsigned long long *bad,
+                    cudaStream_t s);
+void launch_query64_cards(const uint32_t *bm_beg, const uint32_t *bm_cnt, const uint64_t *c_cum, uint64_t nb,
+                          uint64_t *out, cudaStream_t s);
 
 }  // namespace rb200

@@ -3889,6 +3889,9 @@ struct rb200_set64 {
     DevBlock<uint32_t> d_dir;       // the same in device memory (copied there when a kernel first needs it)
     bool dir_on_device = false;
     size_t dir_bytes = 0;
+    // exclusive scan of the buckets' cardinalities (nbuckets + 1 entries), built by the first rank /
+    // get_index / select query (ensure_bcum)
+    DevBlock<uint64_t> b_cum;
     const uint32_t *b_beg() const { return h_dir.get(); }
     const uint32_t *b_cnt() const { return h_dir.get() + n; }
     const uint32_t *high() const { return h_dir.get() + 2 * (size_t)n; }
@@ -4294,6 +4297,47 @@ extern "C++" rb200_set64 *range64_impl(bool add, const std::string &what, const 
     R->inner.reset(range_impl(add, what, S->inner.get(), ib.data(), ib.size(), lo.data(), hi.data()));
     return R->inner ? R.release() : nullptr;
 }
+
+// ---- point queries: roaring64_bitmap_contains / rank / get_index / select (roaring64.c:682, 804, 827, 779) ----
+// out[k] = the answer of 64-bit bitmap S[idx[k]] about vals[k], a warp per query (k_query64): the bucket of
+// the value's high 32 bits (select: of the rank) in the bitmap's run of inner bitmaps, then the 32-bit answer
+// in that inner bitmap.  rank, get_index and select add the cardinalities of the buckets before it; they
+// come from the set's b_cum, built once by the first such query from the inner set's c_cum.
+
+// The set's b_cum (and the inner c_cum) on the library stream, unless it is there already.
+bool ensure_bcum(const rb200_set64 *cs) {
+    rb200_set64 *s = const_cast<rb200_set64 *>(cs);
+    if (s->b_cum) return true;
+    if (!ensure_cum(s->inner.get())) return false;
+    const uint64_t nb = s->nbuckets;
+    if (nb >= 0x7fffffffull) { t_err = "set64_query: more than 2^31 - 2 buckets in the set"; return false; }
+    DevBlock<uint64_t> cards(nb + 1), cum(nb + 1);
+    DevBlock<uint8_t> temp;
+    size_t tb = 0;
+    if (!cards || !cum) return false;
+    if (!build_scan(nullptr, &tb, cards.get(), cum.get(), nb + 1, g.stream) || !temp.reset(tb)) {
+        if (t_err.empty()) t_err = "set64_query: scan setup failed";
+        return false;
+    }
+    const SetView v = s->inner->view();
+    launch_query64_cards(v.bm_beg, v.bm_cnt, s->inner->c_cum.get(), nb, cards.get(), g.stream);
+    if (!build_scan(temp.get(), &tb, cards.get(), cum.get(), nb + 1, g.stream)) {
+        t_err = "set64_query: scan launch failed";
+        return false;
+    }
+    s->b_cum = std::move(cum);   // cards and temp go back to the pool: stream-ordered reuse
+    return true;
+}
+bool query64_enqueue(int kind, const rb200_set64 *S, const uint32_t *d_idx, size_t n, const uint64_t *d_vals,
+                     uint64_t *d_out, uint8_t *d_found, unsigned long long *d_bad) {
+    // an uploaded set has only the host copy of its directory
+    if (!set64_dir_on_device(S) || (kind != Q_CONTAINS && !ensure_bcum(S))) return false;
+    const rb200_set *I = S->inner.get();
+    const uint32_t *beg = S->d_dir.get(), *cnt = beg + S->n, *high = beg + 2 * (size_t)S->n;
+    launch_query64(kind, I->view(), I->c_cum.get(), S->b_cum.get(), beg, cnt, high, S->n, d_idx, d_vals, (uint32_t)n,
+                   d_out, d_found, d_bad, g.stream);
+    return true;
+}
 }  // namespace
 
 rb200_set64_t *rb200_set64_upload_serialized(const char *const *bufs, const size_t *lens, size_t n) {
@@ -4399,6 +4443,74 @@ rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *S, int mode) {
 int rb200_set64_serialize(const rb200_set64_t *s, char **buf, uint64_t **off, uint64_t **len) {
     std::lock_guard<std::recursive_mutex> lk(g.mu);
     return serialize64_impl(s, buf, off, len);
+}
+
+int rb200_set64_batch_query(int kind, const rb200_set64_t *S, const uint32_t *idx, size_t n, const uint64_t *vals,
+                            uint64_t *out, uint8_t *found) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    SelectionOf<rb200_set64> sel{S, idx, n};
+    if (!sel.check("set64_query") || !query_args("set64_query", kind, sel.n, vals, out)) return -1;   // before any CUDA call
+    if (!ctx_init() || !ensure_mirrors(S->inner.get())) return -1;   // a failed batch op fails here, not as data
+    n = sel.n;
+    if (!n) return 0;
+    // one block each way: [first bad position | idx | vals] up, [out | found] down
+    const size_t o_idx = al256(8), o_vals = o_idx + (sel.all() ? 0 : al256(4 * n)), o_out = o_vals + al256(8 * n);
+    const size_t o_found = o_out + 8 * n, bytes = o_found + n;
+    PinBlock<uint8_t> h(bytes);
+    DevBlock<uint8_t> d(bytes);
+    if (!h || !d) return -1;
+    memset(h.get(), 0xff, 8);
+    if (!sel.all()) memcpy(h.get() + o_idx, idx, 4 * n);
+    memcpy(h.get() + o_vals, vals, 8 * n);
+    SyncCall call("set64_query", "set64_query launch");
+    bool ok = cudaMemcpyAsync(d.get(), h.get(), o_out, cudaMemcpyHostToDevice, g.stream) == cudaSuccess &&
+              query64_enqueue(kind, S, sel.all() ? nullptr : (const uint32_t *)(d.get() + o_idx), n,
+                              (const uint64_t *)(d.get() + o_vals), (uint64_t *)(d.get() + o_out), d.get() + o_found,
+                              (unsigned long long *)d.get()) &&
+              cudaMemcpyAsync(h.get() + o_out, d.get() + o_out, 9 * n, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    ok = call.finish(ok, false);
+    if (ok) {
+        memcpy(out, h.get() + o_out, 8 * n);
+        if (found) memcpy(found, h.get() + o_found, n);
+    }
+    return ok ? 0 : -1;
+}
+
+int rb200_set64_batch_query_device(int kind, const rb200_set64_t *S, const uint32_t *d_idx, size_t n,
+                                   const uint64_t *d_vals, uint64_t *d_out, uint8_t *d_found) {
+    std::lock_guard<std::recursive_mutex> lk(g.mu);
+    SelectionOf<rb200_set64> sel{S, nullptr, n};
+    if (!sel.check("set64_query_device")) return -1;   // the entries of d_idx are checked by the kernel
+    if (d_idx) {
+        if (n > 0xffffffffull) { t_err = "set64_query_device: more than 2^32 - 1 queries"; return -1; }
+        sel.n = n;
+    }
+    n = sel.n;
+    if (!query_args("set64_query_device", kind, n, d_vals, d_out) || !ctx_init()) return -1;
+    // a host pointer never reaches the kernel
+    const char *what = "set64_query_device";
+    if (n && (!device_memory(what, "vals", d_vals) || !device_memory(what, "out", d_out) ||
+              (d_idx && !device_memory(what, "idx", d_idx)) || (d_found && !device_memory(what, "found", d_found))))
+        return -1;
+    if (!ensure_mirrors(S->inner.get())) return -1;
+    if (!n) return 0;
+    DevBlock<unsigned long long> d_bad(1);
+    PinBlock<unsigned long long> h_bad(1);
+    if (!d_bad || !h_bad) return -1;
+    SyncCall call(what, "set64_query_device launch");
+    bool ok = cudaMemsetAsync(d_bad.get(), 0xff, 8, g.stream) == cudaSuccess &&
+              query64_enqueue(kind, S, d_idx, n, d_vals, d_out, d_found, d_bad.get()) &&
+              cudaMemcpyAsync(h_bad.get(), d_bad.get(), 8, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess;
+    ok = call.finish(ok, false);
+    if (ok && *h_bad.get() != ~0ull) {   // the first out-of-range entry, reported as the host check does
+        const uint64_t k = *h_bad.get();
+        uint32_t v = 0;
+        if (cudaMemcpyAsync(&v, d_idx + k, 4, cudaMemcpyDeviceToHost, g.stream) == cudaSuccess)
+            cudaStreamSynchronize(g.stream);
+        index_error(what, k, v, S->n);
+        ok = false;
+    }
+    return ok ? 0 : -1;
 }
 
 // result[k] = roaring64 op of (a[ia[k]], b[ib[k]]), all in the 64-bit portable format.  *out is

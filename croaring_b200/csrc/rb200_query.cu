@@ -13,11 +13,19 @@
 // Inside bitmap b the values before container c number c_cum[c] - c_cum[bm_beg[b]] (u64, modular:
 // only entries inside the bitmap enter the difference), so no count is ever held in 32 bits.
 //
+// 64-bit sets: a 64-bit bitmap is a run of inner bitmaps, one per high-32 bucket.
+//   k_query64_cards  the values of every inner bitmap from the inner c_cum, the input of the set's b_cum
+//                    scan (exclusive, nbuckets + 1 entries; built once per set by the host)
+//   k_query64<KIND>  warp per query: the bucket by a 32-ary search of the bitmap's highs (SELECT: of its
+//                    b_cum range), then answer<KIND> on that inner bitmap, plus the buckets before it
+//
 // Reference semantics restated here (file:line relative to /root/reference):
 //   roaring_bitmap_contains    include/roaring/roaring.h:478
 //   roaring_bitmap_rank        src/roaring.c:2862 (values <= x)
 //   roaring_bitmap_get_index   src/roaring.c:2916 (-1 when x is absent)
 //   roaring_bitmap_select      src/roaring.c:2974 (0-based rank; false -> -1 here)
+//   roaring64_bitmap_contains / rank / get_index / select   src/roaring64.c:682, 804, 827, 779 (a false
+//                              return is found = 0, with the answer 2^64 - 1)
 #include "rb200_device.cuh"
 
 namespace rb200 {
@@ -205,6 +213,73 @@ k_query_cards(const uint32_t *__restrict__ c_card, uint64_t nc, uint64_t *__rest
         out[c] = c < nc ? (uint64_t)(c_card[c] & CARD_MASK) : 0ull;
 }
 
+// The answer about x of the 64-bit bitmap whose buckets are [beg, beg + cnt) of the inner set (bucket j
+// holding the values high[j] << 32 | v of the inner bitmap j): the bucket by a 32-ary search of the highs (SELECT:
+// of the bucket prefix b_cum), then answer<KIND> inside it.  Empty buckets (results of x XOR x, of a
+// removal) hold no container: contains and rank find nothing in them and their b_cum step is 0, so
+// select never stops on one.  r: the answer, left as it is on a get_index or select miss, which returns
+// false; contains returns its answer, rank true.
+template <int KIND>
+__device__ __forceinline__ bool answer64(const SetView &S, const uint64_t *c_cum, const uint64_t *b_cum,
+                                         const uint32_t *high, uint32_t beg, uint32_t cnt, uint64_t x, int lane,
+                                         uint64_t &r) {
+    if (KIND == Q_SELECT) {
+        const uint64_t base = b_cum[beg];
+        if (x >= b_cum[beg + cnt] - base) return false;
+        const uint32_t i = warp_partition(cnt, lane, [&](uint32_t j) { return b_cum[beg + j + 1] - base <= x; });
+        // a bucket holds at most 2^32 values, so the rank inside it fits 32 bits
+        const int64_t lo = answer<Q_SELECT>(S, c_cum, beg + i, (uint32_t)(x - (b_cum[beg + i] - base)), lane);
+        r = (uint64_t)high[beg + i] << 32 | (uint32_t)lo;
+        return true;
+    }
+    const uint32_t hx = (uint32_t)(x >> 32);
+    const uint32_t i = warp_partition(cnt, lane, [&](uint32_t j) { return high[beg + j] < hx; });
+    const bool present = i < cnt && high[beg + i] == hx;
+    if (KIND == Q_CONTAINS) {
+        r = present ? (uint64_t)answer<Q_CONTAINS>(S, c_cum, beg + i, (uint32_t)x, lane) : 0ull;
+        return r != 0;
+    }
+    if (KIND == Q_GET_INDEX && !present) return false;
+    const int64_t in = present ? answer<KIND>(S, c_cum, beg + i, (uint32_t)x, lane) : 0;
+    if (in < 0) return false;   // get_index: x's bucket is there, x is not
+    r = b_cum[beg + i] - b_cum[beg] + (uint64_t)in;   // (read after the inner answer: fewer live registers)
+    return true;
+}
+
+// (256, 6): at most 42 registers, where ptxas's own choice of 32 for (256) spills the get_index path
+template <int KIND>
+__global__ void __launch_bounds__(256, 6)
+k_query64(SetView S, const uint64_t *__restrict__ c_cum, const uint64_t *__restrict__ b_cum,
+          const uint32_t *__restrict__ b_beg, const uint32_t *__restrict__ b_cnt, const uint32_t *__restrict__ high,
+          uint32_t n64, const uint32_t *__restrict__ idx, const uint64_t *__restrict__ vals, uint32_t n,
+          uint64_t *__restrict__ out, uint8_t *__restrict__ found, unsigned long long *bad) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t nwarps = (gridDim.x * (uint64_t)blockDim.x) >> 5;
+    for (uint64_t q = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; q < n; q += nwarps) {
+        const uint32_t b = idx ? idx[q] : (uint32_t)q;
+        uint64_t r = ~0ull;   // a miss, and an index out of range
+        bool hit = false;
+        if (b < n64) hit = answer64<KIND>(S, c_cum, b_cum, high, b_beg[b], b_cnt[b], vals[q], lane, r);
+        else if (lane == 0) atomicMin(bad, (unsigned long long)q);   // no directory read
+        if (lane == 0) {
+            out[q] = r;
+            if (found) found[q] = hit;
+        }
+    }
+}
+
+// Values of every inner bitmap (bucket) from the inner set's c_cum, 0 for an empty one; nb + 1 entries,
+// the last zero, the input of the set's b_cum scan.
+__global__ void __launch_bounds__(256)
+k_query64_cards(const uint32_t *__restrict__ bm_beg, const uint32_t *__restrict__ bm_cnt,
+                const uint64_t *__restrict__ c_cum, uint64_t nb, uint64_t *__restrict__ out) {
+    const uint64_t stride = gridDim.x * (uint64_t)blockDim.x;
+    for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j <= nb; j += stride) {
+        const uint32_t cnt = j < nb ? bm_cnt[j] : 0u;
+        out[j] = cnt ? c_cum[bm_beg[j] + cnt] - c_cum[bm_beg[j]] : 0ull;   // (no c_cum without containers)
+    }
+}
+
 }  // namespace
 
 void launch_query(int kind, const SetView &S, const uint64_t *c_cum, uint32_t n_bitmaps, const uint32_t *idx,
@@ -222,6 +297,28 @@ void launch_query(int kind, const SetView &S, const uint64_t *c_cum, uint32_t n_
 
 void launch_query_cards(const uint32_t *c_card, uint64_t nc, uint64_t *out, cudaStream_t s) {
     launch_kernel(k_query_cards, grid_for(nc + 1, 256, 8), 256, 0, s, c_card, nc, out);
+}
+
+void launch_query64(int kind, const SetView &S, const uint64_t *c_cum, const uint64_t *b_cum, const uint32_t *b_beg,
+                    const uint32_t *b_cnt, const uint32_t *high, uint32_t n64, const uint32_t *idx,
+                    const uint64_t *vals, uint32_t n, uint64_t *out, uint8_t *found, unsigned long long *bad,
+                    cudaStream_t s) {
+    if (!n) return;
+    const dim3 grid = grid_for(n, 8, 6);   // a warp per query, 8 warps per block
+    const auto go = [&](auto kernel) {
+        launch_kernel(kernel, grid, 256, 0, s, S, c_cum, b_cum, b_beg, b_cnt, high, n64, idx, vals, n, out, found, bad);
+    };
+    switch (kind) {
+        case Q_CONTAINS: go(k_query64<Q_CONTAINS>); break;
+        case Q_RANK: go(k_query64<Q_RANK>); break;
+        case Q_GET_INDEX: go(k_query64<Q_GET_INDEX>); break;
+        default: go(k_query64<Q_SELECT>); break;
+    }
+}
+
+void launch_query64_cards(const uint32_t *bm_beg, const uint32_t *bm_cnt, const uint64_t *c_cum, uint64_t nb,
+                          uint64_t *out, cudaStream_t s) {
+    launch_kernel(k_query64_cards, grid_for(nb + 1, 256, 8), 256, 0, s, bm_beg, bm_cnt, c_cum, nb, out);
 }
 
 }  // namespace rb200

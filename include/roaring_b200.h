@@ -355,6 +355,27 @@ rb200_set64_t *rb200_set64_batch_remove_range_closed(const rb200_set64_t *S, con
                                                      const uint64_t *min, const uint64_t *max);
 /* mode 1 = roaring64_bitmap_run_optimize, mode 0 = remove the run containers (as rb200_set_run_optimize). */
 rb200_set64_t *rb200_set64_run_optimize(const rb200_set64_t *s, int mode);
+/* Point queries on 64-bit bitmaps, with the RB200_Q_* kinds and the selection rules of rb200_batch_query:
+ * query k asks bitmap S[idx[k]] about vals[k], k < n; idx == NULL: query k asks bitmap k
+ * (n = rb200_set64_count(S)).  out[k] is what the reference returns or writes through its out-pointer,
+ * found[k] its bool return:
+ *   RB200_Q_CONTAINS   1 / 0, found = out              as roaring64_bitmap_contains, src/roaring64.c:682
+ *   RB200_Q_RANK       the number of values <= vals[k], found = 1
+ *                                                       as roaring64_bitmap_rank, src/roaring64.c:804
+ *   RB200_Q_GET_INDEX  the index of vals[k]            as roaring64_bitmap_get_index, src/roaring64.c:827
+ *   RB200_Q_SELECT     the value of rank vals[k] (0-based)
+ *                                                       as roaring64_bitmap_select, src/roaring64.c:779
+ * A get_index or select miss writes out[k] = 2^64 - 1 and found[k] = 0.  found may be NULL, but it is the only
+ * way to tell a miss from a select whose answer is the value 2^64 - 1.  The first rank / get_index / select
+ * query of a set builds its cardinality prefixes on the device, which stay with the set.  vals / out may be
+ * NULL only when n == 0.  0 on success, -1 on error (rb200_last_error). */
+int rb200_set64_batch_query(int kind, const rb200_set64_t *S, const uint32_t *idx, size_t n, const uint64_t *vals,
+                            uint64_t *out, uint8_t *found);
+/* Same with idx / vals / out / found in device memory of the library's device (anything else is refused
+ * before the launch): read and written on the library stream, complete when the call returns.  The kernel
+ * checks every entry of d_idx; the call then fails with the host check's message. */
+int rb200_set64_batch_query_device(int kind, const rb200_set64_t *S, const uint32_t *d_idx, size_t n,
+                                   const uint64_t *d_vals, uint64_t *d_out, uint8_t *d_found);
 /* Device-side roaring64_bitmap_portable_serialize of every bitmap + one D2H: blob i = *buf + (*off)[i],
  * (*len)[i] bytes (blob starts 16-byte aligned); release all three with rb200_serialized_free. */
 int rb200_set64_serialize(const rb200_set64_t *s, char **buf, uint64_t **off, uint64_t **len);
